@@ -107,7 +107,7 @@ def load_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s)"
 
 
 def algorithmic_bytes_search(n_map: int, k: int = 5) -> int:
@@ -181,7 +181,7 @@ def cpu_update_loop(pr, n_scans: int, nthreads: int, warm: int = 3):
     tree.close()
     return {"times": times, "median_s": float(np.median(times)), "mean_s": float(np.mean(times)), "kind": kind, "threads": best,
             "calibration_ms": {str(c): round(1e3 * v, 2) for c, v in med.items()},
-            "median_s_3_threads": float(np.median(t3)), "x": result.x, "P": result.P}
+            "median_s_3_threads": float(np.median(t3)), "x": result.x, "P": result.P, "result": result}
 
 
 def rot_angle(qa, qb):
@@ -201,6 +201,19 @@ def state_parity(x, P, xo, Po):
             "against": "cpu_baseline leg's final state (reference ikd-Tree + restated update), same scan / prior"}
 
 
+def write_outputs(out_dir, x, P, near, cnt, selected=None):
+    """What the timed path hands its caller after its last step: the state, its covariance, and the scan's
+    Nearest_Points / point_selected_surf (the inputs of map_incremental).  About 3 MB at 30k points.  Both arms write
+    the same names, so the GPU and the CPU reference path can be compared output for output."""
+    out = {"x": np.asarray(x, np.float64), "P": np.asarray(P, np.float64), "nearest": np.asarray(near, np.float32),
+           "nearest_cnt": np.asarray(cnt, np.float32)}
+    if selected is not None:
+        out["selected"] = np.asarray(selected, np.float32)
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
 # ----------------------------------------------------------------------------- reference arm
 def run_reference(args, rank: int):
     if rank != 0:
@@ -211,6 +224,9 @@ def run_reference(args, rank: int):
     with c_stdout_to_stderr():
         c = cpu_update_loop(pr, args.steps, cores, warm=args.warmup)
     times = c["times"]
+    if args.dump_outputs:
+        r = c["result"]
+        write_outputs(args.dump_outputs, r.x, r.P, r.nearest, r.nearest_cnt, r.selected)
     val = 1.0 / c["median_s"]
     line = {
         "impl": "reference", "metric": METRIC, "value": val, "unit": UNIT, "n_gpus": args.gpus, "steps": len(times),
@@ -291,6 +307,10 @@ def run_ours(args, rank: int, world: int, local_rank: int):
     t_wall = time.perf_counter() - t_wall0
     launches = filt.gpu_launches() * args.steps
     x_res, P_res, n_pass = filt.download_state()
+    if args.dump_outputs and rank == 0:
+        near, cnt = filt.nearest(Q)
+        # under sharding point_selected_surf lives on each rank
+        write_outputs(args.dump_outputs, x_res, P_res, near, cnt, filt.selected(Q) if world == 1 else None)
     ms_warm = filt.time_resident(args.steps, flush_l2=False)
     # ---- dominant kernel alone
     ms_search = filt.time_search_pass(max(5, args.steps), flush_l2=True) / max(5, args.steps)
@@ -390,11 +410,12 @@ def main():
     ap.add_argument("--comm", default="p2p", choices=["p2p", "nccl"])
     ap.add_argument("--cpu-scans", type=int, default=20)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the timed path computed in its last step to DIR/<name>.npy")
     args = ap.parse_args()
     rank, world, local_rank = env_int("RANK", 0), env_int("WORLD_SIZE", 1), env_int("LOCAL_RANK", 0)
     # Pin the OpenMP threads of the CPU reference path (must be in the environment before any OpenMP runtime starts) -- ONLY in a
     # single-process run: under torchrun the binding would put the main thread of EVERY rank on the same core (place 0), and the
-    # ranks' host loops would time-share it (measured: 11 ms / 33 ms of wall clock per step at 4 / 8 ranks, device time unchanged).
+    # ranks' host loops would time-share it (wall clock per step grows with the rank count, device time unchanged).
     if args.impl != "reference" and world != args.gpus and world == 1 and args.gpus > 1:
         # convenience: re-launch under torchrun (before the binding below enters the environment the ranks would inherit)
         port = 29500 + (os.getpid() % 1000)

@@ -60,7 +60,7 @@ def load():
     if _lib is not None:
         return _lib
     if not os.path.exists(_build.LIB):
-        raise FastLioError(f"{_build.LIB} is missing -- run `python -m fast_lio_b200.build` (nvcc, sm_100a); "
+        raise FastLioError(f"{_build.LIB} is missing -- run `python -m fast_lio_b200.build` (nvcc, sm_90a); "
                            "there is no CPU fallback")
     L = C.CDLL(_build.LIB)
     L.fl_last_error.restype = C.c_char_p

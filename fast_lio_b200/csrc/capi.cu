@@ -226,7 +226,7 @@ int fl_filter_time_resident(fl_filter_t* f, int reps, int flush_l2, float* ms_to
     fl::Filter* F = f->impl;
     cudaStream_t st = F->stream();
     FL_CUDA(cudaSetDevice(F->map()->device()));
-    const size_t flush_bytes = 256u << 20;       // > 126 MB of L2
+    const size_t flush_bytes = 256u << 20;       // > 50 MB of H100 L2
     if (flush_l2) FL_CHECK(f->flush.reserve(flush_bytes));
     cudaEvent_t e0, e1;
     FL_CUDA(cudaEventCreate(&e0));

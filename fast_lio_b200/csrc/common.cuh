@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels of the FAST-LIO2 measurement-update path.
+// Shared helpers for the sm_90a kernels of the FAST-LIO2 measurement-update path.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -33,7 +33,7 @@ void set_last_error(const char* fmt, ...);
 // ----------------------------------------------------------------------------- constants
 constexpr int LEAF = 32;            // slots per leaf bucket == warp width (one coalesced 512 B load)
 constexpr int FAN = 32;             // children per internal node (one lane per child box)
-constexpr int MAX_LEVELS = 7;       // 32^7 leaves -- far beyond 180 GB of HBM
+constexpr int MAX_LEVELS = 7;       // 32^7 leaves -- far beyond 80 GB of HBM
 constexpr int KNN_K = 5;            // NUM_MATCH_POINTS, reference include/common_lib.h:26
 constexpr unsigned FULL = 0xffffffffu;
 

@@ -1,4 +1,4 @@
-// Host-side owner of the per-scan iterated-EKF measurement update on the device: the B200
+// Host-side owner of the per-scan iterated-EKF measurement update on the device: the H100
 // counterpart of esekfom::esekf<state_ikfom,12,input_ikfom>::update_iterated_dyn_share_modified
 // (reference include/IKFoM_toolkit/esekfom/esekfom.hpp:1619-1931) with h_share_model
 // (reference src/laserMapping.cpp:638-754) bound as a fused device measurement model.

@@ -1,5 +1,5 @@
 // Device point map: build / refit / search / box-delete / incremental insert.
-// B200-native replacement for the subset of KD_TREE<PointType> that FAST-LIO's
+// H100-native replacement for the subset of KD_TREE<PointType> that FAST-LIO's
 // laserMapping.cpp calls (reference include/ikd-Tree/ikd_Tree.cpp).  See map.cuh for the
 // memory layout and DESIGN.md for the rationale.
 #include <cub/device/device_radix_sort.cuh>
@@ -696,7 +696,7 @@ __global__ void __launch_bounds__(256) k_insert(MapView m, const float4* __restr
 }
 
 // ============================================================================= host
-static inline int blocks_for(long long threads, int block, int cap = 148 * 16) {
+static inline int blocks_for(long long threads, int block, int cap = 132 * 16) {      // 16 blocks on each of the H100 SXM's 132 SMs
     long long b = (threads + block - 1) / block;
     return (int)std::max<long long>(1, std::min<long long>(b, cap));
 }

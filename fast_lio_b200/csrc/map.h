@@ -1,4 +1,4 @@
-// Host-side owner of the device point map (the B200 counterpart of KD_TREE<PointType>,
+// Host-side owner of the device point map (the H100 counterpart of KD_TREE<PointType>,
 // reference include/ikd-Tree/ikd_Tree.h:48-341).  All methods return fl::Status.
 #pragma once
 #include <vector>

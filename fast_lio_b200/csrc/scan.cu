@@ -281,7 +281,7 @@ int ScanFrontEnd::voxel_downsample(float leaf, int* n_out) {
     VgCtl* ctl = ctl_.as<VgCtl>();
     const int block = 256, grid = (n + block - 1) / block;
     k_vg_reset<<<1, 32, 0, st>>>(ctl);
-    k_vg_minmax<<<std::min(grid, 148), block, 0, st>>>(raw_.as<float4>(), n, ctl);
+    k_vg_minmax<<<std::min(grid, 132), block, 0, st>>>(raw_.as<float4>(), n, ctl);
     k_vg_keys<<<grid, block, 0, st>>>(raw_.as<float4>(), n, leaf, ctl, keys_.as<unsigned>(), vals_.as<int>());
     size_t tmp_sort = 0, tmp_scan = 0;
     FL_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, keys_.as<unsigned>(), keys_alt_.as<unsigned>(), vals_.as<int>(), vals_alt_.as<int>(), n, 0, 32, st));

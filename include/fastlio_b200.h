@@ -1,4 +1,4 @@
-/* fastlio_b200.h -- C ABI of the B200-native FAST-LIO2 measurement-update path.
+/* fastlio_b200.h -- C ABI of the H100-native FAST-LIO2 measurement-update path.
  *
  * The reference (hku-mars/FAST_LIO) has no FFI layer: the hot path is reached through two
  * C++ class APIs used by src/laserMapping.cpp.  This header is the extern "C" boundary that

@@ -1,5 +1,5 @@
 // Drop-in facade: KD_TREE<PointType> with the call surface of the reference's
-// include/ikd-Tree/ikd_Tree.h (hku-mars/ikd-Tree @ e2e3f4e), served by the B200 device map
+// include/ikd-Tree/ikd_Tree.h (hku-mars/ikd-Tree @ e2e3f4e), served by the H100 device map
 // through the C ABI in fastlio_b200.h.  Put this directory in front of the reference's
 // include path and link libfastlio_b200.so; src/laserMapping.cpp compiles unchanged.
 //
@@ -68,7 +68,7 @@ public:
         if (dev < 0) { const char* e = getenv("FASTLIO_B200_DEVICE"); dev = e ? atoi(e) : 0; }
         device_ = dev;
         if (fl_map_create(&map_, dev, box_length) != FL_OK) {
-            fprintf(stderr, "KD_TREE(B200): cannot create the device map on CUDA device %d: %s\n", dev, fl_last_error());
+            fprintf(stderr, "KD_TREE(H100): cannot create the device map on CUDA device %d: %s\n", dev, fl_last_error());
             map_ = nullptr;
             failed_ = true;
         }
@@ -241,14 +241,14 @@ private:
         return p;
     }
     int check(int rc, const char* what) {
-        if (rc < 0) { failed_ = true; fprintf(stderr, "KD_TREE(B200)::%s failed: %s\n", what, fl_last_error()); }
+        if (rc < 0) { failed_ = true; fprintf(stderr, "KD_TREE(H100)::%s failed: %s\n", what, fl_last_error()); }
         return rc;
     }
     bool check_k(int k) {
         if (k >= 1 && k <= 5) return true;
         failed_ = true;
         static bool told = false;
-        if (!told) { told = true; fprintf(stderr, "KD_TREE(B200)::Nearest_Search: k_nearest = %d is not supported (1 <= k <= 5, NUM_MATCH_POINTS)\n", k); }
+        if (!told) { told = true; fprintf(stderr, "KD_TREE(H100)::Nearest_Search: k_nearest = %d is not supported (1 <= k <= 5, NUM_MATCH_POINTS)\n", k); }
         return false;
     }
     static int& default_device() { static int d = -1; return d; }

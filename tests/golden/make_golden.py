@@ -3,9 +3,12 @@
 The reference ships no fixtures (SURVEY.md section 4), so the goldens are produced here from
 (a) the reference's own unmodified ikd-Tree compiled into oracle/_ref -- kNN results -- and
 (b) the CPU restatement in oracle/fastlio_oracle.cpp -- per-pass normal equations and final state.
-Run from the repository root in the build container (needs /root/reference for oracle/_ref):
+Run from the repository root with the original project's sources present (oracle/_ref is built from them):
 
     python tests/golden/make_golden.py
+
+The reference answers of tests/golden/ref/ (see tests/refcalls.py) are written by running the suite on a GPU with
+oracle/_ref built and FASTLIO_RECORD_REF=<dir>, then copying <dir>/*.npz here.
 """
 import os
 import sys

@@ -1,4 +1,4 @@
-"""CPU: the bench.py output contract -- the committed B200 lines under profiles/ carry every key the driver reads, and the
+"""CPU: the bench.py output contract -- the committed H100 lines under profiles/ carry every key a reader needs, and the
 reference arm (which needs no GPU) prints exactly one JSON line with its own required keys."""
 import glob
 import json
@@ -18,7 +18,7 @@ def _baseline():
         return json.load(f)
 
 
-@pytest.mark.parametrize("path", sorted(glob.glob(os.path.join(ROOT, "profiles", "r[12]_bench_n*.json"))))
+@pytest.mark.parametrize("path", sorted(glob.glob(os.path.join(ROOT, "profiles", "h100_bench_n*.json"))))
 def test_committed_bench_lines_follow_the_contract(path):
     with open(path) as f:
         lines = [l for l in f.read().splitlines() if l.strip()]

@@ -4,7 +4,7 @@ import numpy as np
 import pytest
 
 from fast_lio_b200 import synth
-from oracle import bind
+from refcalls import RefTree, digest
 from cell_directory_model import CellDirectoryModel
 from test_oracle_golden import world_queries
 
@@ -35,12 +35,11 @@ def test_rings_give_the_exact_knn(problems, cell):
 def test_model_matches_reference_ikdtree(problems):
     pr = problems("tiny")
     m = CellDirectoryModel(pr.map_pts, 1.0)
-    t = bind.KdTree(pr.map_pts, "auto")
+    t = RefTree("cell_directory_model", pr.map_pts)
     q = world_queries(pr)[:200]
     _, d_ref, cnt = t.knn(q, 5)
-    for i, qq in enumerate(q):
-        _, d2, _, _ = m.knn(qq)
-        assert cnt[i] == 5 and np.array_equal(d2, d_ref[i])
+    d_model = np.stack([m.knn(qq)[1] for qq in q]).astype(np.float32)
+    assert (cnt == 5).all() and digest(d_model) == d_ref
 
 
 def test_sparse_and_degenerate_maps():

@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 
 from fast_lio_b200 import api, build, synth
-from oracle import bind
+from refcalls import RefTree
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -61,7 +61,7 @@ def test_cpp_facades_run_on_the_gpu(problems, tmp_path, name):
     assert len(t.acquire_removed_points()) == n_removed == del_ret
     assert (t.size(), t.validnum()) == (size, validnum)
     # ---- and the CPU oracle (north-star tolerance)
-    o = bind.update_iterated(bind.KdTree(pr.map_pts, "auto"), pr.scan, pr.x_prior, pr.P_prior, pr.cfg.max_iter, pr.R, pr.limit, 0)
+    o = RefTree(f"update_{name}_e0", pr.map_pts).update_iterated(pr.scan, pr.x_prior, pr.P_prior, pr.cfg.max_iter, pr.R, pr.limit, 0)
     assert np.abs(x[:3] - o.x[:3]).max() <= 1e-4 and np.abs(x[3:7] - o.x[3:7]).max() <= 1e-4
     assert np.abs(x[11:] - o.x[11:]).max() <= 1e-4
 

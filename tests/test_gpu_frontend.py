@@ -5,6 +5,7 @@ import pytest
 
 from fast_lio_b200 import api, synth
 from oracle import bind
+from refcalls import RefTree
 
 pytestmark = pytest.mark.gpu
 
@@ -111,8 +112,7 @@ def test_resident_chain_matches_host_chain(problems, tree, raw):
     o_pts, _ = bind.undistort(raw.xyzi, raw.offset_ms, raw.imu_pose, raw.x_end)
     o_down = bind.voxelgrid(o_pts, 0.5)
     assert len(o_down) == n
-    ot = bind.KdTree(pr.map_pts, "auto")
-    r = bind.update_iterated(ot, o_down, pr.x_prior, pr.P_prior, 3, pr.R)
+    r = RefTree("resident_chain", pr.map_pts).update_iterated(o_down, pr.x_prior, pr.P_prior, 3, pr.R)
     assert np.abs(x_dev[:3] - r.x[:3]).max() < 1e-4                   # north-star tolerance: 1e-4 m / 1e-4 rad
     assert np.abs(x_dev[3:7] - r.x[3:7]).max() < 1e-4
     assert np.abs(x_dev - r.x).max() < 1e-4
@@ -126,7 +126,7 @@ def test_localmap_segment_deletes_from_the_map(problems):
     g = api.KdTree(0, 0.5); g.Build(pr.map_pts)
     ours = api.LocalMap(40.0, 8.0)
     ref = bind.LocalMap(40.0, 8.0)
-    rt = bind.KdTree(pr.map_pts, "auto") if bind.have_ref() else None
+    rt = RefTree("localmap_segment", pr.map_pts)
     pos = np.array(pr.x_true[:3], dtype=np.float64)
     total = 0
     for k in range(12):
@@ -134,7 +134,7 @@ def test_localmap_segment_deletes_from_the_map(problems):
         boxes, n_deleted = ours.segment(pos, g)
         b_ref = ref.segment(pos)
         assert np.array_equal(boxes, b_ref)
-        if rt is not None and len(b_ref):
+        if len(b_ref):
             assert n_deleted == rt.delete_boxes(b_ref)
             assert g.validnum() == rt.validnum()
         total += n_deleted

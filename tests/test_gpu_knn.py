@@ -3,7 +3,7 @@ import numpy as np
 import pytest
 
 from fast_lio_b200 import api, synth
-from oracle import bind
+from refcalls import RefTree, digest, row_digests
 
 pytestmark = pytest.mark.gpu
 
@@ -24,19 +24,18 @@ def _world_queries(pr):
 def test_knn_matches_reference_ikdtree(problems, name):
     pr = problems(name)
     q = _world_queries(pr)
-    ref = bind.KdTree(pr.map_pts, "auto")
-    rp, rd, rc = ref.knn(q, 5)
+    ref = RefTree(f"knn_{name}", pr.map_pts)
+    rp, rd, rc = ref.knn(q, 5, neighbours="rows")
     t = api.KdTree(0, 0.5)
     t.Build(pr.map_pts)
     assert t.validnum() == len(pr.map_pts)
     gp, gd, gc = t.Nearest_Search(q, 5)
     assert np.array_equal(gc, rc)
     # bit-exact squared distances (float32, same operation order as ikd_Tree.cpp:1683-1688)
-    assert np.array_equal(gd, rd)
+    assert digest(gd) == rd
     # identical neighbour coordinates and payload wherever distances are not tied
-    tie = np.zeros(len(q), dtype=bool)
-    tie[:] = (np.diff(rd, axis=1) == 0).any(axis=1)
-    assert np.array_equal(gp[~tie], rp[~tie])
+    tie = (np.diff(gd, axis=1) == 0).any(axis=1)
+    assert np.array_equal(row_digests(gp)[~tie], rp[~tie])
 
 
 def _brute_d2(q, pts):
@@ -71,8 +70,8 @@ def test_knn_gridded_map_ties():
     q = np.zeros((600, 4), dtype=np.float32)
     q[:, :3] = np.round(rng.uniform(-5, 5, (600, 3)) * 8) / 8          # multiples of 0.125: plenty of equidistant neighbours
     q[:300, 0] += rng.uniform(-0.05, 0.05, 300).astype(np.float32)
-    ref = bind.KdTree(pts, "reference" if bind.have_ref() else "port")
-    rp, rd, rc = ref.knn(q, 5)
+    ref = RefTree("knn_gridded_map_ties", pts)
+    rp, rd, rc = ref.knn(q, 5, neighbours="points")
     t = api.KdTree(0, 0.5); t.Build(pts)
     gp, gd, gc = t.Nearest_Search(q, 5)
     assert np.array_equal(gc, rc) and np.array_equal(gd, rd)
@@ -99,8 +98,8 @@ def test_knn_planted_ties_are_ordered_by_x():
     pts = np.zeros((len(ps), 4), dtype=np.float32); pts[:, :3] = np.array(ps, dtype=np.float32); pts[:, 3] = np.arange(len(ps))
     pts = pts[rng.permutation(len(pts))]
     q = np.zeros((len(qs), 4), dtype=np.float32); q[:, :3] = np.array(qs, dtype=np.float32)
-    ref = bind.KdTree(pts, "reference" if bind.have_ref() else "port")
-    rp, rd, rc = ref.knn(q, 5)
+    ref = RefTree("knn_planted_ties", pts)
+    rp, rd, rc = ref.knn(q, 5, neighbours="points")
     decided, inner_tie = _decided_rows(q, pts, rp, rd)
     assert inner_tie.sum() >= 100                                       # the x rule is exercised
     t = api.KdTree(0, 0.5); t.Build(pts)

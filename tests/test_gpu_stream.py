@@ -4,15 +4,13 @@ import numpy as np
 import pytest
 
 from fast_lio_b200 import api, synth
-from oracle import bind
-from semantics import map_incremental, sort_rows
+from refcalls import RefTree, digest, rows_digest
+from semantics import map_incremental
 
 pytestmark = pytest.mark.gpu
 
 
 def test_map_incremental_matches_reference(problems):
-    if not bind.have_ref():
-        pytest.skip("oracle/_ref not available")
     pr = problems("small")
     g = api.KdTree(0, 0.5); g.Build(pr.map_pts)
     f = api.Esekf(g, max_points=len(pr.scan), max_iter=pr.cfg.max_iter)
@@ -20,24 +18,22 @@ def test_map_incremental_matches_reference(problems):
     near, cnt = f.nearest(len(pr.scan))
     n_add, n_no, added = f.map_incremental(0.5, True)
     # CPU reference pipeline from the same update result
-    r = bind.KdTree(pr.map_pts, "reference", downsample=0.5)
+    r = RefTree("map_incremental", pr.map_pts)
     to_add, no_need = map_incremental(pr.scan, x, near, cnt, 0.5, True)
     assert (n_add, n_no) == (len(to_add), len(no_need))
     assert added == r.add(to_add, True)
     r.add(no_need, False)
     assert g.validnum() == r.validnum()
-    assert np.array_equal(sort_rows(g.flatten()), sort_rows(r.flatten()))
+    assert rows_digest(g.flatten()) == r.flatten_digest()
 
 
 def test_stream_of_scans(problems):
     """5 scans: the sensor advances 0.1 m per scan; state and map of the device pipeline track the CPU pipeline."""
-    if not bind.have_ref():
-        pytest.skip("oracle/_ref not available")
     pr = problems("small")
     scene = pr.scene
     g = api.KdTree(0, 0.5); g.Build(pr.map_pts)
     f = api.Esekf(g, max_points=2000, max_iter=3)
-    r = bind.KdTree(pr.map_pts, "reference", downsample=0.5)
+    r = RefTree("stream_of_scans_pipeline", pr.map_pts)
     x_g = pr.x_prior.copy(); x_c = pr.x_prior.copy()
     P_g = pr.P_prior.copy(); P_c = pr.P_prior.copy()
     for step in range(5):
@@ -49,14 +45,16 @@ def test_stream_of_scans(problems):
         # crude prediction: carry the state over, inflate the covariance
         P_g = P_g + np.eye(23) * 1e-4; P_c = P_c + np.eye(23) * 1e-4
         x_g, P_g, _ = f.update_iterated_dyn_share_modified(scan, x_g, P_g, pr.R)
-        o = bind.update_iterated(r, scan, x_c, P_c, 3, pr.R, pr.limit, 0)
+        o = r.update_iterated(scan, x_c, P_c, 3, pr.R, pr.limit, 0)
         x_c, P_c = o.x, o.P
         assert np.abs(x_g[:3] - x_c[:3]).max() <= 1e-4 and np.abs(x_g[3:7] - x_c[3:7]).max() <= 1e-4
+        near, cnt = f.nearest(len(scan))
+        assert digest(cnt) == o.nearest_cnt_digest and digest(near) == o.nearest_digest     # the reference's Nearest_Points
         n_add, n_no, added = f.map_incremental(0.5, True)
-        to_add, no_need = map_incremental(scan, x_c, o.nearest, o.nearest_cnt, 0.5, True)
+        to_add, no_need = map_incremental(scan, x_c, near, cnt, 0.5, True)
         assert (n_add, n_no) == (len(to_add), len(no_need))
         assert added == r.add(to_add, True)
         r.add(no_need, False)
         assert g.validnum() == r.validnum()
-    assert np.array_equal(sort_rows(g.flatten()), sort_rows(r.flatten()))
+    assert rows_digest(g.flatten()) == r.flatten_digest()
     assert np.abs(x_g[:3] - synth.true_state(pr.cfg.lidar, 4)[:3]).max() < 0.02

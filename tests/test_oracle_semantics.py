@@ -1,24 +1,20 @@
 """CPU: pin the oracle pieces against each other and against the reference's own ikd-Tree."""
 import numpy as np
-import pytest
 
-from fast_lio_b200 import synth
 from oracle import bind
-from semantics import VoxelMapModel, sort_rows
+from refcalls import RefTree, digest, rows_digest
+from semantics import VoxelMapModel
 
-needs_ref = pytest.mark.skipif(not bind.have_ref(), reason="oracle/_ref (reference ikd-Tree) not built")
 
-
-@needs_ref
 def test_port_knn_equals_reference_ikdtree(problems):
     pr = problems("small")
     q = pr.map_pts[::7].copy()
     q[:, :3] += 0.21
-    a = bind.KdTree(pr.map_pts, "reference")
+    a = RefTree("port_knn", pr.map_pts)
     b = bind.KdTree(pr.map_pts, "port")
     pa, da, ca = a.knn(q)
     pb, db, cb = b.knn(q)
-    assert np.array_equal(ca, cb) and np.array_equal(da, db) and np.array_equal(pa, pb)
+    assert np.array_equal(ca, cb) and da == digest(db) and pa == digest(pb)
 
 
 def test_knn_port_brute_force():
@@ -32,19 +28,18 @@ def test_knn_port_brute_force():
         assert np.array_equal(d[i], np.sort(dd)[:5])
 
 
-@needs_ref
 def test_mutation_model_equals_reference_ikdtree():
     rng = np.random.default_rng(4)
     pts = rng.uniform(-4, 4, (2500, 4)).astype(np.float32)
-    r = bind.KdTree(pts, "reference", downsample=0.5)
+    r = RefTree("mutation_model", pts)
     m = VoxelMapModel(pts, 0.5)
     for rep in range(3):
         batch = rng.uniform(-5, 5, (700, 4)).astype(np.float32)
         assert r.add(batch, True) == m.add_points(batch, True)
-        assert np.array_equal(sort_rows(r.flatten()), sort_rows(m.flatten()))
+        assert r.flatten_digest() == rows_digest(m.flatten())
         box = np.array([[-1.0 + rep, -2, -2, 0.5 + rep, 2, 2]], dtype=np.float32)
         assert r.delete_boxes(box) == m.delete_boxes(box)
-        assert np.array_equal(sort_rows(r.flatten()), sort_rows(m.flatten()))
+        assert r.flatten_digest() == rows_digest(m.flatten())
         extra = rng.uniform(-5, 5, (100, 4)).astype(np.float32)
         assert r.add(extra, False) == m.add_points(extra, False) == 0
     assert r.validnum() == len(m.flatten())
