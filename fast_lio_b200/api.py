@@ -39,7 +39,7 @@ SYMBOLS = [
     "fl_last_error", "fl_device_count", "fl_version", "fl_host_register", "fl_host_unregister", "fl_filter_debug_prof",
     "fl_map_create", "fl_map_destroy", "fl_map_set_downsample", "fl_map_build", "fl_map_size", "fl_map_validnum",
     "fl_map_knn", "fl_map_add_points", "fl_map_delete_boxes", "fl_map_flatten", "fl_map_tree_range",
-    "fl_map_rebuild", "fl_map_stats", "fl_map_add_boxes", "fl_map_acquire_removed", "fl_map_set_cell_directory", "fl_map_dir_stats",
+    "fl_map_rebuild", "fl_map_stats", "fl_map_add_boxes", "fl_map_box_search", "fl_map_radius_search", "fl_map_acquire_removed", "fl_map_set_cell_directory", "fl_map_dir_stats",
     "fl_filter_create", "fl_filter_destroy", "fl_filter_set_params", "fl_filter_set_solver", "fl_filter_set_search", "fl_filter_set_fused", "fl_filter_update",
     "fl_filter_map_incremental", "fl_filter_get_nearest", "fl_filter_get_selected", "fl_filter_get_pass_logs", "fl_filter_upload_scan",
     "fl_filter_upload_state", "fl_filter_run", "fl_filter_download_state", "fl_filter_sync",
@@ -76,6 +76,8 @@ def load():
     L.fl_map_add_points.argtypes = [C.c_void_p, _f32p, C.c_int, C.c_int]
     L.fl_map_delete_boxes.argtypes = [C.c_void_p, _f32p, C.c_int]
     L.fl_map_flatten.argtypes = [C.c_void_p, _f32p, C.c_int]
+    L.fl_map_box_search.argtypes = [C.c_void_p, _f32p, C.c_int, _i32p, _f32p, C.c_int]
+    L.fl_map_radius_search.argtypes = [C.c_void_p, _f32p, C.c_int, _i32p, _f32p, C.c_int]
     L.fl_map_add_boxes.argtypes = [C.c_void_p, _f32p, C.c_int]
     L.fl_map_acquire_removed.argtypes = [C.c_void_p, _f32p, C.c_int]
     L.fl_map_tree_range.argtypes = [C.c_void_p, _f32p]
@@ -207,6 +209,38 @@ class KdTree:
         out = np.zeros((max(n, 1), 4), dtype=np.float32)
         got = _check(self._L.fl_map_flatten(self.h, out, len(out)))
         return out[:got].copy()
+
+    # KD_TREE::Box_Search, batched
+    def Box_Search(self, boxes6, cap: int | None = None):
+        """boxes6: (nb, 6) = (min xyz, max xyz); a point is found when min <= p < max on every axis.  Returns (offsets, points):
+        the points of box i are points[offsets[i]:offsets[i + 1]], rows (x, y, z, intensity)."""
+        boxes6 = np.ascontiguousarray(boxes6, dtype=np.float32).reshape(-1, 6)
+        return self._range(self._L.fl_map_box_search, boxes6, cap)
+
+    # KD_TREE::Radius_Search, batched
+    def Radius_Search(self, centers_xyz, radius, cap: int | None = None):
+        """centers_xyz: (nq, 3) (or (nq, 4): the fourth column is ignored); radius: a scalar or one per centre.  A point is found
+        when its float32 squared distance is <= radius * radius rounded to float32.  Returns (offsets, points) like Box_Search."""
+        c = np.asarray(centers_xyz, dtype=np.float32)
+        c = c.reshape(-1, c.shape[-1])[:, :3]
+        q = np.empty((len(c), 4), dtype=np.float32)
+        q[:, :3] = c
+        q[:, 3] = np.broadcast_to(np.asarray(radius, dtype=np.float32), (len(c),))
+        return self._range(self._L.fl_map_radius_search, q, cap)
+
+    def _range(self, fn, q, cap):
+        """One call with room for `cap` points (default: the map size or the last total, whichever is larger); a second one
+        when the total turns out to be larger."""
+        offsets = np.zeros(len(q) + 1, dtype=np.int32)
+        if cap is None:
+            cap = max(self.validnum(), getattr(self, "_range_hint", 0), 1024)
+        out = np.empty((max(cap, 1), 4), dtype=np.float32)
+        total = _check(fn(self.h, q, len(q), offsets, out, cap))
+        if total > cap:
+            out = np.empty((total, 4), dtype=np.float32)
+            total = _check(fn(self.h, q, len(q), offsets, out, total))
+        self._range_hint = total
+        return offsets, out[:total]
 
     def tree_range(self) -> np.ndarray:
         box = np.zeros(6, dtype=np.float32)

@@ -130,6 +130,18 @@ int fl_map_flatten(fl_map_t* m, float* out, int cap) {
     int rc = m->impl->flatten(out, cap, &n);
     return rc == FL_OK ? n : rc;
 }
+int fl_map_box_search(fl_map_t* m, const float* boxes6, int nb, int* out_offsets, float* out_xyzi, int cap) {
+    MAP_GUARD(m);
+    long long total = 0;
+    int rc = m->impl->range_search(false, boxes6, nb, out_offsets, out_xyzi, cap, &total);
+    return rc == FL_OK ? (int)total : rc;
+}
+int fl_map_radius_search(fl_map_t* m, const float* centers_xyzr, int nq, int* out_offsets, float* out_xyzi, int cap) {
+    MAP_GUARD(m);
+    long long total = 0;
+    int rc = m->impl->range_search(true, centers_xyzr, nq, out_offsets, out_xyzi, cap, &total);
+    return rc == FL_OK ? (int)total : rc;
+}
 int fl_map_tree_range(fl_map_t* m, float* box6) { MAP_GUARD(m); if (!box6) return FL_ERR_ARG; return m->impl->tree_range(box6); }
 int fl_map_rebuild(fl_map_t* m) { MAP_GUARD(m); return m->impl->rebuild(); }
 int fl_map_stats(fl_map_t* m, int* out4) {

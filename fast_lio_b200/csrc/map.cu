@@ -3,6 +3,7 @@
 // laserMapping.cpp calls (reference include/ikd-Tree/ikd_Tree.cpp).  See map.cuh for the
 // memory layout and DESIGN.md for the rationale.
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 
 #include <algorithm>
 #include <cstdarg>
@@ -695,6 +696,123 @@ __global__ void __launch_bounds__(256) k_insert(MapView m, const float4* __restr
     }
 }
 
+// ----------------------------------------------------------------------------- Box_Search / Radius_Search
+// A query is a box (min xyz, max xyz) or a sphere (x, y, z, r).  One warp per query would stall on a single whole-map box, so
+// the work is spread over (query, main leaf) pairs: k_range_leaves lists, per query, the main leaves whose AABB can hold an
+// answer, then one warp per pair decides membership slot by slot with the exact rule (k_range_count, k_range_fill).  The
+// pruning may widen the searched set, never narrow it.
+struct RangeQuery {
+    float bmin[3], bmax[3];      // pruning box: the query box itself, or the sphere's AABB padded outward
+    float c[3], r2, r2_pad;      // sphere: centre, fl(r * r) (the rule of Search_by_radius, ikd_Tree.cpp:1308) and a padded bound
+    bool valid;                  // false: NaN input, negative radius or an empty box -- no answer
+};
+template <bool RADIUS>
+__device__ __forceinline__ RangeQuery range_query(const float* __restrict__ q, int i) {
+    RangeQuery Q;
+    if constexpr (RADIUS) {
+        const float4 s = __ldg(reinterpret_cast<const float4*>(q) + i);
+        Q.c[0] = s.x; Q.c[1] = s.y; Q.c[2] = s.z;
+        Q.valid = !isnan(s.x) && !isnan(s.y) && !isnan(s.z) && s.w >= 0.f;       // NaN radius fails the comparison
+        Q.r2 = __fmul_rn(s.w, s.w);
+        Q.r2_pad = __fmul_rn(Q.r2, 1.0001f);
+        // every point with sq_dist3 <= r2 lies within r (1 + a few ulps) of the centre on each axis; the pad is far wider
+        const float pad = __fadd_rn(__fadd_rn(__fmul_rn(s.w, 1.0001f), 1e-6f * fmaxf(fmaxf(fabsf(s.x), fabsf(s.y)), fabsf(s.z))), 1e-30f);
+#pragma unroll
+        for (int a = 0; a < 3; a++) { Q.bmin[a] = __fsub_rn(Q.c[a], pad); Q.bmax[a] = __fadd_rn(Q.c[a], pad); }
+    } else {
+        bool ok = true;
+#pragma unroll
+        for (int a = 0; a < 3; a++) {
+            Q.bmin[a] = __ldg(&q[6 * (size_t)i + a]);
+            Q.bmax[a] = __ldg(&q[6 * (size_t)i + 3 + a]);
+            ok &= Q.bmin[a] < Q.bmax[a];                     // false for NaN and for an inverted or empty box
+        }
+        Q.valid = ok;
+        Q.c[0] = Q.c[1] = Q.c[2] = Q.r2 = Q.r2_pad = 0.f;
+    }
+    return Q;
+}
+// the per-point rule: Search_by_range's half-open box (ikd_Tree.cpp:1263), or Search_by_radius's calc_dist(p, q) <= r * r (:1308)
+template <bool RADIUS>
+__device__ __forceinline__ bool range_hit(const float4& p, const RangeQuery& Q) {
+    if (!slot_valid(p)) return false;
+    if constexpr (RADIUS) return sq_dist3(Q.c[0], Q.c[1], Q.c[2], p.x, p.y, p.z) <= Q.r2;
+    else return in_box(p, Q.bmin, Q.bmax);
+}
+
+template <bool RADIUS>
+struct RangeLeaves {             // box_query functor: counts (out == nullptr) or lists the candidate leaves of query q
+    const MapView& m; const RangeQuery& Q; int2* out; int q; int lane; int n = 0;
+    __device__ RangeLeaves(const MapView& m_, const RangeQuery& Q_, int2* out_, int q_, int lane_) : m(m_), Q(Q_), out(out_), q(q_), lane(lane_) {}
+    __device__ __forceinline__ void leaf(int l) {
+        if constexpr (RADIUS) {
+            // box_dist3 <= sq_dist3 of every point in the box (both are monotone in the exact distances), so this drop is exact
+            const float4 lo = __ldg(&m.ebox[0][2 * l]), hi = __ldg(&m.ebox[0][2 * l + 1]);
+            if (box_dist3(Q.c[0], Q.c[1], Q.c[2], lo.x, lo.y, lo.z, hi.x, hi.y, hi.z) > Q.r2_pad) return;
+        }
+        if (out && lane == 0) out[n] = make_int2(q, l);
+        n++;
+    }
+};
+// One warp per query.  Count pass (pairs == nullptr): cnt[i] = candidate leaves.  Fill pass: the (query, leaf) pairs at
+// off[i], in ascending leaf order (box_query visits children in lane order).
+template <bool RADIUS>
+__global__ void __launch_bounds__(256) k_range_leaves(MapView m, const float* __restrict__ q, int nq, long long* __restrict__ cnt,
+                                                      const long long* __restrict__ off, int2* __restrict__ pairs) {
+    const int lane = threadIdx.x & 31;
+    const int warps = (gridDim.x * blockDim.x) >> 5;
+    for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < nq; i += warps) {
+        const RangeQuery Q = range_query<RADIUS>(q, i);
+        if (!Q.valid) { if (lane == 0 && !pairs) cnt[i] = 0; continue; }
+        RangeLeaves<RADIUS> f(m, Q, pairs ? pairs + off[i] : nullptr, i, lane);
+        box_query(m, Q.bmin, Q.bmax, f, lane);
+        if (lane == 0 && !pairs) cnt[i] = f.n;
+    }
+}
+// One warp per (query, leaf) pair: the leaf and its overflow chain, one slot per lane.  Count pass (out == nullptr): cnt[w] =
+// points found.  Fill pass: (x, y, z, intensity) of each at off[w] + the prefix popcount, the first `cap` of all only.
+template <bool RADIUS>
+__device__ __forceinline__ void range_points(const MapView& m, const float* __restrict__ q, const int2* __restrict__ pairs, long long npairs,
+                                             long long* __restrict__ cnt, const long long* __restrict__ off, float4* __restrict__ out, long long cap) {
+    const int lane = threadIdx.x & 31;
+    const long long warps = ((long long)gridDim.x * blockDim.x) >> 5;
+    for (long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < npairs; w += warps) {
+        const long long base = out ? off[w] : 0;
+        if (out && base >= cap) continue;
+        const int2 pr = pairs[w];
+        const RangeQuery Q = range_query<RADIUS>(q, pr.x);
+        int leaf = pr.y, n = 0;
+        while (leaf >= 0) {
+            const float4 p = __ldg(&m.pts[leaf * LEAF + lane]);
+            const int nxt = __ldg(&m.next[leaf]);
+            const bool hit = range_hit<RADIUS>(p, Q);
+            const unsigned mask = __ballot_sync(FULL, hit);
+            if (out && hit) {
+                const long long at = base + n + __popc(mask & ((1u << lane) - 1));
+                if (at < cap) out[at] = make_float4(p.x, p.y, p.z, __ldg(&m.payload[leaf * LEAF + lane]));
+            }
+            n += __popc(mask);
+            leaf = nxt;
+        }
+        if (!out && lane == 0) cnt[w] = n;
+    }
+}
+template <bool RADIUS>
+__global__ void __launch_bounds__(256) k_range_count(MapView m, const float* __restrict__ q, const int2* __restrict__ pairs, long long npairs,
+                                                     long long* __restrict__ cnt) {
+    range_points<RADIUS>(m, q, pairs, npairs, cnt, nullptr, nullptr, 0);
+}
+template <bool RADIUS>
+__global__ void __launch_bounds__(256) k_range_fill(MapView m, const float* __restrict__ q, const int2* __restrict__ pairs, long long npairs,
+                                                    const long long* __restrict__ off, float4* __restrict__ out, long long cap) {
+    range_points<RADIUS>(m, q, pairs, npairs, nullptr, off, out, cap);
+}
+// CSR offsets of the queries: the points before query i's first pair
+__global__ void k_range_offsets(const long long* __restrict__ leaf_off, const long long* __restrict__ point_off, int nq, int* __restrict__ offsets) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i <= nq) offsets[i] = (int)point_off[leaf_off[i]];
+}
+
 // ============================================================================= host
 static inline int blocks_for(long long threads, int block, int cap = 132 * 16) {      // 16 blocks on each of the H100 SXM's 132 SMs
     long long b = (threads + block - 1) / block;
@@ -710,6 +828,7 @@ Map::~Map() {
     segid_.release(); segtab_[0].release(); segtab_[1].release(); bbox_.release();
     src_.release(); keys_in_.release(); keys_out_.release(); vals_in_.release(); vals_out_.release();
     cub_tmp_.release(); scratch_.release(); scratch2_.release(); scratch3_.release();
+    rs_q_.release(); rs_lcnt_.release(); rs_loff_.release(); rs_pairs_.release(); rs_pcnt_.release(); rs_poff_.release(); rs_out_.release(); rs_offsets_.release();
     if (h_counters_) cudaFreeHost(h_counters_);
     if (stream_) cudaStreamDestroy(stream_);
 }
@@ -717,6 +836,7 @@ Map::~Map() {
 int Map::init() {
     FL_CUDA(cudaSetDevice(device_));
     FL_CUDA(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
+    FL_CUDA(cudaDeviceGetAttribute(&n_sm_, cudaDevAttrMultiProcessorCount, device_));
     FL_CHECK(counters_.reserve(sizeof(int) * C_COUNT));
     FL_CUDA(cudaMemsetAsync(counters_.ptr, 0, sizeof(int) * C_COUNT, stream_));
     FL_CUDA(cudaMallocHost(&h_counters_, sizeof(int) * C_COUNT));
@@ -1017,6 +1137,102 @@ int Map::flatten(float* out_xyzi, int cap, int* n_out) {
         FL_CUDA(cudaMemcpyAsync(out_xyzi, src_.ptr, sizeof(float4) * (size_t)std::min(n, cap), cudaMemcpyDeviceToHost, stream_));
         FL_CUDA(cudaStreamSynchronize(stream_));
     }
+    return FL_OK;
+}
+
+// Blocks for a grid-stride kernel over `threads` threads: no more than the device keeps resident at once.
+template <class K>
+static int resident_blocks(K kernel, int block, long long threads, int n_sm) {
+    int per_sm = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, 0) != cudaSuccess || per_sm < 1) { cudaGetLastError(); per_sm = 1; }
+    const long long want = (threads + block - 1) / block;
+    return (int)std::max<long long>(1, std::min<long long>(want, (long long)std::max(n_sm, 1) * per_sm));
+}
+
+// out[0 .. n] = exclusive prefix sum of in[0 .. n - 1]; in[n] must be 0 (out[n] is the total)
+static int exclusive_sum(DeviceBuffer& tmp, long long* in, long long* out, long long n, cudaStream_t st) {
+    size_t bytes = 0;
+    FL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, in, out, n + 1, st));
+    FL_CHECK(tmp.reserve(bytes));
+    bytes = tmp.bytes;
+    FL_CUDA(cub::DeviceScan::ExclusiveSum(tmp.ptr, bytes, in, out, n + 1, st));
+    return FL_OK;
+}
+
+template <bool RADIUS>
+static int launch_range_leaves(const MapView& v, const float* q, int nq, long long* cnt, const long long* off, int2* pairs, int n_sm, cudaStream_t st) {
+    k_range_leaves<RADIUS><<<resident_blocks(k_range_leaves<RADIUS>, 256, (long long)nq * 32, n_sm), 256, 0, st>>>(v, q, nq, cnt, off, pairs);
+    FL_CUDA(cudaGetLastError());
+    return FL_OK;
+}
+template <bool RADIUS>
+static int launch_range_points(const MapView& v, const float* q, const int2* pairs, long long npairs, long long* cnt, const long long* off,
+                               float4* out, long long cap, int n_sm, cudaStream_t st) {
+    if (!out) k_range_count<RADIUS><<<resident_blocks(k_range_count<RADIUS>, 256, npairs * 32, n_sm), 256, 0, st>>>(v, q, pairs, npairs, cnt);
+    else k_range_fill<RADIUS><<<resident_blocks(k_range_fill<RADIUS>, 256, npairs * 32, n_sm), 256, 0, st>>>(v, q, pairs, npairs, off, out, cap);
+    FL_CUDA(cudaGetLastError());
+    return FL_OK;
+}
+
+int Map::range_search(bool radius, const float* queries, int nq, int* out_offsets, float* out_xyzi, int cap, long long* total) {
+    if (total) *total = 0;
+    const char* what = radius ? "radius_search" : "box_search";
+    if (nq < 0 || cap < 0 || !out_offsets || (nq > 0 && !queries) || (cap > 0 && !out_xyzi)) {
+        set_last_error("%s: bad arguments (null buffer or negative size)", what);
+        return FL_ERR_ARG;
+    }
+    memset(out_offsets, 0, sizeof(int) * ((size_t)nq + 1));
+    if (nq == 0) return FL_OK;
+    FL_CUDA(cudaSetDevice(device_));
+    const size_t qbytes = sizeof(float) * (radius ? 4 : 6) * (size_t)nq;
+    FL_CHECK(rs_q_.reserve(qbytes));
+    FL_CHECK(rs_lcnt_.reserve(sizeof(long long) * ((size_t)nq + 1)));
+    FL_CHECK(rs_loff_.reserve(sizeof(long long) * ((size_t)nq + 1)));
+    const float* d_q = rs_q_.as<float>();
+    long long* lcnt = rs_lcnt_.as<long long>();
+    long long* loff = rs_loff_.as<long long>();
+    FL_CUDA(cudaMemcpyAsync(rs_q_.ptr, queries, qbytes, cudaMemcpyHostToDevice, stream_));
+    // 1. candidate leaves per query, their offsets, the number of (query, leaf) pairs
+    FL_CUDA(cudaMemsetAsync(lcnt + nq, 0, sizeof(long long), stream_));
+    FL_CHECK(radius ? launch_range_leaves<true>(v_, d_q, nq, lcnt, nullptr, nullptr, n_sm_, stream_)
+                    : launch_range_leaves<false>(v_, d_q, nq, lcnt, nullptr, nullptr, n_sm_, stream_));
+    FL_CHECK(exclusive_sum(cub_tmp_, lcnt, loff, nq, stream_));
+    long long npairs = 0;
+    FL_CUDA(cudaMemcpyAsync(&npairs, loff + nq, sizeof(long long), cudaMemcpyDeviceToHost, stream_));
+    FL_CUDA(cudaStreamSynchronize(stream_));
+    if (npairs == 0) return FL_OK;
+    if (npairs > INT_MAX) { set_last_error("%s: %lld (query, leaf) pairs exceed INT_MAX; split the batch", what, npairs); return FL_ERR_CAPACITY; }
+    // 2. the pairs in ascending leaf order per query, then the points of each pair and their offsets
+    FL_CHECK(rs_pairs_.reserve(sizeof(int2) * (size_t)npairs));
+    FL_CHECK(rs_pcnt_.reserve(sizeof(long long) * ((size_t)npairs + 1)));
+    FL_CHECK(rs_poff_.reserve(sizeof(long long) * ((size_t)npairs + 1)));
+    int2* pairs = rs_pairs_.as<int2>();
+    long long* pcnt = rs_pcnt_.as<long long>();
+    long long* poff = rs_poff_.as<long long>();
+    FL_CHECK(radius ? launch_range_leaves<true>(v_, d_q, nq, nullptr, loff, pairs, n_sm_, stream_)
+                    : launch_range_leaves<false>(v_, d_q, nq, nullptr, loff, pairs, n_sm_, stream_));
+    FL_CUDA(cudaMemsetAsync(pcnt + npairs, 0, sizeof(long long), stream_));
+    FL_CHECK(radius ? launch_range_points<true>(v_, d_q, pairs, npairs, pcnt, nullptr, nullptr, 0, n_sm_, stream_)
+                    : launch_range_points<false>(v_, d_q, pairs, npairs, pcnt, nullptr, nullptr, 0, n_sm_, stream_));
+    FL_CHECK(exclusive_sum(cub_tmp_, pcnt, poff, npairs, stream_));
+    long long n = 0;
+    FL_CUDA(cudaMemcpyAsync(&n, poff + npairs, sizeof(long long), cudaMemcpyDeviceToHost, stream_));
+    FL_CUDA(cudaStreamSynchronize(stream_));
+    if (n > INT_MAX) { set_last_error("%s: %lld points found exceed INT_MAX; split the batch", what, n); return FL_ERR_CAPACITY; }
+    // 3. CSR offsets and the first `cap` points
+    FL_CHECK(rs_offsets_.reserve(sizeof(int) * ((size_t)nq + 1)));
+    k_range_offsets<<<(nq + 256) / 256, 256, 0, stream_>>>(loff, poff, nq, rs_offsets_.as<int>());
+    FL_CUDA(cudaGetLastError());
+    const long long m = std::min<long long>(n, cap);
+    if (m > 0) {
+        FL_CHECK(rs_out_.reserve(sizeof(float4) * (size_t)m));
+        FL_CHECK(radius ? launch_range_points<true>(v_, d_q, pairs, npairs, nullptr, poff, rs_out_.as<float4>(), m, n_sm_, stream_)
+                        : launch_range_points<false>(v_, d_q, pairs, npairs, nullptr, poff, rs_out_.as<float4>(), m, n_sm_, stream_));
+        FL_CUDA(cudaMemcpyAsync(out_xyzi, rs_out_.ptr, sizeof(float4) * (size_t)m, cudaMemcpyDeviceToHost, stream_));
+    }
+    FL_CUDA(cudaMemcpyAsync(out_offsets, rs_offsets_.ptr, sizeof(int) * ((size_t)nq + 1), cudaMemcpyDeviceToHost, stream_));
+    FL_CUDA(cudaStreamSynchronize(stream_));
+    if (total) *total = n;
     return FL_OK;
 }
 

@@ -37,6 +37,10 @@ public:
     int acquire_removed(float* out_xyzi, int cap, int* n_out);
     // all valid points, unordered (flatten(Root_Node, ..., NOT_RECORD), ikd_Tree.cpp:1627-1658)
     int flatten(float* out_xyzi, int cap, int* n_out);
+    // KD_TREE::Box_Search (ikd_Tree.cpp:464-468, radius = false; queries: nq x (min xyz, max xyz)) and KD_TREE::Radius_Search
+    // (:470-475, radius = true; queries: nq x (x, y, z, r)), batched.  Host buffers.  The points of query i are
+    // out_xyzi[out_offsets[i] .. out_offsets[i + 1]) (only the first `cap` of all are written); *total = out_offsets[nq].
+    int range_search(bool radius, const float* queries, int nq, int* out_offsets, float* out_xyzi, int cap, long long* total);
     // re-sort every valid point into fresh, evenly filled leaves (ikd-Tree's Rebuild, ikd_Tree.cpp:736-764)
     int rebuild();
     // re-list every live slot in the hashed cell directory (map.cuh); done by build / rebuild, and when inserts crowd it
@@ -86,6 +90,9 @@ private:
     DeviceBuffer ebox_[MAX_LEVELS];
     DeviceBuffer segid_, segtab_[2], bbox_;        // k-d partition build scratch
     DeviceBuffer src_, keys_in_, keys_out_, vals_in_, vals_out_, cub_tmp_, scratch_, scratch2_, scratch3_;
+    // range search: queries, per-query leaf counts / offsets, (query, leaf) pairs, per-pair point counts / offsets, output
+    DeviceBuffer rs_q_, rs_lcnt_, rs_loff_, rs_pairs_, rs_pcnt_, rs_poff_, rs_out_, rs_offsets_;
+    int n_sm_ = 0;                  // multiprocessors of the device (grid sizing)
     int* h_counters_ = nullptr;     // pinned mirror of the device counters
 };
 

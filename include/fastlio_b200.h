@@ -86,6 +86,19 @@ int fl_map_acquire_removed(fl_map_t* m, float* out_xyzi, int cap);
 /* KD_TREE::flatten(Root_Node, Storage, NOT_RECORD): all valid points  ikd_Tree.cpp:1627-1658
  * returns the number of valid points (writes at most cap of them) or an error (< 0) */
 int fl_map_flatten(fl_map_t* m, float* out_xyzi, int cap);
+/* KD_TREE::Box_Search(const BoxPointType&, PointVector&), batched     ikd_Tree.cpp:464-468 (Search_by_range :1247-1289)
+ * boxes6: nb x (min xyz, max xyz); a point is found when min <= p < max on every axis.
+ * KD_TREE::Radius_Search(PointType, float, PointVector&), batched     ikd_Tree.cpp:470-475 (Search_by_radius :1292-1332)
+ * centers_xyzr: nq x (x, y, z, radius); a point is found when its float32 squared distance (x, y, z summed in that order)
+ * is <= radius * radius rounded to float32 -- the test of :1308.  The reference decides leaves and whole subtrees by
+ * sqrtf(d2) <= radius instead, so the two answers may differ on points with d2 > fl(r * r) and sqrtf(d2) <= r.
+ * Both: CSR output.  out_offsets[nq + 1] is always written; the points of query i are out_xyzi[4 * out_offsets[i] ..
+ * 4 * out_offsets[i + 1]), in an order that is deterministic but unrelated to the reference's.  At most cap points are
+ * written (out_xyzi may be NULL when cap is 0).  Returns the total number of points found (call again with cap >= it)
+ * or an error (< 0): FL_ERR_ARG for a null buffer, FL_ERR_CAPACITY for a total above INT_MAX.  NaN input, a negative
+ * radius and an empty or inverted box find nothing. */
+int fl_map_box_search(fl_map_t* m, const float* boxes6, int nb, int* out_offsets, float* out_xyzi, int cap);
+int fl_map_radius_search(fl_map_t* m, const float* centers_xyzr, int nq, int* out_offsets, float* out_xyzi, int cap);
 /* KD_TREE::tree_range()                                              ikd_Tree.cpp:100-137 */
 int fl_map_tree_range(fl_map_t* m, float* box6);
 /* KD_TREE::Rebuild of the whole tree (ikd_Tree.cpp:736-764): re-sorts all valid points into fresh leaves */

@@ -20,8 +20,12 @@
 //   Delete_Point_Boxes(vector<Box>&)         fl_map_delete_boxes      (same return value)
 //   size() / validnum() / tree_range()       fl_map_size / fl_map_validnum / fl_map_tree_range
 //   flatten(root, Storage, type)             fl_map_flatten (all valid points)
-//   Box_Search / Radius_Search               host filter over fl_map_flatten (compat only; never
-//                                            called by laserMapping.cpp)
+//   Box_Search(box, Storage)                 fl_map_box_search, one box per call (same point set; order differs)
+//   Radius_Search(p, r, Storage)             fl_map_radius_search, one sphere per call: the literal test of
+//                                            ikd_Tree.cpp:1308, d2 <= r * r; the reference may differ on points with
+//                                            d2 > fl(r * r) and sqrtf(d2) <= r (it decides leaves by sqrtf)
+//   (extension) Box_Search_Batch /           the same, all queries in one call
+//               Radius_Search_Batch
 //   Delete_Points(PointVector&)              fl_map_delete_boxes with 2e-6 m boxes (same_point EPSS)
 //   Add_Point_Boxes(vector<Box>&)            fl_map_add_boxes: box-deleted points not yet overwritten come back
 //   acquire_removed_points(PointVector&)     fl_map_acquire_removed: the points removed by Delete_Point_Boxes since the last call
@@ -141,22 +145,35 @@ public:
     }
 
     void Box_Search(const BoxPointType& box, PointVector& Storage) {
-        PointVector all;
-        flatten(Root_Node, all, NOT_RECORD);
         Storage.clear();
-        for (const auto& p : all)
-            if (box.vertex_min[0] <= p.x && box.vertex_max[0] > p.x && box.vertex_min[1] <= p.y && box.vertex_max[1] > p.y &&
-                box.vertex_min[2] <= p.z && box.vertex_max[2] > p.z)
-                Storage.push_back(p);
+        float b[6];
+        box6(box, b);
+        range_search(fl_map_box_search, b, 1, &Storage, "Box_Search");
     }
     void Radius_Search(PointType point, const float radius, PointVector& Storage) {
-        PointVector all;
-        flatten(Root_Node, all, NOT_RECORD);
         Storage.clear();
-        for (const auto& p : all) {
-            const float d = (p.x - point.x) * (p.x - point.x) + (p.y - point.y) * (p.y - point.y) + (p.z - point.z) * (p.z - point.z);
-            if (d <= radius * radius) Storage.push_back(p);
+        const float q[4] = {point.x, point.y, point.z, radius};
+        range_search(fl_map_radius_search, q, 1, &Storage, "Radius_Search");
+    }
+    // extension: all boxes / spheres in one call (out[i] = Box_Search(boxes[i]) / Radius_Search(centers[i], radii[i]))
+    void Box_Search_Batch(const std::vector<BoxPointType>& boxes, std::vector<PointVector>& out) {
+        std::vector<float> b(boxes.size() * 6);
+        for (size_t i = 0; i < boxes.size(); i++) box6(boxes[i], &b[6 * i]);
+        out.assign(boxes.size(), PointVector());
+        if (!boxes.empty()) range_search(fl_map_box_search, b.data(), (int)boxes.size(), out.data(), "Box_Search_Batch");
+    }
+    void Radius_Search_Batch(const PointVector& centers, const std::vector<float>& radii, std::vector<PointVector>& out) {
+        out.assign(centers.size(), PointVector());
+        if (radii.size() != centers.size() && radii.size() != 1) { check(FL_ERR_ARG, "Radius_Search_Batch (one radius, or one per centre)"); return; }
+        std::vector<float> q(centers.size() * 4);
+        for (size_t i = 0; i < centers.size(); i++) {
+            q[4 * i] = centers[i].x; q[4 * i + 1] = centers[i].y; q[4 * i + 2] = centers[i].z;
+            q[4 * i + 3] = radii.size() == 1 ? radii[0] : radii[i];
         }
+        if (!centers.empty()) range_search(fl_map_radius_search, q.data(), (int)centers.size(), out.data(), "Radius_Search_Batch");
+    }
+    void Radius_Search_Batch(const PointVector& centers, float radius, std::vector<PointVector>& out) {
+        Radius_Search_Batch(centers, std::vector<float>(1, radius), out);
     }
 
     int Add_Points(PointVector& PointToAdd, bool downsample_on) {
@@ -240,6 +257,25 @@ private:
         set_intensity(p, f[3], 0);
         return p;
     }
+    static void box6(const BoxPointType& b, float* out) {
+        for (int a = 0; a < 3; a++) { out[a] = b.vertex_min[a]; out[3 + a] = b.vertex_max[a]; }
+    }
+    // one batched range call; query i's points are appended to out[i].  The buffer kept between calls usually has room; when
+    // the total is larger, the call is repeated once with room for it.
+    void range_search(int (*fn)(fl_map_t*, const float*, int, int*, float*, int), const float* q, int nq, PointVector* out, const char* what) {
+        std::vector<int> offsets((size_t)nq + 1);
+        if (range_buf_.empty()) range_buf_.resize(4 * 4096);
+        int total = fn(map_, q, nq, offsets.data(), range_buf_.data(), (int)(range_buf_.size() / 4));
+        if (total > (int)(range_buf_.size() / 4)) {
+            range_buf_.resize((size_t)total * 4);
+            total = fn(map_, q, nq, offsets.data(), range_buf_.data(), total);
+        }
+        if (check(std::min(0, total), what) < 0) return;
+        for (int i = 0; i < nq; i++) {
+            out[i].reserve(out[i].size() + (size_t)(offsets[i + 1] - offsets[i]));
+            for (int j = offsets[i]; j < offsets[i + 1]; j++) out[i].push_back(unpack(&range_buf_[(size_t)j * 4]));
+        }
+    }
     int check(int rc, const char* what) {
         if (rc < 0) { failed_ = true; fprintf(stderr, "KD_TREE(H100)::%s failed: %s\n", what, fl_last_error()); }
         return rc;
@@ -254,6 +290,7 @@ private:
     static int& default_device() { static int d = -1; return d; }
     int device_ = 0;
     int removed_pending_ = 0;      // points deleted by boxes since the last acquire_removed_points
+    std::vector<float> range_buf_; // host buffer of the range searches, grown to the largest answer seen
     bool failed_ = false;
     fl_map_t* map_ = nullptr;
     float downsample_size_;
