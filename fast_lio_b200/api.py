@@ -38,7 +38,7 @@ _lib = None
 SYMBOLS = [
     "fl_last_error", "fl_device_count", "fl_version", "fl_host_register", "fl_host_unregister", "fl_filter_debug_prof",
     "fl_map_create", "fl_map_destroy", "fl_map_set_downsample", "fl_map_build", "fl_map_size", "fl_map_validnum",
-    "fl_map_knn", "fl_map_add_points", "fl_map_delete_boxes", "fl_map_flatten", "fl_map_tree_range",
+    "fl_map_knn", "fl_map_nearest_search", "fl_map_add_points", "fl_map_delete_boxes", "fl_map_flatten", "fl_map_tree_range",
     "fl_map_rebuild", "fl_map_stats", "fl_map_add_boxes", "fl_map_box_search", "fl_map_radius_search", "fl_map_acquire_removed", "fl_map_set_cell_directory", "fl_map_dir_stats",
     "fl_filter_create", "fl_filter_destroy", "fl_filter_set_params", "fl_filter_set_solver", "fl_filter_set_search", "fl_filter_set_fused", "fl_filter_update",
     "fl_filter_map_incremental", "fl_filter_get_nearest", "fl_filter_get_selected", "fl_filter_get_pass_logs", "fl_filter_upload_scan",
@@ -73,6 +73,7 @@ def load():
     L.fl_map_size.argtypes = [C.c_void_p]
     L.fl_map_validnum.argtypes = [C.c_void_p]
     L.fl_map_knn.argtypes = [C.c_void_p, _f32p, C.c_int, C.c_int, _f32p, _f32p, _i32p]
+    L.fl_map_nearest_search.argtypes = [C.c_void_p, _f32p, C.c_int, C.c_int, C.c_float, _f32p, _f32p, _i32p]
     L.fl_map_add_points.argtypes = [C.c_void_p, _f32p, C.c_int, C.c_int]
     L.fl_map_delete_boxes.argtypes = [C.c_void_p, _f32p, C.c_int]
     L.fl_map_flatten.argtypes = [C.c_void_p, _f32p, C.c_int]
@@ -180,6 +181,18 @@ class KdTree:
         d2 = np.zeros((nq, k), dtype=np.float32)
         cnt = np.zeros(nq, dtype=np.int32)
         _check(self._L.fl_map_knn(self.h, q4, nq, k, pts, d2, cnt))
+        return pts, d2, cnt
+
+    # KD_TREE::Nearest_Search(point, k_nearest, .., max_dist), batched, 1 <= k <= 32
+    def Nearest_Search_K(self, q4, k: int, max_dist: float = np.inf):
+        """The min(k, #candidates) nearest points with float32 d2 <= fl(max_dist * max_dist), nearest first.  Returns
+        (pts[nq, k, 4], d2[nq, k], cnt[nq]); entries past cnt[i] are zero with d2 = +inf."""
+        q4 = np.ascontiguousarray(q4, dtype=np.float32).reshape(-1, 4)
+        nq = len(q4)
+        pts = np.zeros((nq, max(k, 0), 4), dtype=np.float32)
+        d2 = np.zeros((nq, max(k, 0)), dtype=np.float32)
+        cnt = np.zeros(nq, dtype=np.int32)
+        _check(self._L.fl_map_nearest_search(self.h, q4, nq, k, max_dist, pts, d2, cnt))
         return pts, d2, cnt
 
     # KD_TREE::Add_Points

@@ -100,6 +100,11 @@ int fl_map_knn(fl_map_t* m, const float* q, int nq, int k, float* out_pts, float
     if (nq > 0 && (!q || !out_pts || !out_d2 || !out_cnt)) { fl::set_last_error("fl_map_knn: null buffer"); return FL_ERR_ARG; }
     return m->impl->knn(q, nq, k, out_pts, out_d2, out_cnt);
 }
+int fl_map_nearest_search(fl_map_t* m, const float* q, int nq, int k, float max_dist, float* out_pts, float* out_d2, int* out_cnt) {
+    MAP_GUARD(m);
+    if (nq > 0 && (!q || !out_pts || !out_d2 || !out_cnt)) { fl::set_last_error("fl_map_nearest_search: null buffer"); return FL_ERR_ARG; }
+    return m->impl->nearest_search(q, nq, k, max_dist, out_pts, out_d2, out_cnt);
+}
 int fl_map_add_points(fl_map_t* m, const float* pts, int n, int downsample_on) {
     MAP_GUARD(m);
     int added = 0;

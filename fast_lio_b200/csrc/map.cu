@@ -6,6 +6,7 @@
 #include <cub/device/device_scan.cuh>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdarg>
 #include <cstdlib>
 #include <vector>
@@ -415,6 +416,31 @@ __global__ void __launch_bounds__(128) k_knn_batch(MapView m, const float4* __re
         }
         __syncthreads();
     }
+}
+
+// Nearest_Search(point, k, .., max_dist) for 6 <= k <= 32: one warp per query, the k-best list one entry per lane (KBestK),
+// seeded from the cell directory (knn_seed_k) and completed by the BVH walk where the seed is not proven.  A query with a
+// non-finite coordinate, or a NaN md2, finds nothing.  Lane j writes entry j of the row.
+__global__ void __launch_bounds__(256) k_knn_k(MapView m, const float4* __restrict__ q, int nq, int k, float md2,
+                                                float4* __restrict__ out_pts, float* __restrict__ out_d2, int* __restrict__ out_cnt) {
+    const int lane = threadIdx.x & 31;
+    const int warps = (gridDim.x * blockDim.x) >> 5;
+    const float gate = nextafterf(md2, INFINITY);
+    int walked = 0;
+    for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < nq; i += warps) {
+        const float4 qq = __ldg(&q[i]);
+        KBestK kb;
+        kb.init(k, gate);
+        if (isfinite(qq.x) && isfinite(qq.y) && isfinite(qq.z) && !isnan(md2) && !knn_seed_k(m, qq.x, qq.y, qq.z, md2, kb, lane)) {
+            walked++;
+            knn_query_from(m, qq.x, qq.y, qq.z, kb, lane);
+        }
+        float4 p;
+        const int cnt = knn_fetch_warp(m, kb, p, lane);
+        if (lane < k) { out_pts[(size_t)i * k + lane] = p; out_d2[(size_t)i * k + lane] = kb.d; }
+        if (lane == 0) out_cnt[i] = cnt;
+    }
+    if (lane == 0 && walked && m.dir.cap && m.dir.n_walked) atomicAdd(m.dir.n_walked, walked);
 }
 
 // Delete_Point_Boxes: every slot tests itself against the boxes (half-open, ikd_Tree.cpp:796).
@@ -1174,7 +1200,51 @@ static int launch_range_points(const MapView& v, const float* q, const int2* pai
     return FL_OK;
 }
 
-int Map::range_search(bool radius, const float* queries, int nq, int* out_offsets, float* out_xyzi, int cap, long long* total) {
+int Map::nearest_search(const float* q_xyzi, int nq, int k, float max_dist, float* out_pts, float* out_d2, int* out_cnt) {
+    if (nq < 0 || k < 1 || k > KNN_KMAX) { set_last_error("nearest_search: k must be in [1, %d]", KNN_KMAX); return FL_ERR_ARG; }
+    if (nq == 0) return FL_OK;
+    const float md2 = max_dist * max_dist;                 // float32, as ikd_Tree.cpp:1067
+    auto finite = [](const float* p) { return std::isfinite(p[0]) && std::isfinite(p[1]) && std::isfinite(p[2]); };
+    if (k <= KNN_K) {
+        // the thread-per-query search of the update, then the gate: on an ascending list, the leading entries with d2 <= md2
+        std::vector<float> safe;
+        const float* q = q_xyzi;
+        for (int i = 0; i < nq; i++) {
+            if (finite(q_xyzi + 4 * (size_t)i)) continue;
+            if (safe.empty()) safe.assign(q_xyzi, q_xyzi + 4 * (size_t)nq);
+            safe[4 * (size_t)i] = safe[4 * (size_t)i + 1] = safe[4 * (size_t)i + 2] = 0.f;       // answered below with nothing
+            q = safe.data();
+        }
+        FL_CHECK(knn(q, nq, k, out_pts, out_d2, out_cnt));
+        for (int i = 0; i < nq; i++) {
+            const size_t row = (size_t)i * k;
+            int c = 0;
+            if (finite(q_xyzi + 4 * (size_t)i))
+                while (c < out_cnt[i] && out_d2[row + c] <= md2) c++;
+            for (int j = c; j < out_cnt[i]; j++) {
+                memset(out_pts + 4 * (row + j), 0, sizeof(float) * 4);
+                out_d2[row + j] = INFINITY;
+            }
+            out_cnt[i] = c;
+        }
+        return FL_OK;
+    }
+    FL_CUDA(cudaSetDevice(device_));
+    const size_t qb = sizeof(float4) * (size_t)nq, pb = sizeof(float4) * (size_t)nq * k, db = sizeof(float) * (size_t)nq * k, cb = sizeof(int) * (size_t)nq;
+    FL_CHECK(scratch_.reserve(qb + pb + db + cb));
+    char* base = scratch_.as<char>();
+    float4* d_q = (float4*)base; float4* d_p = (float4*)(base + qb); float* d_d = (float*)(base + qb + pb); int* d_c = (int*)(base + qb + pb + db);
+    FL_CUDA(cudaMemcpyAsync(d_q, q_xyzi, qb, cudaMemcpyHostToDevice, stream_));
+    k_knn_k<<<resident_blocks(k_knn_k, 256, (long long)nq * 32, n_sm_), 256, 0, stream_>>>(v_, d_q, nq, k, md2, d_p, d_d, d_c);
+    FL_CUDA(cudaGetLastError());
+    FL_CUDA(cudaMemcpyAsync(out_pts, d_p, pb, cudaMemcpyDeviceToHost, stream_));
+    FL_CUDA(cudaMemcpyAsync(out_d2, d_d, db, cudaMemcpyDeviceToHost, stream_));
+    FL_CUDA(cudaMemcpyAsync(out_cnt, d_c, cb, cudaMemcpyDeviceToHost, stream_));
+    FL_CUDA(cudaStreamSynchronize(stream_));
+    return FL_OK;
+}
+
+int Map::range_search(bool radius,const float* queries, int nq, int* out_offsets, float* out_xyzi, int cap, long long* total) {
     if (total) *total = 0;
     const char* what = radius ? "radius_search" : "box_search";
     if (nq < 0 || cap < 0 || !out_offsets || (nq > 0 && !queries) || (cap > 0 && !out_xyzi)) {

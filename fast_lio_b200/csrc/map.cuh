@@ -73,6 +73,10 @@ struct MapView {
 constexpr int SLOT_FREE = 0, SLOT_VALID = 1, SLOT_BUSY = 2, SLOT_TOMB = 3, SLOT_TOMB_DS = 4;
 __device__ __forceinline__ bool slot_valid(const float4& p) { return __float_as_int(p.w) == SLOT_VALID; }
 // ----------------------------------------------------------------------------- k-best list
+// Squared distances are non-negative floats, so their bit patterns order like the values and
+// +inf (0x7f800000) can serve as the "no candidate" marker of the integer warp reductions.
+constexpr unsigned INF_BITS = 0x7f800000u;
+
 // Lane j < K holds the j-th best (distance, slot); other lanes hold +inf.  Mirrors MANUAL_HEAP
 // + PointType_CMP (ikd_Tree.h:93-201) in effect: a candidate enters only if strictly closer
 // than the current k-th best (ikd_Tree.cpp:1088); `w` caches that k-th best, warp-uniform.
@@ -82,6 +86,8 @@ struct KBest {
     float w;
     int n;          // entries filled so far (warp-uniform)
     __device__ __forceinline__ void init() { d = INFINITY; idx = -1; w = INFINITY; n = 0; }
+    __host__ __device__ static constexpr int cap() { return KNN_K; }
+    __device__ __forceinline__ static constexpr bool gated(unsigned) { return false; }       // no distance gate
     // nd, nidx warp-uniform, nd < w
     __device__ __forceinline__ void insert(float nd, int nidx, int lane) {
         const float up_d = __shfl_up_sync(FULL, d, 1);
@@ -95,14 +101,39 @@ struct KBest {
     }
 };
 
-// Squared distances are non-negative floats, so their bit patterns order like the values and
-// +inf (0x7f800000) can serve as the "no candidate" marker of the integer warp reductions.
-constexpr unsigned INF_BITS = 0x7f800000u;
+// The same list for a runtime k (1..32, lanes 0..k-1) with the distance gate of Nearest_Search's max_dist
+// (ikd_Tree.cpp:1067-1088): a point is admitted while the list is not full when d2 <= md2, and once it is full when d2 is
+// strictly below the k-th best.  gate = nextafterf(md2, +inf), so "strictly below w = min(k-th best, gate)" says both.
+// Every box of the walk is pruned against w as well, which is the reference's box_dist > md2 cut-off.
+constexpr int KNN_KMAX = 32;
+struct KBestK {
+    float d;
+    int idx;
+    float w;
+    int n;
+    int k;
+    float gate;
+    __device__ __forceinline__ void init(int k_, float gate_) { d = INFINITY; idx = -1; w = gate_; n = 0; k = k_; gate = gate_; }
+    __device__ __forceinline__ int cap() const { return k; }
+    // while the list is not full, w is the gate: the first leaf of a query stops at it
+    __device__ __forceinline__ bool gated(unsigned best) const { return best >= __float_as_uint(w); }
+    __device__ __forceinline__ void insert(float nd, int nidx, int lane) {
+        const float up_d = __shfl_up_sync(FULL, d, 1);
+        const int up_i = __shfl_up_sync(FULL, idx, 1);
+        if (lane < k && nd < d) {
+            const bool take_prev = lane > 0 && nd < up_d;
+            d = take_prev ? up_d : nd;
+            idx = take_prev ? up_i : nidx;
+        }
+        w = fminf(__shfl_sync(FULL, d, k - 1), gate);
+    }
+};
 
 // Visit one leaf bucket (and its overflow chain): each lane scores one slot, then the
 // (at most K) improving candidates are extracted in ascending order.
+template <class KB = KBest>
 __device__ __forceinline__ void knn_leaf(const MapView& m, int leaf, float qx, float qy, float qz,
-                                         KBest& kb, int lane) {
+                                         KB& kb, int lane) {
     while (leaf >= 0) {
         const float4 p = __ldg(&m.pts[leaf * LEAF + lane]);
         const int nxt = __ldg(&m.next[leaf]);
@@ -111,15 +142,15 @@ __device__ __forceinline__ void knn_leaf(const MapView& m, int leaf, float qx, f
             // empty list (the first leaf of a query): the r-th smallest goes straight to lane r -- no merge
             unsigned best = INF_BITS;
 #pragma unroll
-            for (int r = 0; r < KNN_K; r++) {
+            for (int r = 0; r < kb.cap(); r++) {
                 best = __reduce_min_sync(FULL, key);
-                if (best == INF_BITS) break;
+                if (best == INF_BITS || kb.gated(best)) break;
                 const int src = __ffs(__ballot_sync(FULL, key == best)) - 1;
                 if (lane == r) { kb.d = __uint_as_float(best); kb.idx = leaf * LEAF + src; }
                 if (lane == src) key = INF_BITS;
                 kb.n = r + 1;
             }
-            if (kb.n == KNN_K) kb.w = __uint_as_float(best);
+            if (kb.n == kb.cap()) kb.w = __uint_as_float(best);
             leaf = nxt;
             continue;
         }
@@ -130,7 +161,7 @@ __device__ __forceinline__ void knn_leaf(const MapView& m, int leaf, float qx, f
             const int src = __ffs(__ballot_sync(FULL, key == best)) - 1;
             const int cidx = leaf * LEAF + src;
             // a walk seeded with candidates found elsewhere (knn_block) meets them again here: never list a slot twice
-            if (!__any_sync(FULL, lane < KNN_K && kb.idx == cidx)) kb.insert(__uint_as_float(best), cidx, lane);
+            if (!__any_sync(FULL, lane < kb.cap() && kb.idx == cidx)) kb.insert(__uint_as_float(best), cidx, lane);
             if (lane == src) key = INF_BITS;
         }
         leaf = nxt;
@@ -143,9 +174,9 @@ __device__ __forceinline__ void knn_leaf(const MapView& m, int leaf, float qx, f
 // the box distance with its low 5 mantissa bits traded for the lane id; a child is skipped only
 // when even that rounded-DOWN distance is not below the k-th best, so pruning never drops a
 // child that could matter (it may visit one whose distance ties the bound within 2^-18).
-template <int L>
+template <int L, class KB = KBest>
 __device__ __forceinline__ void knn_node(const MapView& m, int node, float qx, float qy, float qz,
-                                         KBest& kb, int lane) {
+                                         KB& kb, int lane) {
     const int e = node * FAN + lane;
     unsigned key = 0xffffffffu;
     if (e < m.count[L - 1]) {
@@ -159,8 +190,8 @@ __device__ __forceinline__ void knn_node(const MapView& m, int node, float qx, f
         if ((best & ~31u) >= __float_as_uint(kb.w)) break;
         const int c = best & 31;
         if (lane == c) key = 0xffffffffu;
-        if constexpr (L == 1) knn_leaf(m, node * FAN + c, qx, qy, qz, kb, lane);
-        else knn_node<L - 1>(m, node * FAN + c, qx, qy, qz, kb, lane);
+        if constexpr (L == 1) knn_leaf<KB>(m, node * FAN + c, qx, qy, qz, kb, lane);
+        else knn_node<L - 1, KB>(m, node * FAN + c, qx, qy, qz, kb, lane);
     }
 }
 
@@ -168,8 +199,8 @@ __device__ __forceinline__ void knn_node(const MapView& m, int node, float qx, f
 // strict 32-ary hierarchy would have (1 M points: 41 667 leaves -> 1 303 -> 41 -> root).
 constexpr int ROOT_FAN = 64;
 
-template <int L>
-__device__ __forceinline__ void knn_root(const MapView& m, float qx, float qy, float qz, KBest& kb, int lane) {
+template <int L, class KB = KBest>
+__device__ __forceinline__ void knn_root(const MapView& m, float qx, float qy, float qz, KB& kb, int lane) {
     const int cnt = m.count[L - 1];
     unsigned k0 = 0xffffffffu, k1 = 0xffffffffu;
     if (lane < cnt) {
@@ -186,21 +217,22 @@ __device__ __forceinline__ void knn_root(const MapView& m, float qx, float qy, f
         if ((best & ~63u) >= __float_as_uint(kb.w)) break;
         const int c = best & 63;
         if (lane == (c & 31)) { if (c < 32) k0 = 0xffffffffu; else k1 = 0xffffffffu; }
-        if constexpr (L == 1) knn_leaf(m, c, qx, qy, qz, kb, lane);
-        else knn_node<L - 1>(m, c, qx, qy, qz, kb, lane);
+        if constexpr (L == 1) knn_leaf<KB>(m, c, qx, qy, qz, kb, lane);
+        else knn_node<L - 1, KB>(m, c, qx, qy, qz, kb, lane);
     }
 }
 
 // Exact k-nearest-neighbour search for one query by one warp, continuing from the list in kb (empty after kb.init(), or seeded
 // with live points and their true distances).
-__device__ __forceinline__ void knn_query_from(const MapView& m, float qx, float qy, float qz, KBest& kb, int lane) {
+template <class KB = KBest>
+__device__ __forceinline__ void knn_query_from(const MapView& m, float qx, float qy, float qz, KB& kb, int lane) {
     switch (m.n_levels) {
-        case 1: knn_root<1>(m, qx, qy, qz, kb, lane); break;
-        case 2: knn_root<2>(m, qx, qy, qz, kb, lane); break;
-        case 3: knn_root<3>(m, qx, qy, qz, kb, lane); break;
-        case 4: knn_root<4>(m, qx, qy, qz, kb, lane); break;
-        case 5: knn_root<5>(m, qx, qy, qz, kb, lane); break;
-        default: knn_root<6>(m, qx, qy, qz, kb, lane); break;
+        case 1: knn_root<1, KB>(m, qx, qy, qz, kb, lane); break;
+        case 2: knn_root<2, KB>(m, qx, qy, qz, kb, lane); break;
+        case 3: knn_root<3, KB>(m, qx, qy, qz, kb, lane); break;
+        case 4: knn_root<4, KB>(m, qx, qy, qz, kb, lane); break;
+        case 5: knn_root<5, KB>(m, qx, qy, qz, kb, lane); break;
+        default: knn_root<6, KB>(m, qx, qy, qz, kb, lane); break;
     }
 }
 
@@ -390,6 +422,20 @@ __device__ __forceinline__ void cell_scan_list(const MapView& m, int start, int 
     }
 }
 
+// A lower bound g on the distance from the query, in cell (ix, iy, iz), to every point outside the 3x3x3 block of cells around
+// that cell.  The distances from the query to the faces of its own cell are shrunk by more than any rounding of the cell
+// arithmetic.
+__device__ __forceinline__ float cell_block_dist(const CellDir& D, float qx, float qy, float qz, int ix, int iy, int iz) {
+    const float c = D.cell;
+    const float marg = 4e-6f * (fmaxf(fmaxf(fabsf(qx), fabsf(qy)), fabsf(qz)) + 2.f * c);
+    const float lox = fmaxf(qx - (float)ix * c - marg, 0.f), hix = fmaxf((float)(ix + 1) * c - qx - marg, 0.f);
+    const float loy = fmaxf(qy - (float)iy * c - marg, 0.f), hiy = fmaxf((float)(iy + 1) * c - qy - marg, 0.f);
+    const float loz = fmaxf(qz - (float)iz * c - marg, 0.f), hiz = fmaxf((float)(iz + 1) * c - qz - marg, 0.f);
+    const float c1 = c - marg;
+    const float gx = fminf(lox, hix) + c1, gy = fminf(loy, hiy) + c1, gz = fminf(loz, hiz) + c1;      // distance to the block's nearest face, per axis
+    return fminf(fminf(gx, gy), gz);
+}
+
 // k-NN of one query by one thread.  Returns true when kb is PROVEN to be the exact answer.
 __device__ __forceinline__ bool cell_knn(const MapView& m, float qx, float qy, float qz, TBest& kb) {
     const CellDir& D = m.dir;
@@ -403,16 +449,8 @@ __device__ __forceinline__ bool cell_knn(const MapView& m, float qx, float qy, f
     if (cell_list(D, cell_key(ix, iy, iz), start, cnt) <= 0) return false;
     cell_scan_list(m, start, cnt, qx, qy, qz, kb);
     if (kb.idx[KNN_K - 1] < 0) return false;
-    // ---- 3. proof: every point outside the block is at least g away.  The distances from the query to the faces of its own cell
-    // are shrunk by more than any rounding of the cell arithmetic.
-    const float c = D.cell;
-    const float marg = 4e-6f * (fmaxf(fmaxf(fabsf(qx), fabsf(qy)), fabsf(qz)) + 2.f * c);
-    const float lox = fmaxf(qx - (float)ix * c - marg, 0.f), hix = fmaxf((float)(ix + 1) * c - qx - marg, 0.f);
-    const float loy = fmaxf(qy - (float)iy * c - marg, 0.f), hiy = fmaxf((float)(iy + 1) * c - qy - marg, 0.f);
-    const float loz = fmaxf(qz - (float)iz * c - marg, 0.f), hiz = fmaxf((float)(iz + 1) * c - qz - marg, 0.f);
-    const float c1 = c - marg;
-    const float gx = fminf(lox, hix) + c1, gy = fminf(loy, hiy) + c1, gz = fminf(loz, hiz) + c1;      // distance to the block's nearest face, per axis
-    const float g = fminf(fminf(gx, gy), gz);
+    // ---- 3. proof: every point outside the block is at least g away
+    const float g = cell_block_dist(D, qx, qy, qz, ix, iy, iz);
     return kb.d[KNN_K - 1] < g * g;
 }
 
@@ -513,16 +551,17 @@ __device__ __forceinline__ int knn_fetch(const MapView& m, TBest& kb, float4 (&p
 }
 
 // the same for the warp-cooperative list of the BVH walk (lane j < K holds neighbour j)
-__device__ __forceinline__ int knn_fetch_warp(const MapView& m, KBest& kb, float4& p, int lane) {
-    const bool have = lane < KNN_K && kb.idx >= 0;
+template <class KB = KBest>
+__device__ __forceinline__ int knn_fetch_warp(const MapView& m, KB& kb, float4& p, int lane) {
+    const bool have = lane < kb.cap() && kb.idx >= 0;
     p = make_float4(0.f, 0.f, 0.f, 0.f);
     if (have) { p = __ldg(&m.pts[kb.idx]); p.w = __ldg(&m.payload[kb.idx]); }
     const int cnt = __popc(__ballot_sync(FULL, have));
     const float dn = __shfl_down_sync(FULL, kb.d, 1);
     const bool tie = lane + 1 < cnt && fabsf(dn - kb.d) < 1e-10f;
-    if (__any_sync(FULL, tie)) {                    // odd-even transposition over the (at most five) entries
+    if (__any_sync(FULL, tie)) {                    // odd-even transposition over the (at most K) entries
 #pragma unroll
-        for (int pass = 0; pass < KNN_K; pass++) {
+        for (int pass = 0; pass < kb.cap(); pass++) {
             const int partner = ((lane + pass) & 1) ? lane - 1 : lane + 1;
             const int pl = min(max(partner, 0), 31);
             const float od = __shfl_sync(FULL, kb.d, pl);
@@ -537,6 +576,49 @@ __device__ __forceinline__ int knn_fetch_warp(const MapView& m, KBest& kb, float
         }
     }
     return cnt;
+}
+
+// Seed of a runtime-k query (KBestK, empty on entry) from the cell directory, by one warp: lane 0 finds the query's cell, the
+// warp scores its halo list 32 entries at a time and merges the admissible points like knn_leaf does.  Returns true when the
+// list is PROVEN to be the exact answer: every point outside the block is at least g away (cell_block_dist), so the list is
+// final when it holds k entries and the k-th is below g^2, or when md2 < g^2 (every admissible point lies in the block, however
+// few there are).  Otherwise the list seeds the BVH walk (knn_query_from), which only adds what the block did not hold.
+__device__ __forceinline__ bool knn_seed_k(const MapView& m, float qx, float qy, float qz, float md2, KBestK& kb, int lane) {
+    const CellDir& D = m.dir;
+    if (D.cap == 0u) return false;
+    const float inv = D.inv_cell;
+    const int ix = cell_coord(qx, inv), iy = cell_coord(qy, inv), iz = cell_coord(qz, inv);
+    if (abs(ix) >= CELL_CLAMP - 1 || abs(iy) >= CELL_CLAMP - 1 || abs(iz) >= CELL_CLAMP - 1) return false;
+    int start = 0, cnt = 0, ok = 0;
+    if (lane == 0) ok = cell_list(D, cell_key(ix, iy, iz), start, cnt);
+    ok = __shfl_sync(FULL, ok, 0);
+    if (ok <= 0) return false;
+    start = __shfl_sync(FULL, start, 0);
+    cnt = __shfl_sync(FULL, cnt, 0);
+#pragma unroll 1
+    for (int b = 0; b < cnt; b += 32) {
+        unsigned key = INF_BITS;
+        int slot = -1;
+        if (b + lane < cnt) {
+            slot = __ldg(&D.lists[start + b + lane]);
+            const float4 p = __ldg(&m.pts[slot]);
+            if (slot_valid(p)) key = __float_as_uint(sq_dist3(qx, qy, qz, p.x, p.y, p.z));
+        }
+#pragma unroll 1
+        while (true) {
+            const unsigned best = __reduce_min_sync(FULL, key);
+            if (best >= __float_as_uint(kb.w)) break;
+            const int src = __ffs(__ballot_sync(FULL, key == best)) - 1;
+            const int cidx = __shfl_sync(FULL, slot, src);
+            // a list may name a slot twice: never list it twice
+            if (!__any_sync(FULL, lane < kb.k && kb.idx == cidx)) kb.insert(__uint_as_float(best), cidx, lane);
+            if (lane == src) key = INF_BITS;
+        }
+    }
+    kb.n = __popc(__ballot_sync(FULL, kb.idx >= 0));
+    const float g = cell_block_dist(D, qx, qy, qz, ix, iy, iz);
+    const float g2 = g * g;
+    return __shfl_sync(FULL, kb.d, kb.k - 1) < g2 || md2 < g2;
 }
 
 }  // namespace fl

@@ -27,6 +27,8 @@ public:
     int build_device(const float4* d_pts_xyzi, int n);
     // KD_TREE::Nearest_Search, batched (ikd_Tree.cpp:426-461); host buffers
     int knn(const float* q_xyzi, int nq, int k, float* out_pts, float* out_d2, int* out_cnt);
+    // KD_TREE::Nearest_Search(point, k, .., max_dist), batched, 1 <= k <= KNN_KMAX (fl_map_nearest_search); host buffers
+    int nearest_search(const float* q_xyzi, int nq, int k, float max_dist, float* out_pts, float* out_d2, int* out_cnt);
     // KD_TREE::Delete_Point_Boxes (ikd_Tree.cpp:632-658); returns the number of points invalidated in *deleted
     int delete_boxes(const float* boxes6, int nb, int* deleted);
     // KD_TREE::Add_Points (ikd_Tree.cpp:478-573); *added = the reference's return value

@@ -68,6 +68,21 @@ int fl_map_validnum(fl_map_t* m);
  * out_pts: nq*k*4 floats (ascending distance), out_d2: nq*k floats, out_cnt: nq ints.  Safe for
  * concurrent host callers on one handle (internally serialised). */
 int fl_map_knn(fl_map_t* m, const float* q_xyzi, int nq, int k, float* out_pts, float* out_d2, int* out_cnt);
+/* KD_TREE::Nearest_Search(point, k_nearest, Nearest_Points, Point_Distance, max_dist), batched
+ *                                                                    ikd_Tree.cpp:426-461, Search :1062-1244
+ * The layout of fl_map_knn: out_pts nq*k*4 floats, out_d2 nq*k floats, out_cnt nq ints; entries j >= out_cnt[i] are
+ * (0, 0, 0, 0) with d2 = +inf.  1 <= k <= 32, else FL_ERR_ARG (so is a null buffer with nq > 0).
+ * With md2 = max_dist * max_dist rounded to float32 (:1067), a point is a candidate when its float32 squared distance (x, y, z
+ * summed in that order, bit-identical to the reference's) is <= md2; the answer is the min(k, #candidates) nearest
+ * candidates.  So max_dist = +inf applies no gate, a negative max_dist acts as |max_dist|, 0 finds only coincident points
+ * and NaN finds nothing, as in the reference.  A query with a non-finite coordinate finds nothing.
+ * Order: ascending d2; adjacent entries whose d2 differ by less than 1e-10 are ordered by ascending x (PointType_CMP,
+ * ikd_Tree.h:102-108).  Where the k-th and the (k+1)-th candidates tie, the reference keeps whichever its traversal found
+ * first; this map keeps one deterministically (the same bytes on every call for the same map and queries).
+ * k <= 5 runs the search of fl_map_knn and cuts its answer at md2; 6 <= k <= 32 runs one warp per query.  Serialised on the
+ * handle like the other map calls. */
+int fl_map_nearest_search(fl_map_t* m, const float* q_xyzi, int nq, int k, float max_dist,
+                          float* out_pts, float* out_d2, int* out_cnt);
 /* KD_TREE::Add_Points(PointVector&, bool downsample_on) -> int       ikd_Tree.cpp:478-573
  * returns the reference's return value (>= 0) or an error (< 0) */
 int fl_map_add_points(fl_map_t* m, const float* pts_xyzi, int n, int downsample_on);

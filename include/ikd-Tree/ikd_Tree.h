@@ -26,6 +26,8 @@
 //                                            d2 > fl(r * r) and sqrtf(d2) <= r (it decides leaves by sqrtf)
 //   (extension) Box_Search_Batch /           the same, all queries in one call
 //               Radius_Search_Batch
+//   (extension) Nearest_Search_K(p, k, out,  fl_map_nearest_search: any 1 <= k <= 32, max_dist applied on the device
+//               dist, max) / _K_Batch        (d2 <= fl(max_dist * max_dist)); one query per call / all queries in one call
 //   Delete_Points(PointVector&)              fl_map_delete_boxes with 2e-6 m boxes (same_point EPSS)
 //   Add_Point_Boxes(vector<Box>&)            fl_map_add_boxes: box-deleted points not yet overwritten come back
 //   acquire_removed_points(PointVector&)     fl_map_acquire_removed: the points removed by Delete_Point_Boxes since the last call
@@ -34,7 +36,8 @@
 //
 // Limits and failure reporting (the reference's members return void / int and cannot fail):
 //   * k_nearest <= 5 (NUM_MATCH_POINTS, include/common_lib.h:26 -- the only k FAST-LIO uses).  A larger k is an error:
-//     the call prints a diagnostic once, returns no neighbours and sets failed().
+//     the call prints a diagnostic once, returns no neighbours and sets failed().  Nearest_Search_K takes 1 <= k <= 32;
+//     outside that range it returns no neighbours and sets failed().
 //   * the CUDA device is chosen by KD_TREE::set_default_device(i) before construction, else by the environment variable
 //     FASTLIO_B200_DEVICE, else device 0 (the reference's tree is a global object, laserMapping.cpp:120).
 //   * ok() tells whether the device map exists (no GPU / out of memory at construction); failed() whether any call on
@@ -137,6 +140,32 @@ public:
         out_points.assign(nq, PointVector());
         out_dist.assign(nq, std::vector<float>());
         if (nq == 0 || check(fl_map_knn(map_, q.data(), nq, k, pts.data(), d2.data(), cnt.data()), "Nearest_Search_Batch") != FL_OK) return;
+        for (int i = 0; i < nq; i++)
+            for (int j = 0; j < cnt[i]; j++) {
+                out_points[i].push_back(unpack(&pts[((size_t)i * k + j) * 4]));
+                out_dist[i].push_back(d2[(size_t)i * k + j]);
+            }
+    }
+
+    // extension: KD_TREE::Nearest_Search for any 1 <= k_nearest <= 32, with max_dist applied by the device search
+    void Nearest_Search_K(PointType point, int k_nearest, PointVector& Nearest_Points, std::vector<float>& Point_Distance,
+                          float max_dist = INFINITY) {
+        std::vector<PointVector> p;
+        std::vector<std::vector<float>> d;
+        Nearest_Search_K_Batch(PointVector(1, point), k_nearest, p, d, max_dist);
+        Nearest_Points.swap(p[0]);
+        Point_Distance.swap(d[0]);
+    }
+    void Nearest_Search_K_Batch(const PointVector& queries, int k_nearest, std::vector<PointVector>& out_points,
+                                std::vector<std::vector<float>>& out_dist, float max_dist = INFINITY) {
+        const int nq = (int)queries.size();
+        out_points.assign(nq, PointVector());
+        out_dist.assign(nq, std::vector<float>());
+        const int k = std::max(k_nearest, 1);
+        std::vector<float> q, pts((size_t)nq * k * 4), d2((size_t)nq * k);
+        std::vector<int> cnt(std::max(nq, 1));
+        pack(queries, q);
+        if (check(fl_map_nearest_search(map_, q.data(), nq, k_nearest, max_dist, pts.data(), d2.data(), cnt.data()), "Nearest_Search_K") != FL_OK) return;
         for (int i = 0; i < nq; i++)
             for (int j = 0; j < cnt[i]; j++) {
                 out_points[i].push_back(unpack(&pts[((size_t)i * k + j) * 4]));
