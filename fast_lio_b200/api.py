@@ -40,6 +40,8 @@ SYMBOLS = [
     "fl_map_create", "fl_map_destroy", "fl_map_set_downsample", "fl_map_build", "fl_map_size", "fl_map_validnum",
     "fl_map_knn", "fl_map_nearest_search", "fl_map_add_points", "fl_map_delete_boxes", "fl_map_flatten", "fl_map_tree_range",
     "fl_map_rebuild", "fl_map_stats", "fl_map_add_boxes", "fl_map_box_search", "fl_map_radius_search", "fl_map_acquire_removed", "fl_map_set_cell_directory", "fl_map_dir_stats",
+    "fl_map_nearest_search_device", "fl_map_range_workspace_bytes", "fl_map_box_search_device", "fl_map_radius_search_device",
+    "fl_map_build_device", "fl_map_add_points_device",
     "fl_filter_create", "fl_filter_destroy", "fl_filter_set_params", "fl_filter_set_solver", "fl_filter_set_search", "fl_filter_set_fused", "fl_filter_update",
     "fl_filter_map_incremental", "fl_filter_get_nearest", "fl_filter_get_selected", "fl_filter_get_pass_logs", "fl_filter_upload_scan",
     "fl_filter_upload_state", "fl_filter_run", "fl_filter_download_state", "fl_filter_sync",
@@ -86,6 +88,14 @@ def load():
     L.fl_map_stats.argtypes = [C.c_void_p, _i32p]
     L.fl_map_set_cell_directory.argtypes = [C.c_void_p, C.c_int, C.c_float]
     L.fl_map_dir_stats.argtypes = [C.c_void_p, _i32p]
+    # device-buffer forms: raw device addresses and a cudaStream_t
+    _vp = C.c_void_p
+    L.fl_map_nearest_search_device.argtypes = [_vp, _vp, C.c_int, C.c_int, C.c_float, _vp, _vp, _vp, _vp]
+    L.fl_map_range_workspace_bytes.argtypes = [_vp, C.c_int, C.c_longlong, C.POINTER(C.c_ulonglong)]
+    for fn in (L.fl_map_box_search_device, L.fl_map_radius_search_device):
+        fn.argtypes = [_vp, _vp, C.c_int, _vp, _vp, C.c_longlong, _vp, C.c_ulonglong, _vp, _vp]
+    L.fl_map_build_device.argtypes = [_vp, _vp, C.c_int, _vp]
+    L.fl_map_add_points_device.argtypes = [_vp, _vp, C.c_int, C.c_int, _vp]
     L.fl_filter_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int]
     L.fl_filter_destroy.argtypes = [C.c_void_p]
     L.fl_filter_set_params.argtypes = [C.c_void_p, C.c_int, _f64p, C.c_int]
@@ -144,6 +154,7 @@ class KdTree:
         h = C.c_void_p()
         _check(self._L.fl_map_create(C.byref(h), device, downsample))
         self.h = h
+        self.device = device
         if not cell_directory or cell_size > 0.0:
             _check(self._L.fl_map_set_cell_directory(self.h, int(cell_directory), cell_size))
 
@@ -254,6 +265,107 @@ class KdTree:
             total = _check(fn(self.h, q, len(q), offsets, out, total))
         self._range_hint = total
         return offsets, out[:total]
+
+    # ---- device-buffer forms: CUDA tensors on the map's device, enqueued on torch.cuda.current_stream()
+    def _tensor(self, t, name: str, cols: int | None):
+        import torch
+        if not isinstance(t, torch.Tensor):
+            raise TypeError(f"{name}: expected a torch.Tensor, got {type(t).__name__}")
+        if t.device.type != "cuda" or t.device.index != self.device:
+            raise ValueError(f"{name}: expected a tensor on cuda:{self.device}, got one on {t.device}")
+        if t.dtype != torch.float32:
+            raise TypeError(f"{name}: expected float32, got {t.dtype}")
+        if not t.is_contiguous():
+            raise ValueError(f"{name}: expected a contiguous tensor")
+        if cols is not None and (t.dim() != 2 or t.shape[1] != cols):
+            raise ValueError(f"{name}: expected shape (n, {cols}), got {tuple(t.shape)}")
+        return t
+
+    def _stream(self):
+        import torch
+        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def nearest_search_device(self, q, k: int, max_dist: float = float("inf")):
+        """fl_map_nearest_search on device tensors: q (nq, 4) float32.  Returns (pts [nq, k, 4], d2 [nq, k], cnt [nq] int32),
+        the bytes Nearest_Search_K returns, written on the current stream without a host synchronisation."""
+        import torch
+        q = self._tensor(q, "q", 4)
+        nq = q.shape[0]
+        if not 1 <= k <= 32:
+            raise ValueError(f"k must be in [1, 32], got {k}")
+        pts = torch.empty((nq, k, 4), dtype=torch.float32, device=q.device)
+        d2 = torch.empty((nq, k), dtype=torch.float32, device=q.device)
+        cnt = torch.empty((nq,), dtype=torch.int32, device=q.device)
+        _check(self._L.fl_map_nearest_search_device(self.h, q.data_ptr(), nq, k, max_dist, pts.data_ptr(), d2.data_ptr(),
+                                                    cnt.data_ptr(), self._stream()))
+        return pts, d2, cnt
+
+    def range_workspace_bytes(self, nq: int, max_pairs: int) -> int:
+        out = C.c_ulonglong(0)
+        _check(self._L.fl_map_range_workspace_bytes(self.h, nq, max_pairs, C.byref(out)))
+        return out.value
+
+    def range_workspace(self, nq: int, max_pairs: int):
+        """A uint8 CUDA tensor large enough for a range query of nq queries and up to max_pairs (query, leaf) pairs."""
+        import torch
+        return torch.empty(self.range_workspace_bytes(nq, max_pairs), dtype=torch.uint8, device=f"cuda:{self.device}")
+
+    def box_search_device(self, boxes, cap: int | None = None, workspace=None):
+        """fl_map_box_search_device: boxes (nb, 6) float32.  Returns (offsets [nb + 1] int32, pts, status [2] int64) as tensors.
+        With both `cap` and `workspace` given, one call is enqueued and nothing synchronises: pts has `cap` rows, of which the
+        first min(status[0], cap) are written when status[0] >= 0 (see the header).  Otherwise the status is read (a
+        synchronisation) and the call is repeated once with enough room; pts then holds exactly the points found."""
+        return self._range_device(self._L.fl_map_box_search_device, self._tensor(boxes, "boxes", 6), cap, workspace)
+
+    def radius_search_device(self, centers_xyzr, cap: int | None = None, workspace=None):
+        """fl_map_radius_search_device: centers_xyzr (nq, 4) float32 = (x, y, z, radius).  Returns like box_search_device."""
+        return self._range_device(self._L.fl_map_radius_search_device, self._tensor(centers_xyzr, "centers_xyzr", 4), cap, workspace)
+
+    def _range_device(self, fn, q, cap, workspace):
+        import torch
+        nq = q.shape[0]
+        dev = q.device
+        offsets = torch.empty(nq + 1, dtype=torch.int32, device=dev)
+        status = torch.empty(2, dtype=torch.int64, device=dev)
+
+        def call(cap_, ws):
+            if ws is not None and (not isinstance(ws, torch.Tensor) or ws.device != dev or not ws.is_contiguous()):
+                raise ValueError(f"workspace: expected a contiguous tensor on {dev}")
+            pts = torch.empty((max(cap_, 0), 4), dtype=torch.float32, device=dev)
+            _check(fn(self.h, q.data_ptr(), nq, offsets.data_ptr(), pts.data_ptr() if cap_ > 0 else None, cap_,
+                      ws.data_ptr() if ws is not None and nq > 0 else None, ws.numel() * ws.element_size() if ws is not None else 0,
+                      status.data_ptr(), self._stream()))
+            return pts
+
+        if cap is not None and workspace is not None:
+            return offsets, call(cap, workspace), status
+        if cap is None:
+            cap = max(self.validnum(), getattr(self, "_range_hint", 0), 1024)
+        if workspace is None:
+            workspace = self.range_workspace(nq, max(getattr(self, "_pairs_hint", 0), 4 * nq, 1024)) if nq > 0 else None
+        pts = call(cap, workspace)
+        total, npairs = (int(x) for x in status.cpu())
+        if total < 0:                                         # the pairs did not fit: a workspace sized from status[1]
+            workspace = self.range_workspace(nq, npairs)
+            pts = call(cap, workspace)
+            total, npairs = (int(x) for x in status.cpu())
+        if total > 2**31 - 1:
+            raise FastLioError(f"{total} points found exceed INT_MAX; split the batch")
+        if total > cap:
+            pts = call(total, workspace)
+        self._range_hint, self._pairs_hint = total, npairs
+        return offsets, pts[:total], status
+
+    def build_device(self, pts):
+        """KD_TREE::Build from a (n, 4) float32 tensor on the map's device (synchronous)."""
+        pts = self._tensor(pts, "pts", 4)
+        _check(self._L.fl_map_build_device(self.h, pts.data_ptr() if len(pts) else None, len(pts), self._stream()))
+
+    def add_points_device(self, pts, downsample_on: bool) -> int:
+        """KD_TREE::Add_Points from a (n, 4) float32 tensor on the map's device (synchronous); the reference's return value."""
+        pts = self._tensor(pts, "pts", 4)
+        return _check(self._L.fl_map_add_points_device(self.h, pts.data_ptr() if len(pts) else None, len(pts), int(downsample_on),
+                                                       self._stream()))
 
     def tree_range(self) -> np.ndarray:
         box = np.zeros(6, dtype=np.float32)

@@ -87,7 +87,13 @@ int fl_map_destroy(fl_map_t* m) {
     map_release(m);
     return FL_OK;
 }
+// Every call that may enqueue work on the handle's stream touch()es the map: the next device-buffer query joins that work.
 #define MAP_GUARD(m)                                                             \
+    if (!(m) || !(m)->impl) { fl::set_last_error("null map handle"); return FL_ERR_ARG; } \
+    std::lock_guard<std::mutex> _lk((m)->mu);                                    \
+    (m)->impl->touch()
+// the device-buffer queries: stream-ordered on the caller's stream, they leave the handle's stream's frontier as it is
+#define MAP_QUERY_GUARD(m)                                                       \
     if (!(m) || !(m)->impl) { fl::set_last_error("null map handle"); return FL_ERR_ARG; } \
     std::lock_guard<std::mutex> _lk((m)->mu)
 
@@ -147,6 +153,40 @@ int fl_map_radius_search(fl_map_t* m, const float* centers_xyzr, int nq, int* ou
     int rc = m->impl->range_search(true, centers_xyzr, nq, out_offsets, out_xyzi, cap, &total);
     return rc == FL_OK ? (int)total : rc;
 }
+int fl_map_nearest_search_device(fl_map_t* m, const float* q_xyzi_device, int nq, int k, float max_dist,
+                                 float* out_pts_device, float* out_d2_device, int* out_cnt_device, void* stream) {
+    MAP_QUERY_GUARD(m);
+    return m->impl->nearest_search_device(q_xyzi_device, nq, k, max_dist, out_pts_device, out_d2_device, out_cnt_device,
+                                          static_cast<cudaStream_t>(stream));
+}
+int fl_map_range_workspace_bytes(fl_map_t* m, int nq, long long max_pairs, unsigned long long* out_bytes) {
+    MAP_QUERY_GUARD(m);
+    return m->impl->range_workspace_bytes(nq, max_pairs, out_bytes);
+}
+int fl_map_box_search_device(fl_map_t* m, const float* boxes6_device, int nb, int* out_offsets_device, float* out_xyzi_device,
+                             long long cap, void* workspace_device, unsigned long long workspace_bytes, long long* status2_device,
+                             void* stream) {
+    MAP_QUERY_GUARD(m);
+    return m->impl->range_search_device(false, boxes6_device, nb, out_offsets_device, out_xyzi_device, cap, workspace_device,
+                                        workspace_bytes, status2_device, static_cast<cudaStream_t>(stream));
+}
+int fl_map_radius_search_device(fl_map_t* m, const float* centers_xyzr_device, int nq, int* out_offsets_device, float* out_xyzi_device,
+                                long long cap, void* workspace_device, unsigned long long workspace_bytes, long long* status2_device,
+                                void* stream) {
+    MAP_QUERY_GUARD(m);
+    return m->impl->range_search_device(true, centers_xyzr_device, nq, out_offsets_device, out_xyzi_device, cap, workspace_device,
+                                        workspace_bytes, status2_device, static_cast<cudaStream_t>(stream));
+}
+int fl_map_build_device(fl_map_t* m, const float* pts_xyzi_device, int n, void* stream) {
+    MAP_GUARD(m);
+    return m->impl->build_from_caller(pts_xyzi_device, n, static_cast<cudaStream_t>(stream));
+}
+int fl_map_add_points_device(fl_map_t* m, const float* pts_xyzi_device, int n, int downsample_on, void* stream) {
+    MAP_GUARD(m);
+    int added = 0;
+    int rc = m->impl->add_points_from_caller(pts_xyzi_device, n, downsample_on != 0, static_cast<cudaStream_t>(stream), &added);
+    return rc == FL_OK ? added : rc;
+}
 int fl_map_tree_range(fl_map_t* m, float* box6) { MAP_GUARD(m); if (!box6) return FL_ERR_ARG; return m->impl->tree_range(box6); }
 int fl_map_rebuild(fl_map_t* m) { MAP_GUARD(m); return m->impl->rebuild(); }
 int fl_map_stats(fl_map_t* m, int* out4) {
@@ -171,7 +211,8 @@ int fl_map_dir_stats(fl_map_t* m, int* out6) {
 // ------------------------------------------------------------------------------------ filter
 #define FILTER_GUARD(f)                                                                        \
     if (!(f) || !(f)->impl) { fl::set_last_error("null filter handle"); return FL_ERR_ARG; }   \
-    std::lock_guard<std::mutex> _lk((f)->map->mu)
+    std::lock_guard<std::mutex> _lk((f)->map->mu);                                             \
+    (f)->map->impl->touch()
 
 int fl_filter_create(fl_filter_t** out, fl_map_t* map, int max_points) {
     if (!out || !map || !map->impl) { fl::set_last_error("fl_filter_create: null argument"); return FL_ERR_ARG; }
@@ -324,7 +365,8 @@ int fl_filter_time_search_pass(fl_filter_t* f, int reps, int flush_l2, float* ms
 // ------------------------------------------------------------------------------------ scan front end
 #define SCAN_GUARD(s)                                                                        \
     if (!(s) || !(s)->impl) { fl::set_last_error("null scan handle"); return FL_ERR_ARG; }   \
-    std::lock_guard<std::mutex> _lk((s)->map->mu)
+    std::lock_guard<std::mutex> _lk((s)->map->mu);                                             \
+    (s)->map->impl->touch()
 
 int fl_scan_create(fl_scan_t** out, fl_map_t* map) {
     if (!out) return FL_ERR_ARG;

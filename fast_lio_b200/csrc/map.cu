@@ -2,6 +2,8 @@
 // H100-native replacement for the subset of KD_TREE<PointType> that FAST-LIO's
 // laserMapping.cpp calls (reference include/ikd-Tree/ikd_Tree.cpp).  See map.cuh for the
 // memory layout and DESIGN.md for the rationale.
+#include <cub/block/block_reduce.cuh>
+#include <cub/block/block_scan.cuh>
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
@@ -390,10 +392,13 @@ __global__ void __launch_bounds__(256) k_halo_fix(MapView m, const unsigned* __r
 }
 
 // Batched Nearest_Search: one lane per query (cell directory), BVH walk by the warp for what that cannot prove.
-__global__ void __launch_bounds__(128) k_knn_batch(MapView m, const float4* __restrict__ q, int nq, int k,
-                                                    float4* __restrict__ out_pts, float* __restrict__ out_d2,
-                                                    int* __restrict__ out_cnt) {
-    __shared__ WalkPool pool;
+// GATED (the device form of fl_map_nearest_search for k <= KNN_K): a query with a non-finite coordinate is searched at the
+// origin, as the host form does (so fl_map_dir_stats counts it the same way), and finds nothing; every other row keeps its
+// leading entries with d2 <= md2.  Dropped entries are (0, 0, 0, 0) with d2 = +inf.
+template <bool GATED>
+__device__ __forceinline__ void knn_batch(const MapView& m, const float4* __restrict__ q, int nq, int k, float md2,
+                                          float4* __restrict__ out_pts, float* __restrict__ out_d2, int* __restrict__ out_cnt,
+                                          WalkPool& pool) {
     if (threadIdx.x == 0) pool.n[0] = pool.n[1] = 0;
     __syncthreads();
     int phase = 0;
@@ -403,19 +408,47 @@ __global__ void __launch_bounds__(128) k_knn_batch(MapView m, const float4* __re
         const bool active = i < nq;
         float4 qq = make_float4(0.f, 0.f, 0.f, 0.f);
         if (active) qq = __ldg(&q[i]);
+        bool finite = true;
+        if constexpr (GATED) {
+            finite = isfinite(qq.x) && isfinite(qq.y) && isfinite(qq.z);
+            if (!finite) qq.x = qq.y = qq.z = 0.f;
+        }
         TBest kb;
         knn_block(m, active, qq.x, qq.y, qq.z, kb, pool, phase);
         if (active) {
             float4 p[KNN_K];
             const int cnt = knn_fetch(m, kb, p);
+            int c = min(k, cnt);
+            if constexpr (GATED) {
+                int g = 0;
+#pragma unroll
+                for (int j = 0; j < KNN_K; j++) g += (finite && g == j && j < c && kb.d[j] <= md2) ? 1 : 0;
+                c = g;
+#pragma unroll
+                for (int j = 0; j < KNN_K; j++) {
+                    if (j >= c) { p[j] = make_float4(0.f, 0.f, 0.f, 0.f); kb.d[j] = INFINITY; }
+                }
+            }
 #pragma unroll
             for (int j = 0; j < KNN_K; j++) {
                 if (j < k) { out_pts[(size_t)i * k + j] = p[j]; out_d2[(size_t)i * k + j] = kb.d[j]; }
             }
-            out_cnt[i] = min(k, cnt);
+            out_cnt[i] = c;
         }
         __syncthreads();
     }
+}
+__global__ void __launch_bounds__(128) k_knn_batch(MapView m, const float4* __restrict__ q, int nq, int k,
+                                                    float4* __restrict__ out_pts, float* __restrict__ out_d2,
+                                                    int* __restrict__ out_cnt) {
+    __shared__ WalkPool pool;
+    knn_batch<false>(m, q, nq, k, 0.f, out_pts, out_d2, out_cnt, pool);
+}
+__global__ void __launch_bounds__(128) k_knn_batch_gated(MapView m, const float4* __restrict__ q, int nq, int k, float md2,
+                                                          float4* __restrict__ out_pts, float* __restrict__ out_d2,
+                                                          int* __restrict__ out_cnt) {
+    __shared__ WalkPool pool;
+    knn_batch<true>(m, q, nq, k, md2, out_pts, out_d2, out_cnt, pool);
 }
 
 // Nearest_Search(point, k, .., max_dist) for 6 <= k <= 32: one warp per query, the k-best list one entry per lane (KBestK),
@@ -783,8 +816,8 @@ struct RangeLeaves {             // box_query functor: counts (out == nullptr) o
 // One warp per query.  Count pass (pairs == nullptr): cnt[i] = candidate leaves.  Fill pass: the (query, leaf) pairs at
 // off[i], in ascending leaf order (box_query visits children in lane order).
 template <bool RADIUS>
-__global__ void __launch_bounds__(256) k_range_leaves(MapView m, const float* __restrict__ q, int nq, long long* __restrict__ cnt,
-                                                      const long long* __restrict__ off, int2* __restrict__ pairs) {
+__device__ __forceinline__ void range_leaves(const MapView& m, const float* __restrict__ q, int nq, long long* __restrict__ cnt,
+                                             const long long* __restrict__ off, int2* __restrict__ pairs) {
     const int lane = threadIdx.x & 31;
     const int warps = (gridDim.x * blockDim.x) >> 5;
     for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < nq; i += warps) {
@@ -794,6 +827,18 @@ __global__ void __launch_bounds__(256) k_range_leaves(MapView m, const float* __
         box_query(m, Q.bmin, Q.bmax, f, lane);
         if (lane == 0 && !pairs) cnt[i] = f.n;
     }
+}
+template <bool RADIUS>
+__global__ void __launch_bounds__(256) k_range_leaves(MapView m, const float* __restrict__ q, int nq, long long* __restrict__ cnt,
+                                                      const long long* __restrict__ off, int2* __restrict__ pairs) {
+    range_leaves<RADIUS>(m, q, nq, cnt, off, pairs);
+}
+// the fill pass of the device-buffer form: the pairs are listed only when all off[nq] of them fit the caller's workspace
+template <bool RADIUS>
+__global__ void __launch_bounds__(256) k_range_leaves_bounded(MapView m, const float* __restrict__ q, int nq, const long long* __restrict__ off,
+                                                              int2* __restrict__ pairs, long long max_pairs) {
+    if (off[nq] > max_pairs) return;
+    range_leaves<RADIUS>(m, q, nq, nullptr, off, pairs);
 }
 // One warp per (query, leaf) pair: the leaf and its overflow chain, one slot per lane.  Count pass (out == nullptr): cnt[w] =
 // points found.  Fill pass: (x, y, z, intensity) of each at off[w] + the prefix popcount, the first `cap` of all only.
@@ -839,6 +884,103 @@ __global__ void k_range_offsets(const long long* __restrict__ leaf_off, const lo
     if (i <= nq) offsets[i] = (int)point_off[leaf_off[i]];
 }
 
+// ----------------------------------------------------------------------------- the same, sized on the device
+// fl_map_box_search_device / fl_map_radius_search_device never read a count back: the number of pairs and of points stay in
+// device memory (the control words below), and every kernel runs a grid sized from host-known bounds and loops up to them.
+enum RangeCtl { RS_PAIRS = 0,       // pairs listed: off[nq] when it fits the workspace, else 0
+                RS_FILL,            // pairs whose points are written: RS_PAIRS, or 0 when nothing may be written
+                RS_OK,              // 1: the offsets are written in full
+                RS_CTL_COUNT };
+__global__ void k_range_plan(const long long* __restrict__ leaf_off, int nq, long long max_pairs, long long* __restrict__ ctl) {
+    const long long np = leaf_off[nq];
+    ctl[RS_PAIRS] = np <= max_pairs ? np : 0;
+}
+template <bool RADIUS>
+__global__ void __launch_bounds__(256) k_range_count_dev(MapView m, const float* __restrict__ q, const int2* __restrict__ pairs,
+                                                         const long long* __restrict__ npairs, long long* __restrict__ cnt) {
+    range_points<RADIUS>(m, q, pairs, *npairs, cnt, nullptr, nullptr, 0);
+}
+template <bool RADIUS>
+__global__ void __launch_bounds__(256) k_range_fill_dev(MapView m, const float* __restrict__ q, const int2* __restrict__ pairs,
+                                                        const long long* __restrict__ npairs, const long long* __restrict__ off,
+                                                        float4* __restrict__ out, long long cap) {
+    range_points<RADIUS>(m, q, pairs, *npairs, nullptr, off, out, cap);
+}
+// status2 = (points found, pairs needed), or (-1, pairs needed) when the pairs did not fit; decides what may be written
+__global__ void k_range_status(const long long* __restrict__ leaf_off, const long long* __restrict__ point_off, int nq, long long max_pairs,
+                               long long* __restrict__ ctl, long long* __restrict__ status2) {
+    const long long np = leaf_off[nq];
+    long long total = -1;
+    bool ok = false;
+    if (np <= max_pairs) {
+        total = point_off[ctl[RS_PAIRS]];
+        ok = total <= INT_MAX;                 // above: the counterpart of FL_ERR_CAPACITY, the total alone is reported
+    }
+    ctl[RS_FILL] = ok ? ctl[RS_PAIRS] : 0;
+    ctl[RS_OK] = ok;
+    status2[0] = total;
+    status2[1] = np;
+}
+__global__ void k_range_offsets_dev(const long long* __restrict__ leaf_off, const long long* __restrict__ point_off, int nq,
+                                    const long long* __restrict__ ctl, int* __restrict__ offsets) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i <= nq) offsets[i] = ctl[RS_OK] ? (int)point_off[leaf_off[i]] : 0;
+}
+
+// Exclusive prefix sum whose length lives in device memory: out[0 .. n] with out[n] the total, n = *len.  CUB's scans take a host
+// count, and scanning the whole capacity would make every call pay for the workspace rather than for the answer.  A fixed grid
+// of gridDim.x blocks splits [0, n) into contiguous chunks: (1) each block sums its chunk, (2) one block scans the partial sums,
+// (3) each block scans its chunk from its partial.  Integer sums: the result equals CUB's ExclusiveSum exactly.
+constexpr int DSCAN_THREADS = 256;
+using DScanReduce = cub::BlockReduce<long long, DSCAN_THREADS>;
+using DScanBlock = cub::BlockScan<long long, DSCAN_THREADS>;
+__device__ __forceinline__ void dscan_chunk(long long n, long long& lo, long long& hi) {
+    const long long per = (n + gridDim.x - 1) / gridDim.x;
+    lo = min(n, (long long)blockIdx.x * per);
+    hi = min(n, lo + per);
+}
+__global__ void __launch_bounds__(DSCAN_THREADS) k_dscan_reduce(const long long* __restrict__ in, const long long* __restrict__ len,
+                                                                long long* __restrict__ part) {
+    __shared__ typename DScanReduce::TempStorage tmp;
+    long long lo, hi;
+    dscan_chunk(*len, lo, hi);
+    long long s = 0;
+    for (long long i = lo + threadIdx.x; i < hi; i += DSCAN_THREADS) s += in[i];
+    s = DScanReduce(tmp).Sum(s);
+    if (threadIdx.x == 0) part[blockIdx.x] = s;
+}
+// one block: part[0 .. nb) becomes its exclusive scan, part[nb] the total
+__global__ void __launch_bounds__(DSCAN_THREADS) k_dscan_partials(long long* __restrict__ part, int nb) {
+    __shared__ typename DScanBlock::TempStorage tmp;
+    long long carry = 0;
+    for (int base = 0; base < nb; base += DSCAN_THREADS) {
+        const int i = base + threadIdx.x;
+        long long y, tile;
+        DScanBlock(tmp).ExclusiveSum(i < nb ? part[i] : 0ll, y, tile);
+        if (i < nb) part[i] = carry + y;
+        carry += tile;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) part[nb] = carry;
+}
+__global__ void __launch_bounds__(DSCAN_THREADS) k_dscan_down(const long long* __restrict__ in, const long long* __restrict__ len,
+                                                              const long long* __restrict__ part, long long* __restrict__ out) {
+    __shared__ typename DScanBlock::TempStorage tmp;
+    const long long n = *len;
+    long long lo, hi;
+    dscan_chunk(n, lo, hi);
+    long long carry = part[blockIdx.x];
+    for (long long base = lo; base < hi; base += DSCAN_THREADS) {       // block-uniform trip count
+        const long long i = base + threadIdx.x;
+        long long y, tile;
+        DScanBlock(tmp).ExclusiveSum(i < hi ? in[i] : 0ll, y, tile);
+        if (i < hi) out[i] = carry + y;
+        carry += tile;
+        __syncthreads();
+    }
+    if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) out[n] = part[gridDim.x];
+}
+
 // ============================================================================= host
 static inline int blocks_for(long long threads, int block, int cap = 132 * 16) {      // 16 blocks on each of the H100 SXM's 132 SMs
     long long b = (threads + block - 1) / block;
@@ -856,6 +998,8 @@ Map::~Map() {
     cub_tmp_.release(); scratch_.release(); scratch2_.release(); scratch3_.release();
     rs_q_.release(); rs_lcnt_.release(); rs_loff_.release(); rs_pairs_.release(); rs_pcnt_.release(); rs_poff_.release(); rs_out_.release(); rs_offsets_.release();
     if (h_counters_) cudaFreeHost(h_counters_);
+    if (ev_front_) cudaEventDestroy(ev_front_);
+    if (ev_caller_) cudaEventDestroy(ev_caller_);
     if (stream_) cudaStreamDestroy(stream_);
 }
 
@@ -863,6 +1007,8 @@ int Map::init() {
     FL_CUDA(cudaSetDevice(device_));
     FL_CUDA(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
     FL_CUDA(cudaDeviceGetAttribute(&n_sm_, cudaDevAttrMultiProcessorCount, device_));
+    FL_CUDA(cudaEventCreateWithFlags(&ev_front_, cudaEventDisableTiming));
+    FL_CUDA(cudaEventCreateWithFlags(&ev_caller_, cudaEventDisableTiming));
     FL_CHECK(counters_.reserve(sizeof(int) * C_COUNT));
     FL_CUDA(cudaMemsetAsync(counters_.ptr, 0, sizeof(int) * C_COUNT, stream_));
     FL_CUDA(cudaMallocHost(&h_counters_, sizeof(int) * C_COUNT));
@@ -1304,6 +1450,190 @@ int Map::range_search(bool radius,const float* queries, int nq, int* out_offsets
     FL_CUDA(cudaStreamSynchronize(stream_));
     if (total) *total = n;
     return FL_OK;
+}
+
+// ----------------------------------------------------------------------------- device-buffer forms
+// true: p is device memory of `device` (or managed memory allocated against it), aligned to `align` bytes
+static bool device_ptr(const void* p, int device, size_t align) {
+    if (!p || (reinterpret_cast<uintptr_t>(p) % align) != 0) return false;
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
+    return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == device;
+}
+
+// Outside stream capture the caller's stream first waits for everything enqueued on the handle's stream (a filter run, a
+// mutation); the event is recorded anew only when that stream may have received work since the last query (touch()), so
+// queries on two caller streams do not wait for each other.  While `st` is capturing nothing is joined.
+int Map::query_begin(cudaStream_t st, bool* joined) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    FL_CUDA(cudaStreamGetCaptureInfo(st, &cs));
+    *joined = cs == cudaStreamCaptureStatusNone;
+    if (!*joined) return FL_OK;
+    if (front_stale_) { FL_CUDA(cudaEventRecord(ev_front_, stream_)); front_stale_ = false; }
+    FL_CUDA(cudaStreamWaitEvent(st, ev_front_, 0));
+    return FL_OK;
+}
+// ... and afterwards the handle's stream waits for the query, so no later mutation overwrites the map under it
+int Map::query_end(cudaStream_t st, bool joined) {
+    FL_CUDA(cudaGetLastError());
+    if (!joined) return FL_OK;
+    FL_CUDA(cudaEventRecord(ev_caller_, st));
+    FL_CUDA(cudaStreamWaitEvent(stream_, ev_caller_, 0));
+    return FL_OK;
+}
+// a synchronous call that reads caller device memory: its work on the handle's stream starts after what `st` holds
+int Map::wait_for_caller(cudaStream_t st, const char* what) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    FL_CUDA(cudaStreamGetCaptureInfo(st, &cs));
+    if (cs != cudaStreamCaptureStatusNone) { set_last_error("%s: synchronous, cannot be called on a capturing stream", what); return FL_ERR_ARG; }
+    FL_CUDA(cudaEventRecord(ev_caller_, st));
+    FL_CUDA(cudaStreamWaitEvent(stream_, ev_caller_, 0));
+    return FL_OK;
+}
+
+int Map::build_from_caller(const float* d_pts_xyzi, int n, cudaStream_t st) {
+    if (n < 0 || (n > 0 && !device_ptr(d_pts_xyzi, device_, 16))) {
+        set_last_error("build_device: n < 0, or the points are not 16-byte aligned device memory on device %d", device_);
+        return FL_ERR_ARG;
+    }
+    FL_CUDA(cudaSetDevice(device_));
+    FL_CHECK(wait_for_caller(st, "build_device"));
+    return build_device(reinterpret_cast<const float4*>(d_pts_xyzi), n);
+}
+
+int Map::add_points_from_caller(const float* d_pts_xyzi, int n, bool downsample_on, cudaStream_t st, int* added) {
+    if (added) *added = 0;
+    if (n < 0 || (n > 0 && !device_ptr(d_pts_xyzi, device_, 16))) {
+        set_last_error("add_points_device: n < 0, or the points are not 16-byte aligned device memory on device %d", device_);
+        return FL_ERR_ARG;
+    }
+    if (n == 0) return FL_OK;
+    FL_CUDA(cudaSetDevice(device_));
+    FL_CHECK(wait_for_caller(st, "add_points_device"));
+    return add_points_device(reinterpret_cast<const float4*>(d_pts_xyzi), n, downsample_on, added);
+}
+
+int Map::nearest_search_device(const float* q_xyzi, int nq, int k, float max_dist, float* out_pts, float* out_d2, int* out_cnt, cudaStream_t st) {
+    if (nq < 0 || k < 1 || k > KNN_KMAX) { set_last_error("nearest_search_device: k must be in [1, %d]", KNN_KMAX); return FL_ERR_ARG; }
+    if (nq > 0 && (!device_ptr(q_xyzi, device_, 16) || !device_ptr(out_pts, device_, 16) || !device_ptr(out_d2, device_, 4) ||
+                   !device_ptr(out_cnt, device_, 4))) {
+        set_last_error("nearest_search_device: every buffer must be device memory on device %d (queries and points 16-byte aligned)", device_);
+        return FL_ERR_ARG;
+    }
+    if (nq == 0) return FL_OK;
+    FL_CUDA(cudaSetDevice(device_));
+    const float md2 = max_dist * max_dist;                 // float32, as ikd_Tree.cpp:1067
+    const float4* q = reinterpret_cast<const float4*>(q_xyzi);
+    float4* p = reinterpret_cast<float4*>(out_pts);
+    bool joined = false;
+    FL_CHECK(query_begin(st, &joined));
+    if (k <= KNN_K) k_knn_batch_gated<<<blocks_for(nq, 128, 1 << 20), 128, 0, st>>>(v_, q, nq, k, md2, p, out_d2, out_cnt);
+    else k_knn_k<<<resident_blocks(k_knn_k, 256, (long long)nq * 32, n_sm_), 256, 0, st>>>(v_, q, nq, k, md2, p, out_d2, out_cnt);
+    return query_end(st, joined);
+}
+
+// The one layout of a range query's workspace: byte offsets from the first 256-byte boundary of the caller's buffer.
+int Map::range_workspace(int nq, long long max_pairs, RangeWorkspace& w) const {
+    size_t cub_bytes = 0;
+    FL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, (long long*)nullptr, (long long*)nullptr, (long long)nq + 1));
+    range_layout(nq, max_pairs, cub_bytes, w);
+    return FL_OK;
+}
+void Map::range_layout(int nq, long long max_pairs, size_t cub_bytes, RangeWorkspace& w) const {
+    size_t at = 0;
+    auto take = [&at](size_t bytes) { const size_t o = at; at = (at + bytes + 255) & ~(size_t)255; return o; };
+    w.q = take(sizeof(float) * 6 * (size_t)nq);                     // a copy of the queries (boxes or spheres), 16-byte aligned
+    w.lcnt = take(sizeof(long long) * ((size_t)nq + 1));            // candidate leaves per query
+    w.loff = take(sizeof(long long) * ((size_t)nq + 1));            // their offsets; loff[nq] = the pairs needed
+    w.ctl = take(sizeof(long long) * RS_CTL_COUNT);
+    w.part = take(sizeof(long long) * ((size_t)scan_blocks() + 1)); // partial sums of the device-length scan
+    w.cub = take(cub_bytes);
+    w.cub_bytes = cub_bytes;
+    w.pairs = take(sizeof(int2) * (size_t)max_pairs);               // (query, leaf)
+    w.pcnt = take(sizeof(long long) * (size_t)max_pairs);           // points per pair
+    w.poff = take(sizeof(long long) * ((size_t)max_pairs + 1));     // their offsets
+    w.bytes = at + 256;                                             // room to align the caller's pointer
+}
+
+int Map::range_workspace_bytes(int nq, long long max_pairs, unsigned long long* out) const {
+    if (nq < 0 || max_pairs < 0 || max_pairs > (1ll << 40) || !out) { set_last_error("range_workspace_bytes: bad arguments"); return FL_ERR_ARG; }
+    FL_CUDA(cudaSetDevice(device_));
+    RangeWorkspace w;
+    FL_CHECK(range_workspace(nq, max_pairs, w));
+    *out = w.bytes;
+    return FL_OK;
+}
+
+int Map::range_search_device(bool radius, const float* queries, int nq, int* out_offsets, float* out_xyzi, long long cap,
+                             void* workspace, unsigned long long workspace_bytes, long long* status2, cudaStream_t st) {
+    const char* what = radius ? "radius_search_device" : "box_search_device";
+    if (nq < 0 || cap < 0) { set_last_error("%s: negative size", what); return FL_ERR_ARG; }
+    if (!device_ptr(out_offsets, device_, 4) || !device_ptr(status2, device_, 8) || (nq > 0 && !device_ptr(queries, device_, 4)) ||
+        (nq > 0 && !device_ptr(workspace, device_, 1)) || (cap > 0 && !device_ptr(out_xyzi, device_, 16))) {
+        set_last_error("%s: every buffer must be device memory on device %d (points 16-byte aligned)", what, device_);
+        return FL_ERR_ARG;
+    }
+    FL_CUDA(cudaSetDevice(device_));
+    RangeWorkspace w;
+    long long max_pairs = 0;
+    if (nq > 0) {                       // the most pairs the workspace holds
+        FL_CHECK(range_workspace(nq, 0, w));
+        if (workspace_bytes < w.bytes) {
+            set_last_error("%s: a workspace of %llu bytes is below the %zu that %d queries need", what, workspace_bytes, w.bytes, nq);
+            return FL_ERR_ARG;
+        }
+        // 24 bytes per pair; the 256-byte rounding of the three per-pair arrays moves the size by less than 64 pairs' worth
+        const long long est = (long long)std::min<unsigned long long>((workspace_bytes - w.bytes) / (sizeof(int2) + 2 * sizeof(long long)), 1ull << 40);
+        for (max_pairs = est + 64; max_pairs > 0; max_pairs--) {
+            range_layout(nq, max_pairs, w.cub_bytes, w);
+            if (w.bytes <= workspace_bytes) break;
+        }
+        range_layout(nq, max_pairs, w.cub_bytes, w);
+    }
+    bool joined = false;
+    FL_CHECK(query_begin(st, &joined));
+    if (nq == 0) {
+        FL_CUDA(cudaMemsetAsync(out_offsets, 0, sizeof(int), st));
+        FL_CUDA(cudaMemsetAsync(status2, 0, 2 * sizeof(long long), st));
+        return query_end(st, joined);
+    }
+    char* base = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
+    float* d_q = reinterpret_cast<float*>(base + w.q);
+    long long* lcnt = reinterpret_cast<long long*>(base + w.lcnt);
+    long long* loff = reinterpret_cast<long long*>(base + w.loff);
+    long long* ctl = reinterpret_cast<long long*>(base + w.ctl);
+    long long* part = reinterpret_cast<long long*>(base + w.part);
+    int2* pairs = reinterpret_cast<int2*>(base + w.pairs);
+    long long* pcnt = reinterpret_cast<long long*>(base + w.pcnt);
+    long long* poff = reinterpret_cast<long long*>(base + w.poff);
+    float4* out = reinterpret_cast<float4*>(out_xyzi);
+    FL_CUDA(cudaMemcpyAsync(d_q, queries, sizeof(float) * (radius ? 4 : 6) * (size_t)nq, cudaMemcpyDeviceToDevice, st));
+    // 1. candidate leaves per query and their offsets (CUB over the host-known nq + 1); loff[nq] = the pairs needed
+    FL_CUDA(cudaMemsetAsync(lcnt + nq, 0, sizeof(long long), st));
+    FL_CHECK(radius ? launch_range_leaves<true>(v_, d_q, nq, lcnt, nullptr, nullptr, n_sm_, st)
+                    : launch_range_leaves<false>(v_, d_q, nq, lcnt, nullptr, nullptr, n_sm_, st));
+    size_t cub_bytes = w.cub_bytes;
+    FL_CUDA(cub::DeviceScan::ExclusiveSum(base + w.cub, cub_bytes, lcnt, loff, (long long)nq + 1, st));
+    k_range_plan<<<1, 1, 0, st>>>(loff, nq, max_pairs, ctl);
+    // 2. the pairs (only when they all fit), the points of each, their offsets by the device-length scan
+    const int lb = resident_blocks(radius ? k_range_leaves_bounded<true> : k_range_leaves_bounded<false>, 256, (long long)nq * 32, n_sm_);
+    if (radius) k_range_leaves_bounded<true><<<lb, 256, 0, st>>>(v_, d_q, nq, loff, pairs, max_pairs);
+    else k_range_leaves_bounded<false><<<lb, 256, 0, st>>>(v_, d_q, nq, loff, pairs, max_pairs);
+    const int cb = resident_blocks(radius ? k_range_count_dev<true> : k_range_count_dev<false>, 256, max_pairs * 32, n_sm_);
+    if (radius) k_range_count_dev<true><<<cb, 256, 0, st>>>(v_, d_q, pairs, ctl + RS_PAIRS, pcnt);
+    else k_range_count_dev<false><<<cb, 256, 0, st>>>(v_, d_q, pairs, ctl + RS_PAIRS, pcnt);
+    k_dscan_reduce<<<scan_blocks(), DSCAN_THREADS, 0, st>>>(pcnt, ctl + RS_PAIRS, part);
+    k_dscan_partials<<<1, DSCAN_THREADS, 0, st>>>(part, scan_blocks());
+    k_dscan_down<<<scan_blocks(), DSCAN_THREADS, 0, st>>>(pcnt, ctl + RS_PAIRS, part, poff);
+    // 3. the status words, the CSR offsets, the first `cap` points
+    k_range_status<<<1, 1, 0, st>>>(loff, poff, nq, max_pairs, ctl, status2);
+    k_range_offsets_dev<<<(nq + 256) / 256, 256, 0, st>>>(loff, poff, nq, ctl, out_offsets);
+    if (cap > 0) {
+        const int fb = resident_blocks(radius ? k_range_fill_dev<true> : k_range_fill_dev<false>, 256, max_pairs * 32, n_sm_);
+        if (radius) k_range_fill_dev<true><<<fb, 256, 0, st>>>(v_, d_q, pairs, ctl + RS_FILL, poff, out, cap);
+        else k_range_fill_dev<false><<<fb, 256, 0, st>>>(v_, d_q, pairs, ctl + RS_FILL, poff, out, cap);
+    }
+    return query_end(st, joined);
 }
 
 int Map::rebuild() {

@@ -1,6 +1,7 @@
 // Host-side owner of the device point map (the H100 counterpart of KD_TREE<PointType>,
 // reference include/ikd-Tree/ikd_Tree.h:48-341).  All methods return fl::Status.
 #pragma once
+#include <algorithm>
 #include <vector>
 
 #include "map.cuh"
@@ -43,6 +44,17 @@ public:
     // (:470-475, radius = true; queries: nq x (x, y, z, r)), batched.  Host buffers.  The points of query i are
     // out_xyzi[out_offsets[i] .. out_offsets[i + 1]) (only the first `cap` of all are written); *total = out_offsets[nq].
     int range_search(bool radius, const float* queries, int nq, int* out_offsets, float* out_xyzi, int cap, long long* total);
+
+    // Device-buffer forms (fl_map_*_device): stream-ordered on the caller's stream `st`, no host synchronisation, capturable.
+    int nearest_search_device(const float* q_xyzi, int nq, int k, float max_dist, float* out_pts, float* out_d2, int* out_cnt, cudaStream_t st);
+    int range_workspace_bytes(int nq, long long max_pairs, unsigned long long* out) const;
+    int range_search_device(bool radius, const float* queries, int nq, int* out_offsets, float* out_xyzi, long long cap,
+                            void* workspace, unsigned long long workspace_bytes, long long* status2, cudaStream_t st);
+    // Build / Add_Points from caller device memory, read in order on `st` (synchronous, like the host forms)
+    int build_from_caller(const float* d_pts_xyzi, int n, cudaStream_t st);
+    int add_points_from_caller(const float* d_pts_xyzi, int n, bool downsample_on, cudaStream_t st, int* added);
+    // every call that may enqueue work on the handle's stream marks it, so the next device query joins that work
+    void touch() { front_stale_ = true; }
     // re-sort every valid point into fresh, evenly filled leaves (ikd-Tree's Rebuild, ikd_Tree.cpp:736-764)
     int rebuild();
     // re-list every live slot in the hashed cell directory (map.cuh); done by build / rebuild, and when inserts crowd it
@@ -70,6 +82,15 @@ public:
     float rebuild_overflow_frac_ = 0.05f;   // rebuild when overflow leaves exceed this fraction of main leaves
 
 private:
+    // workspace of a device-buffer range query: byte offsets from its first 256-byte boundary (range_workspace)
+    struct RangeWorkspace { size_t q, lcnt, loff, ctl, part, cub, cub_bytes, pairs, pcnt, poff, bytes; };
+    int range_workspace(int nq, long long max_pairs, RangeWorkspace& w) const;
+    void range_layout(int nq, long long max_pairs, size_t cub_bytes, RangeWorkspace& w) const;
+    int scan_blocks() const { return 2 * std::max(n_sm_, 1); }      // grid of the device-length scan
+    int query_begin(cudaStream_t st, bool* joined);
+    int query_end(cudaStream_t st, bool joined);
+    int wait_for_caller(cudaStream_t st, const char* what);
+
     int ensure_capacity(int n_points);
     int build_from_sorted(const float4* d_src, int n);
     int insert_device(const float4* d_pts, int n);
@@ -96,6 +117,10 @@ private:
     DeviceBuffer rs_q_, rs_lcnt_, rs_loff_, rs_pairs_, rs_pcnt_, rs_poff_, rs_out_, rs_offsets_;
     int n_sm_ = 0;                  // multiprocessors of the device (grid sizing)
     int* h_counters_ = nullptr;     // pinned mirror of the device counters
+    // device-buffer queries: ev_front_ marks the handle's stream for callers to wait on (re-recorded when front_stale_),
+    // ev_caller_ a caller's stream for the handle's stream to wait on
+    cudaEvent_t ev_front_ = nullptr, ev_caller_ = nullptr;
+    bool front_stale_ = true;
 };
 
 }  // namespace fl

@@ -114,6 +114,51 @@ int fl_map_flatten(fl_map_t* m, float* out_xyzi, int cap);
  * radius and an empty or inverted box find nothing. */
 int fl_map_box_search(fl_map_t* m, const float* boxes6, int nb, int* out_offsets, float* out_xyzi, int cap);
 int fl_map_radius_search(fl_map_t* m, const float* centers_xyzr, int nq, int* out_offsets, float* out_xyzi, int cap);
+
+/* ---- device-buffer forms of the queries and of Build / Add_Points
+ * Every *_device pointer is device memory on the map's device (or managed memory allocated against it); point and query
+ * buffers of 4 floats are 16-byte aligned.  `stream` is a cudaStream_t passed as void* (NULL: the legacy default stream).
+ * The queries return an enqueue status (FL_OK, FL_ERR_ARG, FL_ERR_CUDA); their answers stay on the device and are complete
+ * when `stream` reaches them.  They never synchronise the host, allocate, or size a launch from a value produced on the
+ * device, so they may be captured into a CUDA graph.  A host pointer, a pointer to another device, a null buffer with
+ * nq > 0 or a misaligned one returns FL_ERR_ARG before anything is enqueued.
+ * Ordering: outside stream capture a query first waits for everything already enqueued on the handle's stream (a
+ * fl_filter_run still in flight, a scan step, a mutation), and the handle's stream then waits for the query, so a later
+ * Add_Points, Delete_Point_Boxes, rebuild or filter launch does not overwrite the map under it.  Two queries on two caller
+ * streams with no other call on the handle between them do not wait for each other.  While `stream` is capturing, the
+ * call joins nothing: the caller orders replays against mutations ("mutators must not overlap searches"), and a captured
+ * graph holds the map's layout of capture time, so capture again after any call that changes the map. */
+/* KD_TREE::Nearest_Search(point, k_nearest, Nearest_Points, Point_Distance, max_dist), batched, on device buffers
+ *                                                                    ikd_Tree.cpp:426-461, Search :1062-1244
+ * Writes exactly the bytes fl_map_nearest_search returns for the same map and queries: points, d2, counts, the (0, 0, 0, 0) /
+ * +inf padding; a non-finite query and a NaN max_dist find nothing.  fl_map_dir_stats counts its walked queries the same way.
+ * k <= 5 runs fl_map_knn's search with the non-finite queries moved to the origin and the cut at md2 on the device;
+ * 6 <= k <= 32 the one-warp-per-query search.  k outside [1, 32] is FL_ERR_ARG; nq = 0 writes nothing. */
+int fl_map_nearest_search_device(fl_map_t* m, const float* q_xyzi_device, int nq, int k, float max_dist,
+                                 float* out_pts_device, float* out_d2_device, int* out_cnt_device, void* stream);
+/* Bytes of caller-provided workspace for a range query of nq queries and up to max_pairs (query, main leaf) pairs.  The only
+ * sizing rule: a workspace of W bytes holds the largest max_pairs whose size is <= W. */
+int fl_map_range_workspace_bytes(fl_map_t* m, int nq, long long max_pairs, unsigned long long* out_bytes);
+/* KD_TREE::Box_Search / Radius_Search, batched, on device buffers     ikd_Tree.cpp:464-475 (Search_by_range :1247-1289,
+ * Search_by_radius :1292-1332).  The rules, the offsets and the points (in the same order) of fl_map_box_search /
+ * fl_map_radius_search.  status2_device[1] always receives the number of (query, leaf) pairs needed; status2_device[0]:
+ *   -1            the pairs did not fit the workspace: the offsets are all zero and no point is written;
+ *   > INT_MAX     the total (the counterpart of FL_ERR_CAPACITY): the offsets are all zero and no point is written;
+ *   otherwise     the total: out_offsets[nb + 1] is written in full and at most cap points (out_xyzi may be NULL when cap = 0).
+ * Read the status when convenient and retry with a larger workspace or cap.  Nothing outside the given buffers is written.
+ * nb = 0 writes out_offsets[0] = 0 and status (0, 0).  The workspace is the caller's (the handle's scratch is not used), and
+ * a workspace may not be shared by two queries in flight. */
+int fl_map_box_search_device(fl_map_t* m, const float* boxes6_device, int nb, int* out_offsets_device, float* out_xyzi_device,
+                             long long cap, void* workspace_device, unsigned long long workspace_bytes, long long* status2_device,
+                             void* stream);
+int fl_map_radius_search_device(fl_map_t* m, const float* centers_xyzr_device, int nq, int* out_offsets_device, float* out_xyzi_device,
+                                long long cap, void* workspace_device, unsigned long long workspace_bytes, long long* status2_device,
+                                void* stream);
+/* KD_TREE::Build / Add_Points from device memory                      ikd_Tree.cpp:409-423 / :478-573
+ * Synchronous, with the return values of fl_map_build / fl_map_add_points; the input is read after the work already
+ * enqueued on `stream`, and may be reused when the call returns.  Cannot be called on a capturing stream (FL_ERR_ARG). */
+int fl_map_build_device(fl_map_t* m, const float* pts_xyzi_device, int n, void* stream);
+int fl_map_add_points_device(fl_map_t* m, const float* pts_xyzi_device, int n, int downsample_on, void* stream);
 /* KD_TREE::tree_range()                                              ikd_Tree.cpp:100-137 */
 int fl_map_tree_range(fl_map_t* m, float* box6);
 /* KD_TREE::Rebuild of the whole tree (ikd_Tree.cpp:736-764): re-sorts all valid points into fresh leaves */
