@@ -82,11 +82,17 @@ public:
     float rebuild_overflow_frac_ = 0.05f;   // rebuild when overflow leaves exceed this fraction of main leaves
 
 private:
-    // workspace of a device-buffer range query: byte offsets from its first 256-byte boundary (range_workspace)
-    struct RangeWorkspace { size_t q, lcnt, loff, ctl, part, cub, cub_bytes, pairs, pcnt, poff, bytes; };
+    // workspace of a range query: byte offsets from its first 256-byte boundary (range_workspace), room for max_pairs pairs
+    struct RangeWorkspace { size_t q, lcnt, loff, ctl, part, cub, cub_bytes, pairs, pcnt, poff, bytes; long long max_pairs; };
     int range_workspace(int nq, long long max_pairs, RangeWorkspace& w) const;
     void range_layout(int nq, long long max_pairs, size_t cub_bytes, RangeWorkspace& w) const;
     int scan_blocks() const { return 2 * std::max(n_sm_, 1); }      // grid of the device-length scan
+    // the two stages of every range query, enqueued on `st` over the workspace at `base`: count (writes status2), then emit
+    int range_count(bool radius, int nq, const RangeWorkspace& w, char* base, long long* status2, cudaStream_t st);
+    int range_emit(bool radius, int nq, const RangeWorkspace& w, char* base, int* out_offsets, float4* out, long long cap, cudaStream_t st);
+    // the kernel and grid of every nearest search; knn_host runs it on host buffers
+    void launch_knn(bool gated, const float4* q, int nq, int k, float md2, float4* p, float* d2, int* cnt, cudaStream_t st);
+    int knn_host(bool gated, const float* q_xyzi, int nq, int k, float md2, float* out_pts, float* out_d2, int* out_cnt);
     int query_begin(cudaStream_t st, bool* joined);
     int query_end(cudaStream_t st, bool joined);
     int wait_for_caller(cudaStream_t st, const char* what);
@@ -113,8 +119,9 @@ private:
     DeviceBuffer ebox_[MAX_LEVELS];
     DeviceBuffer segid_, segtab_[2], bbox_;        // k-d partition build scratch
     DeviceBuffer src_, keys_in_, keys_out_, vals_in_, vals_out_, cub_tmp_, scratch_, scratch2_, scratch3_;
-    // range search: queries, per-query leaf counts / offsets, (query, leaf) pairs, per-pair point counts / offsets, output
-    DeviceBuffer rs_q_, rs_lcnt_, rs_loff_, rs_pairs_, rs_pcnt_, rs_poff_, rs_out_, rs_offsets_;
+    // host-buffer range search: the workspace (laid out for range_ws_pairs_ pairs, the most of any call so far) and status2 + output
+    DeviceBuffer range_ws_, range_out_;
+    long long range_ws_pairs_ = 0;
     int n_sm_ = 0;                  // multiprocessors of the device (grid sizing)
     int* h_counters_ = nullptr;     // pinned mirror of the device counters
     // device-buffer queries: ev_front_ marks the handle's stream for callers to wait on (re-recorded when front_stale_),

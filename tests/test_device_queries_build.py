@@ -82,7 +82,9 @@ def test_new_kernels_do_not_spill(map_cubin):
     assert by(r"k_range_leaves_boundedILb1") <= by(r"k_range_leavesILb1") + 8
 
 
-def test_existing_kernels_compile_to_the_same_sass(map_cubin):
+def test_kept_kernels_compile_to_the_same_sass(map_cubin):
+    """k_knn_batch, k_knn_k and k_range_leaves, whose bodies the device-buffer queries reuse, compile to the SASS recorded
+    before those queries were added."""
     want = json.load(open(os.path.join(ROOT, "tests", "golden", "sass_existing_kernels_sm90a.json")))
     if map_cubin[2] != want["nvcc"]:
         pytest.skip(f"digests recorded with nvcc {want['nvcc']}, this is {map_cubin[2]}")
@@ -90,3 +92,11 @@ def test_existing_kernels_compile_to_the_same_sass(map_cubin):
     for name, digest in want["functions"].items():
         assert name in got, name
         assert hashlib.sha256("\n".join(got[name]).encode()).hexdigest() == digest, name
+
+
+def test_host_range_search_has_no_kernels_of_its_own(map_cubin):
+    """The host-buffer range search runs the device-buffer pipeline: its former kernels are gone from the cubin."""
+    names = sass_functions(map_cubin[1])
+    gone = [n for n in names if re.search(r"k_range_(count|fill)ILb|k_range_offsetsE", n)]
+    assert not gone, gone
+    assert any("k_range_count_dev" in n for n in names) and any("k_range_offsets_dev" in n for n in names)
