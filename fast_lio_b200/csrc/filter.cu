@@ -971,14 +971,18 @@ __global__ void __launch_bounds__(RESID_THREADS) k_residual(ScanView sc, FilterC
 // The pass that ends the update stores the result (header, state, covariance) straight into the caller-visible
 // page-locked mirror over PCIe: the host then only waits for the stream instead of queueing a device-to-host copy
 // behind the last kernel.  Block-wide; the block's own writes to ctl are visible after the barrier.
-__device__ __forceinline__ void mirror_result(const FilterCtl* ctl) {
-    __syncthreads();
+// mirror_copy: the copy alone, by threads 0 .. nthreads-1, after the caller's barrier.
+__device__ __forceinline__ void mirror_copy(const FilterCtl* ctl, int nthreads) {
     if (!ctl->done || !ctl->host_mirror) return;
     constexpr int ND = (int)(offsetof(FilterCtl, P_prop) / sizeof(double));
     static_assert(offsetof(FilterCtl, P_prop) % sizeof(double) == 0, "mirror copies 8-byte words");
     const double* src = reinterpret_cast<const double*>(ctl);
     double* dst = reinterpret_cast<double*>(ctl->host_mirror);
-    for (int i = threadIdx.x; i < ND; i += blockDim.x) dst[i] = src[i];
+    for (int i = threadIdx.x; i < ND; i += nthreads) dst[i] = src[i];
+}
+__device__ __forceinline__ void mirror_result(const FilterCtl* ctl) {
+    __syncthreads();
+    mirror_copy(ctl, blockDim.x);
 }
 
 // multi-GPU: the Kalman step from the all-reduced sums
@@ -1141,11 +1145,15 @@ int Filter::init() {
     else FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_search<4>, SEARCH_THREADS, 0));
     search_grid_max_ = sms_ * std::max(1, occ);
     if (const char* e = getenv("FASTLIO_B200_LEGACY")) fused_ = !(e[0] == '1');      // A/B: the split kernels of round 1
-    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update<false>, UPD_THREADS, 0));
-    upd_capacity_[0] = sms_ * std::max(1, occ);
-    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update<true>, UPD_THREADS, 0));
-    upd_capacity_[1] = sms_ * std::max(1, occ);
-    FL_CHECK(partials_.reserve(sizeof(double) * PSTRIDE * (size_t)std::max(upd_capacity_[0], upd_capacity_[1])));
+    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update<false, 1>, UPD_THREADS, 0));
+    upd_capacity_[0][0] = sms_ * std::max(1, occ);
+    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update<true, 1>, UPD_THREADS, 0));
+    upd_capacity_[1][0] = sms_ * std::max(1, occ);
+    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update<false, 2>, 2 * UPD_THREADS, 0));
+    upd_capacity_[0][1] = sms_ * occ;
+    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update<true, 2>, 2 * UPD_THREADS, 0));
+    upd_capacity_[1][1] = sms_ * occ;
+    FL_CHECK(partials_.reserve(sizeof(double) * PSTRIDE * (size_t)std::max(upd_capacity_[0][0], upd_capacity_[1][0])));
     max_resid_grid_ = sms_;
     FL_CHECK(partials_.reserve(sizeof(double) * PSTRIDE * (size_t)max_resid_grid_));
     FL_CHECK(reserve(std::max(1, max_points_)));
@@ -1262,11 +1270,10 @@ int Filter::complete_neighbours() {
         a.logs = logs_.as<PassLog>(); a.p2p = p2p_.as<P2PState>();
         a.mode = 0; a.max_passes = 1; a.search_only = 1; a.dbg = 0; a.pose_from_search = 1;
         a.pub = pub_.as<unsigned long long>(); a.nonce = ++launch_nonce_;
-        const int cap = upd_capacity_[extrinsic_est_ ? 1 : 0];
+        const int cap = upd_capacity_[extrinsic_est_ ? 1 : 0][0];
         const int nq = scan_.q_end - scan_.q_begin;
         const int workers = std::max(1, std::min(cap - 1, (nq + UPD_THREADS - 1) / UPD_THREADS));
-        cudaError_t e = extrinsic_est_ ? launch_pdl(k_update<true>, workers + 1, UPD_THREADS, stream(), false, a)
-                                       : launch_pdl(k_update<false>, workers + 1, UPD_THREADS, stream(), false, a);
+        cudaError_t e = launch_upd(workers, false, a, upd_pair(nq));
         if (e != cudaSuccess) { scan_.q_begin = keep_b; scan_.q_end = keep_e; set_last_error("complete_neighbours: %s", cudaGetErrorString(e)); return FL_ERR_CUDA; }
     }
     scan_.q_begin = keep_b; scan_.q_end = keep_e;
@@ -1328,14 +1335,29 @@ int Filter::launch_update(int max_passes, int mode, int search_only) {
     a.pub = pub_.as<unsigned long long>(); a.nonce = ++launch_nonce_;
     { const char* e = getenv("FASTLIO_B200_DBG"); a.dbg = e ? atoi(e) : 0; }
     a.pose_from_search = 0;
-    const int cap = upd_capacity_[extrinsic_est_ ? 1 : 0];
+    const int cap = upd_capacity_[extrinsic_est_ ? 1 : 0][0];
     // every co-resident block works (a searching pass wants many warps in flight); small scans: at least 4 points per warp
     // one thread per point: full warps (the search is bound by a thread's own chain of loads, not by the number of SMs)
     int workers = mode == 3 ? 0 : std::min(cap - 1, (nq + UPD_THREADS - 1) / UPD_THREADS);
     if (workers < 0) workers = 0;
-    if (extrinsic_est_) FL_CUDA(launch_pdl(k_update<true>, workers + 1, UPD_THREADS, stream(), pdl_, a));
-    else FL_CUDA(launch_pdl(k_update<false>, workers + 1, UPD_THREADS, stream(), pdl_, a));
+    FL_CUDA(launch_upd(workers, pdl_, a, upd_pair(nq)));
     return FL_OK;
+}
+
+// Two threads per point (k_update<EXTR, 2>) when the shard's tiles all fit the co-resident 512-thread grid, so the tiles, the
+// workers and their partial rows are exactly those of the one-thread form; a larger scan keeps one thread per point rather
+// than idle half its warps on the passes that do not search.  FASTLIO_B200_PAIR=1 forces one thread per point (A/B).
+int Filter::upd_pair(int nq) const {
+    if (const char* e = getenv("FASTLIO_B200_PAIR")) if (e[0] == '1') return 1;
+    const int tiles = (nq + UPD_THREADS - 1) / UPD_THREADS;
+    return tiles >= 1 && tiles <= upd_capacity_[extrinsic_est_ ? 1 : 0][1] - 1 ? 2 : 1;
+}
+cudaError_t Filter::launch_upd(int workers, bool pdl, const UpdArgs& a, int pair) {
+    const int block = pair * UPD_THREADS;
+    if (extrinsic_est_) return pair == 2 ? launch_pdl(k_update<true, 2>, workers + 1, block, stream(), pdl, a)
+                                         : launch_pdl(k_update<true, 1>, workers + 1, block, stream(), pdl, a);
+    return pair == 2 ? launch_pdl(k_update<false, 2>, workers + 1, block, stream(), pdl, a)
+                     : launch_pdl(k_update<false, 1>, workers + 1, block, stream(), pdl, a);
 }
 
 int Filter::launch_search_only() {

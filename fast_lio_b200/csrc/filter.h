@@ -54,6 +54,7 @@ struct ScanView {
 };
 
 struct NcclApi;
+struct UpdArgs;
 
 // Peer-memory exchange of the per-pass sums (fused into k_residual's solver block): every rank owns a
 // mailbox [2 epoch parities][nranks][96] values, each two epoch-tagged 8-byte words; peers store into it over NVLink.
@@ -144,8 +145,10 @@ private:
     bool fused_ = true;
     DeviceBuffer pub_;                 // k_update's publication block
     unsigned launch_nonce_ = 0;
-    int upd_capacity_[2] = {0, 0};     // co-resident k_update<EXTR> blocks on this device
+    int upd_capacity_[2][2] = {{0, 0}, {0, 0}};   // co-resident k_update<EXTR, PAIR> blocks on this device, [EXTR][PAIR - 1]
     int launch_update(int max_passes, int mode, int search_only);
+    int upd_pair(int nq) const;                   // 2: the shard's tiles fit the 512-thread grid (two threads per point), else 1
+    cudaError_t launch_upd(int workers, bool pdl, const UpdArgs& a, int pair);
     int launches_ = 0;
     long long host_ns_[4] = {0, 0, 0, 0};
     bool shard_set_ = false;

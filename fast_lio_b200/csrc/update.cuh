@@ -108,14 +108,171 @@ __device__ __forceinline__ void pub_publish(unsigned long long* pub, unsigned ta
     }
 }
 
+// ============================================================================= paired search (PAIR = 2)
+// In a 512-thread worker block, thread t < 256 owns point tile + t exactly as in the 256-thread block, and thread t + 256 is
+// its search partner: on a searching pass both score the query's halo list, the owner its first ceil(n / 2) 8-candidate chunks
+// and the partner the rest, so each thread runs about half the dependent round trips of cell_scan_list.  Each keeps the k best
+// of its chunks in a TBest, and the owner then inserts the partner's k best, in order, into its own.  That is exactly
+// cell_scan_list's answer: TBest keeps the first of two equal distances and refuses a slot it holds, so a whole-list scan ends
+// with the k smallest distinct slots by (d2, first listing); the owner's list is that scan's state after the first half, and a
+// listing of the second half that is not among the partner's k best has k distinct slots ahead of it in that half and so cannot
+// be in the answer (tests/test_update_pair_merge.py checks the rule on the CPU).
+
+// cell_scan_list over the chunks [c0, c1) of the halo list [start, start + cnt)
+__device__ __forceinline__ void cell_scan_chunks(const MapView& m, int start, int cnt, int c0, int c1, float qx, float qy, float qz, TBest& kb) {
+    const int4* list = reinterpret_cast<const int4*>(m.dir.lists + start);
+    int4 ia = make_int4(0, 0, 0, 0), ib = make_int4(0, 0, 0, 0);
+    if (c0 < c1) {
+        ia = __ldg(&list[2 * c0]);
+        if (cnt - 8 * c0 > 4) ib = __ldg(&list[2 * c0 + 1]);
+    }
+#pragma unroll 1
+    for (int c = c0; c < c1; c++) {
+        const int n8 = cnt - 8 * c;                                            // candidates left, >= 1
+        float4 p0, p1, p2, p3, p4, p5, p6, p7;
+        p1 = p2 = p3 = p4 = p5 = p6 = p7 = make_float4(0.f, 0.f, 0.f, 0.f);  // flag 0: not a live point
+        p0 = __ldg(&m.pts[ia.x]);
+        if (n8 > 1) p1 = __ldg(&m.pts[ia.y]);
+        if (n8 > 2) p2 = __ldg(&m.pts[ia.z]);
+        if (n8 > 3) p3 = __ldg(&m.pts[ia.w]);
+        if (n8 > 4) p4 = __ldg(&m.pts[ib.x]);
+        if (n8 > 5) p5 = __ldg(&m.pts[ib.y]);
+        if (n8 > 6) p6 = __ldg(&m.pts[ib.z]);
+        if (n8 > 7) p7 = __ldg(&m.pts[ib.w]);
+        int4 na = ia, nb = ib;
+        if (c + 1 < c1) {
+            na = __ldg(&list[2 * c + 2]);
+            if (n8 > 12) nb = __ldg(&list[2 * c + 3]);
+        }
+        cell_consider(p0, ia.x, qx, qy, qz, kb);
+        cell_consider(p1, ia.y, qx, qy, qz, kb);
+        cell_consider(p2, ia.z, qx, qy, qz, kb);
+        cell_consider(p3, ia.w, qx, qy, qz, kb);
+        cell_consider(p4, ib.x, qx, qy, qz, kb);
+        cell_consider(p5, ib.y, qx, qy, qz, kb);
+        cell_consider(p6, ib.z, qx, qy, qz, kb);
+        cell_consider(p7, ib.w, qx, qy, qz, kb);
+        ia = na; ib = nb;
+    }
+}
+
+// the partner's list, handed to its owner through the owner warp's `stage` slice (unused during the search)
+struct PairXch {
+    float d[KNN_K][32];
+    int idx[KNN_K][32];
+};
+
+// The owner's merge: its TBest holds what cell_scan_list holds after the owner's chunks; the partner's entries go in after
+// them, in the partner's order, through the same insert (equal distances keep their arrival order, a held slot is refused).
+__device__ __forceinline__ void pair_merge(const PairXch& X, int lane, TBest& kb) {
+#pragma unroll
+    for (int j = 0; j < KNN_K; j++) {
+        const float d = X.d[j][lane];
+        const int i = X.idx[j][lane];
+        if (i >= 0 && d < kb.d[KNN_K - 1]) kb.insert(d, i);
+    }
+}
+
+// owner warp w and partner warp w + 8 only
+__device__ __forceinline__ void pair_sync(int warp) { asm volatile("bar.sync %0, 64;" ::"r"(1 + (warp & (UPD_WARPS - 1))) : "memory"); }
+
+// knn_block for the 512-thread block: every thread calls it; kb is the answer for owners (threadIdx.x < UPD_THREADS), the
+// partner's kb is undefined.  The thread search is the paired scan above; what it cannot prove goes through the same walk pool,
+// walked by all 16 warps, and pool overflow is walked by the owner's warp.  `stage` is the owner warp's stage slice.
+__device__ __forceinline__ void knn_block_pair(const MapView& m, bool active, float qx, float qy, float qz, TBest& kb, WalkPool& W,
+                                               int& phase, double* stage) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+    const bool owner = threadIdx.x < UPD_THREADS;
+    const CellDir& D = m.dir;
+    kb.init();
+    int ix = 0, iy = 0, iz = 0;
+    bool listed = false;                             // the query's halo list was scored (by both threads of the pair)
+    if (active && D.cap != 0u) {
+        const float inv = D.inv_cell;
+        ix = cell_coord(qx, inv); iy = cell_coord(qy, inv); iz = cell_coord(qz, inv);
+        if (!(abs(ix) >= CELL_CLAMP - 1 || abs(iy) >= CELL_CLAMP - 1 || abs(iz) >= CELL_CLAMP - 1)) {
+            int start, cnt;
+            if (cell_list(D, cell_key(ix, iy, iz), start, cnt) > 0) {
+                const int nchunks = (cnt + 7) >> 3, h = (nchunks + 1) >> 1;
+                cell_scan_chunks(m, start, cnt, owner ? 0 : h, owner ? h : nchunks, qx, qy, qz, kb);
+                listed = true;
+            }
+        }
+    }
+    PairXch& X = *reinterpret_cast<PairXch*>(stage);
+    pair_sync(warp);                                 // the owner warp is done with its stage slice (previous tile)
+    if (!owner) {
+#pragma unroll
+        for (int j = 0; j < KNN_K; j++) { X.d[j][lane] = kb.d[j]; X.idx[j][lane] = kb.idx[j]; }
+    }
+    pair_sync(warp);
+    bool exact = true;
+    if (owner && active) {
+        exact = false;
+        if (listed) {
+            pair_merge(X, lane, kb);
+            if (kb.idx[KNN_K - 1] >= 0) {
+                const float g = cell_block_dist(D, qx, qy, qz, ix, iy, iz);
+                exact = kb.d[KNN_K - 1] < g * g;
+            }
+        }
+    }
+    // from here on: knn_block's pool, with the pool filled by the owners only
+    int mine_slot = -1;
+    int* counter = &W.n[phase & 1];
+    if (owner && active && !exact) {
+        mine_slot = atomicAdd(counter, 1);
+        if (mine_slot < WALK_POOL) {
+            W.who[mine_slot] = (int)threadIdx.x; W.x[mine_slot] = qx; W.y[mine_slot] = qy; W.z[mine_slot] = qz;
+            const bool full = kb.idx[KNN_K - 1] >= 0;
+#pragma unroll
+            for (int j = 0; j < KNN_K; j++) { W.rd[mine_slot][j] = full ? kb.d[j] : INFINITY; W.ri[mine_slot][j] = full ? kb.idx[j] : -1; }
+        }
+    }
+    __syncthreads();
+    const int total = *counter, n = min(total, WALK_POOL);
+    if (threadIdx.x == 0) W.n[(phase + 1) & 1] = 0;
+    phase++;
+    for (int i = warp; i < n; i += nwarps) {
+        KBest w;
+        w.init();
+        if (lane < KNN_K) { w.d = W.rd[i][lane]; w.idx = W.ri[i][lane]; }
+        w.w = __shfl_sync(FULL, w.d, KNN_K - 1);
+        w.n = w.w < INFINITY ? KNN_K : 0;
+        knn_query_from(m, W.x[i], W.y[i], W.z[i], w, lane);
+        __syncwarp();
+        if (lane < KNN_K) { W.rd[i][lane] = w.d; W.ri[i][lane] = w.idx; }
+    }
+    unsigned todo = __ballot_sync(FULL, mine_slot >= WALK_POOL);      // partner warps never pool: todo == 0 there
+    while (todo) {
+        const int src = __ffs(todo) - 1;
+        todo &= todo - 1;
+        KBest w;
+        knn_query(m, __shfl_sync(FULL, qx, src), __shfl_sync(FULL, qy, src), __shfl_sync(FULL, qz, src), w, lane);
+#pragma unroll
+        for (int j = 0; j < KNN_K; j++) {
+            const float dj = __shfl_sync(FULL, w.d, j);
+            const int ij = __shfl_sync(FULL, w.idx, j);
+            if (lane == src) { kb.d[j] = dj; kb.idx[j] = ij; }
+        }
+    }
+    __syncthreads();
+    if (mine_slot >= 0 && mine_slot < WALK_POOL) {
+#pragma unroll
+        for (int j = 0; j < KNN_K; j++) { kb.d[j] = W.rd[mine_slot][j]; kb.idx[j] = W.ri[mine_slot][j]; }
+    }
+    if (threadIdx.x == 0 && total && m.dir.cap && m.dir.n_walked) atomicAdd(m.dir.n_walked, total);
+}
+
 // ============================================================================= workers
 // Everything of h_share_model for one scan point (laserMapping.cpp:650-692), one thread per point.  Block-collective on a
 // searching pass (the queries the directory cannot prove are walked through the BVH by all warps of the block, knn_block).  On a searching pass the five neighbours go from the search's registers
 // straight into the plane fit; they are stored once (map_incremental reads them, laserMapping.cpp:438-460).  Returns true when
-// the point contributes a row.
-template <bool EXTR>
+// the point contributes a row.  PAIR = 2: the partner threads (threadIdx.x >= UPD_THREADS) call it on searching passes only,
+// for the paired search, and return false.
+template <bool EXTR, int PAIR>
 __device__ __forceinline__ bool measure_fused(const MapView& m, const ScanView& sc, int q, bool active, const PoseS& s, bool searched,
-                                              bool search_only, WalkPool& walks, int& phase, double* h, double& z, float& absres) {
+                                              bool search_only, WalkPool& walks, int& phase, double* stage, double* h, double& z, float& absres) {
     float4 pb = make_float4(0.f, 0.f, 0.f, 0.f);
     float wx = 0.f, wy = 0.f, wz = 0.f;
     D3 p_this = d3(0.0, 0.0, 0.0);
@@ -129,7 +286,12 @@ __device__ __forceinline__ bool measure_fused(const MapView& m, const ScanView& 
     float pabcd[4] = {0.f, 0.f, 0.f, 0.f};
     if (searched) {                                                         // :667
         TBest kb;
-        knn_block(m, active, wx, wy, wz, kb, walks, phase);                        // :670 (block-wide: two barriers)
+        if constexpr (PAIR == 1) {
+            knn_block(m, active, wx, wy, wz, kb, walks, phase);                    // :670 (block-wide: two barriers)
+        } else {
+            knn_block_pair(m, active, wx, wy, wz, kb, walks, phase, stage);
+            if (threadIdx.x >= UPD_THREADS) return false;
+        }
         if (active) {
             float4 p[KNN_K];
             const int cnt = knn_fetch(m, kb, p);
@@ -171,6 +333,10 @@ __device__ __forceinline__ bool measure_fused(const MapView& m, const ScanView& 
 }
 
 // ============================================================================= solver
+// The solver runs on threads 0..255 of block 0 whatever the block size (in a 512-thread block the others leave at once), so its
+// barriers name those 256 threads.
+__device__ __forceinline__ void sol_sync() { asm volatile("bar.sync 2, 256;" ::: "memory"); }
+
 // once per launch: the control block into shared memory
 __device__ void sol_load(SolverSm& S, const FilterCtl* ctl) {
     const int tid = threadIdx.x;
@@ -182,9 +348,9 @@ __device__ void sol_load(SolverSm& S, const FilterCtl* ctl) {
         S.iter = __ldcg(&ctl->iter); S.t = __ldcg(&ctl->t); S.converge = __ldcg(&ctl->converge); S.done = __ldcg(&ctl->done);
         S.n_pass = __ldcg(&ctl->n_pass); S.max_iter = __ldcg(&ctl->max_iter); S.error = 0; S.late = 0;
     }
-    __syncthreads();
+    sol_sync();
     if (tid == 0) S2_Bx(ld3(S.xprop + X_GRAV), S.Bprop);
-    __syncthreads();
+    sol_sync();
 }
 
 // the state-only half of a pass (esekfom.hpp:1651-1699): dx = x [-] x_prop, dx_new, the congruence blocks, Pt = T P_prop T^T
@@ -217,7 +383,7 @@ __device__ void sol_prepare(SolverSm& S) {
         const double d = S.x[xo + c] - S.xprop[xo + c];
         S.dx[dof + c] = d; S.dxn[dof + c] = d;
     }
-    __syncthreads();
+    sol_sync();
     // W1 = P_prop T^T  (columns of the SO3 / S2 blocks), then Pt = T W1 (their rows): T P T^T as :1659-1699 apply it block by block
 #pragma unroll 1
     for (int e = tid; e < n * n; e += UPD_THREADS) {
@@ -233,7 +399,7 @@ __device__ void sol_prepare(SolverSm& S) {
         } else v = row[j];
         S.W1[e] = v;
     }
-    __syncthreads();
+    sol_sync();
 #pragma unroll 1
     for (int e = tid; e < n * n; e += UPD_THREADS) {
         const int i = e / n, j = e - i * n;
@@ -247,7 +413,7 @@ __device__ void sol_prepare(SolverSm& S) {
         } else v = S.W1[e];
         S.Pt[e] = v;
     }
-    __syncthreads();
+    sol_sync();
 }
 
 // fixed-order reduction of the workers' block partials into S.red
@@ -267,7 +433,7 @@ __device__ void sol_reduce(SolverSm& S, const double* __restrict__ partials, int
         for (int k = 0; k < 8; k++) { a0 += v[k][0]; a1 += v[k][1]; a2 += v[k][2]; }
     }
     S.wred[warp][lane] = a0; S.wred[warp][lane + 32] = a1; S.wred[warp][lane + 64] = a2;
-    __syncthreads();
+    sol_sync();
     if (tid < PSTRIDE) {
         double v = 0.0;
 #pragma unroll
@@ -280,13 +446,13 @@ __device__ void sol_reduce(SolverSm& S, const double* __restrict__ partials, int
             S.HTH[a * 12 + b] = v; S.HTH[b * 12 + a] = v;
         }
     }
-    __syncthreads();
+    sol_sync();
 }
 // the same expansion for sums that did not come through sol_reduce (peer exchange, NCCL)
 __device__ void sol_expand(SolverSm& S) {
     const int tid = threadIdx.x;
     if (tid < 144) { const int a = tid / 12, b = tid - a * 12; S.HTH[tid] = S.red[a <= b ? tri12(a, b) : tri12(b, a)]; }
-    __syncthreads();
+    sol_sync();
 }
 
 // all-reduce of S.red over the peer mailboxes (see k_residual / DESIGN.md section 5): every rank stores its sums into its slot
@@ -303,7 +469,7 @@ __device__ void sol_exchange(SolverSm& S, P2PState* p2p) {
         asm volatile("st.volatile.global.u64 [%0], %1;" ::"l"(dst), "l"(tag | (bits & 0xffffffffull)) : "memory");
         asm volatile("st.volatile.global.u64 [%0], %1;" ::"l"(dst + 1), "l"(tag | (bits >> 32)) : "memory");
     }
-    __syncthreads();                                  // S.red has been sent before it is overwritten with the sum
+    sol_sync();                                  // S.red has been sent before it is overwritten with the sum
     if (threadIdx.x < PSTRIDE) {
         const unsigned long long* mail = reinterpret_cast<const unsigned long long*>(p2p->peer_mail[me]) + (size_t)par * nr * PSTRIDE * 2;
         double v = 0.0;
@@ -324,7 +490,7 @@ __device__ void sol_exchange(SolverSm& S, P2PState* p2p) {
         if (late) S.late = 1;
     }
     if (threadIdx.x == 0) p2p->epoch = epoch;
-    __syncthreads();
+    sol_sync();
 }
 
 // Gauss-Jordan with partial pivoting on [A | B], ne rows, one COLUMN per lane, rows in registers.  The pivot row is scaled to a
@@ -445,7 +611,7 @@ __device__ void sol_pass(SolverSm& S, FilterCtl* ctl, PassLog* logs, unsigned lo
             pub_publish(pub, tag_next, S.x, S.converge, S.done, lane);
         }
     }
-    __syncthreads();
+    sol_sync();
     PassLog* lg = (logs && S.n_pass < MAX_LOGS) ? &logs[S.n_pass] : nullptr;
     if (S.effct < 1 || !S.ok || S.late) {
         if (tid == 0) {
@@ -456,7 +622,7 @@ __device__ void sol_pass(SolverSm& S, FilterCtl* ctl, PassLog* logs, unsigned lo
             S.n_pass++;
             ctl->iter = S.iter; ctl->n_pass = S.n_pass; ctl->done = S.done; ctl->error = S.error;
         }
-        __syncthreads();
+        sol_sync();
         return;
     }
     // ------------------------------------------------------------------ after the publication
@@ -505,7 +671,7 @@ __device__ void sol_pass(SolverSm& S, FilterCtl* ctl, PassLog* logs, unsigned lo
             S.W1[e] = S.Pt[e] - v;
         }
     }
-    __syncthreads();
+    sol_sync();
     if (tid < XLEN) { ctl->x[tid] = S.xnew[tid]; if (lg) lg->x_after[tid] = S.xnew[tid]; }
     if (tid == 32) { ctl->t = S.t; ctl->converge = S.converge; ctl->iter = S.iter + 1; ctl->n_pass = S.n_pass + 1; ctl->done = finish; }
     if (!finish) {
@@ -526,7 +692,7 @@ __device__ void sol_pass(SolverSm& S, FilterCtl* ctl, PassLog* logs, unsigned lo
             } else v = S.W1[e];
             S.Pt[e] = v;
         }
-        __syncthreads();
+        sol_sync();
 #pragma unroll 1
         for (int e = tid; e < n * n; e += UPD_THREADS) {            // columns
             const int i = e / n, j = e - i * n;
@@ -542,15 +708,21 @@ __device__ void sol_pass(SolverSm& S, FilterCtl* ctl, PassLog* logs, unsigned lo
             ctl->P[e] = v;
         }
     }
-    __syncthreads();
+    sol_sync();
     if (tid < XLEN) S.x[tid] = S.xnew[tid];
     if (tid == 32) { S.iter++; S.n_pass++; S.done = finish; }
-    __syncthreads();
+    sol_sync();
 }
 
 // ============================================================================= the kernel
-template <bool EXTR>
-__global__ void __launch_bounds__(UPD_THREADS, 2) k_update(UpdArgs a) {
+// PAIR = 1: one thread per point, 256 threads, two blocks per SM.  PAIR = 2: the same 256-point tiles, dealt the same way, with a
+// search partner per point (knn_block_pair): 512 threads, one block per SM, the same 128-register cap.  Warps 8..15 only help
+// on the searching passes and otherwise just join the block barriers; the tiles, the partial rows and every sum are those of
+// PAIR = 1, so both forms give the same bytes.
+template <bool EXTR, int PAIR>
+__global__ void __launch_bounds__(UPD_THREADS * PAIR, 3 - PAIR) k_update(UpdArgs a) {
+    static_assert(PAIR == 1 || PAIR == 2, "one or two threads per point");
+    static_assert(sizeof(PairXch) <= sizeof(double) * WorkerSm<EXTR>::STAGE, "the partner's list fits the owner warp's stage slice");
     __shared__ __align__(16) unsigned char smem_raw[sizeof(SolverSm) > sizeof(WorkerSm<EXTR>) ? sizeof(SolverSm) : sizeof(WorkerSm<EXTR>)];
     FilterCtl* ctl = a.ctl;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -602,19 +774,24 @@ __global__ void __launch_bounds__(UPD_THREADS, 2) k_update(UpdArgs a) {
                 s.offT = d3(x14[X_OFFT], x14[X_OFFT + 1], x14[X_OFFT + 2]);
             }
             double acc[3] = {0.0, 0.0, 0.0};
-            double* stage = Wk.stage[warp];
+            const bool owner = PAIR == 1 || tid < UPD_THREADS;
+            double* stage = Wk.stage[warp & (UPD_WARPS - 1)];          // a partner warp hands its lists over in its owner's slice
             // tiles of UPD_THREADS consecutive points, dealt round-robin to the worker blocks -- the same tiles every pass (a point's
             // cached neighbours, plane and flag are only ever touched by its own thread)
             const int q0 = a.sc.q_begin, q1 = a.sc.q_end;
             for (int tile = q0 + wb * UPD_THREADS; tile < q1; tile += nwork * UPD_THREADS) {
-                const int q = tile + tid;
+                const int q = tile + (tid & (UPD_THREADS - 1));
                 double h[12]; double z = 0.0; float ar = 0.f;
-                const bool contrib = measure_fused<EXTR>(a.m, a.sc, q, q < q1, s, searched, a.search_only != 0, Wk.walks, walk_phase, h, z, ar);
-                if (!a.search_only) warp_accumulate<EXTR>(contrib, h, z, ar, acc, lane, stage);
+                bool contrib = false;
+                if (owner || searched)
+                    contrib = measure_fused<EXTR, PAIR>(a.m, a.sc, q, q < q1, s, searched, a.search_only != 0, Wk.walks, walk_phase, stage, h, z, ar);
+                if (owner && !a.search_only) warp_accumulate<EXTR>(contrib, h, z, ar, acc, lane, stage);
             }
             if (a.search_only) return;
+            if (owner) {
 #pragma unroll
-            for (int j = 0; j < 3; j++) Wk.wred[warp][lane + 32 * j] = acc[j];
+                for (int j = 0; j < 3; j++) Wk.wred[warp][lane + 32 * j] = acc[j];
+            }
             __syncthreads();
             if (tid < PSTRIDE) {
                 double v = 0.0;
@@ -630,6 +807,7 @@ __global__ void __launch_bounds__(UPD_THREADS, 2) k_update(UpdArgs a) {
     }
     // ------------------------------------------------------------------ solver block
     if (a.search_only) return;
+    if (tid >= UPD_THREADS) return;                  // PAIR = 2: the solver is the first 256 threads (sol_sync)
     SolverSm& S = *reinterpret_cast<SolverSm*>(smem_raw);
     sol_load(S, ctl);
     int p = 0;
@@ -645,7 +823,7 @@ __global__ void __launch_bounds__(UPD_THREADS, 2) k_update(UpdArgs a) {
                     if (clock64() - t0 > SPIN_LIMIT) { S.late = 2; break; }
                 }
             }
-            __syncthreads();
+            sol_sync();
             if (tid == 0) ctl->prof[9] = clock64();
             sol_reduce(S, a.partials, nwork);
             if (a.mode == 1) {
@@ -655,7 +833,7 @@ __global__ void __launch_bounds__(UPD_THREADS, 2) k_update(UpdArgs a) {
             }
         } else {
             if (tid < PSTRIDE) S.red[tid] = tid < NRED ? a.red_g[tid] : 0.0;
-            __syncthreads();
+            sol_sync();
             sol_expand(S);
         }
         if (a.mode == 2) { sol_exchange(S, a.p2p); sol_expand(S); }
@@ -664,7 +842,8 @@ __global__ void __launch_bounds__(UPD_THREADS, 2) k_update(UpdArgs a) {
         if (tid == 0) ctl->prof[7] = clock64();
     }
     if (tid == 0) { ctl->error = S.error | ctl->error; ctl->ticket = 0; }
-    mirror_result(ctl);
+    sol_sync();
+    mirror_copy(ctl, UPD_THREADS);
 }
 
 }  // namespace fl
