@@ -49,6 +49,7 @@ SYMBOLS = [
     "fl_scan_create", "fl_scan_destroy", "fl_scan_upload", "fl_scan_undistort", "fl_scan_voxel_downsample", "fl_scan_download",
     "fl_filter_update_scan", "fl_localmap_create", "fl_localmap_destroy", "fl_localmap_segment", "fl_localmap_get",
     "fl_comm_unique_id", "fl_filter_comm_init", "fl_filter_set_shard", "fl_filter_p2p_handle", "fl_filter_p2p_connect",
+    "fl_filter_update_device", "fl_filter_get_nearest_device", "fl_filter_get_selected_device",
 ]
 
 
@@ -96,6 +97,9 @@ def load():
         fn.argtypes = [_vp, _vp, C.c_int, _vp, _vp, C.c_longlong, _vp, C.c_ulonglong, _vp, _vp]
     L.fl_map_build_device.argtypes = [_vp, _vp, C.c_int, _vp]
     L.fl_map_add_points_device.argtypes = [_vp, _vp, C.c_int, C.c_int, _vp]
+    L.fl_filter_update_device.argtypes = [_vp, _vp, C.c_int, _vp, _vp, C.c_double, _vp, _vp]
+    L.fl_filter_get_nearest_device.argtypes = [_vp, _vp, _vp, C.c_int, _vp]
+    L.fl_filter_get_selected_device.argtypes = [_vp, _vp, C.c_int, _vp]
     L.fl_filter_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int]
     L.fl_filter_destroy.argtypes = [C.c_void_p]
     L.fl_filter_set_params.argtypes = [C.c_void_p, C.c_int, _f64p, C.c_int]
@@ -267,18 +271,23 @@ class KdTree:
         return offsets, out[:total]
 
     # ---- device-buffer forms: CUDA tensors on the map's device, enqueued on torch.cuda.current_stream()
-    def _tensor(self, t, name: str, cols: int | None):
+    def _tensor(self, t, name: str, cols: int | None, dtype=None, shape: tuple | None = None):
+        """t checked to be a contiguous CUDA tensor on the map's device of `dtype` (default float32), shaped (n, cols) or
+        exactly `shape`."""
         import torch
+        dtype = torch.float32 if dtype is None else dtype
         if not isinstance(t, torch.Tensor):
             raise TypeError(f"{name}: expected a torch.Tensor, got {type(t).__name__}")
         if t.device.type != "cuda" or t.device.index != self.device:
             raise ValueError(f"{name}: expected a tensor on cuda:{self.device}, got one on {t.device}")
-        if t.dtype != torch.float32:
-            raise TypeError(f"{name}: expected float32, got {t.dtype}")
+        if t.dtype != dtype:
+            raise TypeError(f"{name}: expected {str(dtype).replace('torch.', '')}, got {t.dtype}")
         if not t.is_contiguous():
             raise ValueError(f"{name}: expected a contiguous tensor")
         if cols is not None and (t.dim() != 2 or t.shape[1] != cols):
             raise ValueError(f"{name}: expected shape (n, {cols}), got {tuple(t.shape)}")
+        if shape is not None and tuple(t.shape) != shape:
+            raise ValueError(f"{name}: expected shape {shape}, got {tuple(t.shape)}")
         return t
 
     def _stream(self):
@@ -452,6 +461,41 @@ class Esekf:
             out.append(dict(searched=l.searched, valid=l.valid, effct=l.effct, converged=l.converged,
                             res_sum=l.res_sum, HtH=np.array(l.HtH).reshape(12, 12).copy(),
                             Hth=np.array(l.Hth).copy(), x_after=np.array(l.x_after).copy()))
+        return out
+
+    # ---- device-buffer form: CUDA tensors on the map's device, enqueued on torch.cuda.current_stream()
+    def update_device(self, scan, x, P, R: float = 0.001, status=None):
+        """fl_filter_update_device: scan (nq, 4) float32, x (26,) float64, P (23, 23) float64.  x and P are updated in place
+        (only when the update succeeds); returns status, an int32 tensor of shape (2,) = (FL_OK or FL_ERR_STATE, passes run),
+        written on the current stream.  Nothing synchronises, so the call can be captured into a CUDA graph."""
+        import torch
+        t = self.tree
+        scan = t._tensor(scan, "scan", 4)
+        x = t._tensor(x, "x", None, torch.float64, (26,))
+        P = t._tensor(P, "P", None, torch.float64, (23, 23))
+        if status is None:
+            status = torch.empty(2, dtype=torch.int32, device=x.device)
+        status = t._tensor(status, "status", None, torch.int32, (2,))
+        nq = scan.shape[0]
+        _check(self._L.fl_filter_update_device(self.h, scan.data_ptr() if nq else None, nq, x.data_ptr(), P.data_ptr(), R,
+                                               status.data_ptr(), t._stream()))
+        return status
+
+    def nearest_device(self, nq: int):
+        """Nearest_Points of the last update as tensors (pts [nq, 5, 4] float32, cnt [nq] int32), copied on the current stream."""
+        import torch
+        dev = f"cuda:{self.tree.device}"
+        pts = torch.empty((nq, 5, 4), dtype=torch.float32, device=dev)
+        cnt = torch.empty((nq,), dtype=torch.int32, device=dev)
+        _check(self._L.fl_filter_get_nearest_device(self.h, pts.data_ptr() if nq else None, cnt.data_ptr() if nq else None, nq,
+                                                    self.tree._stream()))
+        return pts, cnt
+
+    def selected_device(self, nq: int):
+        """point_selected_surf of the last update as a uint8 tensor [nq], copied on the current stream."""
+        import torch
+        out = torch.empty((nq,), dtype=torch.uint8, device=f"cuda:{self.tree.device}")
+        _check(self._L.fl_filter_get_selected_device(self.h, out.data_ptr() if nq else None, nq, self.tree._stream()))
         return out
 
     # device-resident pieces

@@ -260,6 +260,21 @@ int fl_filter_get_pass_logs(fl_filter_t* f, fl_pass_log_t* out, int cap) {
     int rc = f->impl->get_pass_logs(reinterpret_cast<fl::PassLog*>(out), cap, &n);
     return rc == FL_OK ? n : rc;
 }
+// Device-buffer forms: the guard touch()es the map, so the join in Map::query_begin also orders this call after an earlier
+// device-form update of the filter on another caller stream (they share the filter's buffers).
+int fl_filter_update_device(fl_filter_t* f, const float* body_xyzi_device, int nq, double* x26_device, double* P_device, double R,
+                            int* status2_device, void* stream) {
+    FILTER_GUARD(f);
+    return f->impl->update_on_stream(body_xyzi_device, nq, x26_device, P_device, R, status2_device, static_cast<cudaStream_t>(stream));
+}
+int fl_filter_get_nearest_device(fl_filter_t* f, float* out_pts_device, int* out_cnt_device, int nq, void* stream) {
+    FILTER_GUARD(f);
+    return f->impl->get_nearest_on_stream(out_pts_device, out_cnt_device, nq, static_cast<cudaStream_t>(stream));
+}
+int fl_filter_get_selected_device(fl_filter_t* f, unsigned char* out_device, int nq, void* stream) {
+    FILTER_GUARD(f);
+    return f->impl->get_selected_on_stream(out_device, nq, static_cast<cudaStream_t>(stream));
+}
 int fl_filter_upload_scan(fl_filter_t* f, const float* body, int nq) { FILTER_GUARD(f); return f->impl->upload_scan(body, nq); }
 int fl_filter_upload_state(fl_filter_t* f, const double* x26, const double* P, double R) {
     FILTER_GUARD(f);

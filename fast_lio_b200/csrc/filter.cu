@@ -1063,6 +1063,49 @@ __global__ void k_map_incremental(ScanView sc, const FilterCtl* __restrict__ ctl
     flag_no[q] = cls == 1;
 }
 
+// ============================================================================= device-buffer update (fl_filter_update_device)
+// What upload_state sets up on the host, from kernel arguments and the caller's x26 / P in HBM.
+struct StateIn {
+    double limit[NDOF];
+    double R;
+    int max_iter, extrinsic_est;
+};
+constexpr int STATE_THREADS = 256;
+
+// Also clears k_update's publication block: its workers take a word as current when its tag equals pub_tag(nonce, pass), and
+// every replay of a captured graph passes the same nonce, so words left by the previous replay would otherwise look current.
+// And it clears `done` in the page-locked mirror, so download_state / get_pass_logs fetch this update's control block instead
+// of trusting a result an earlier host-form update mirrored there.
+__global__ void __launch_bounds__(STATE_THREADS) k_state_in(FilterCtl* ctl, unsigned long long* pub, FilterCtl* mirror,
+                                                            const double* __restrict__ x26, const double* __restrict__ P, StateIn s) {
+    pdl_launch();           // k_update may begin launching: its pdl_wait() holds it until this grid is complete and flushed
+    const int t = threadIdx.x;
+    for (int i = t; i < NDOF * NDOF; i += STATE_THREADS) { const double v = P[i]; ctl->P[i] = v; ctl->P_prop[i] = v; }   // P_propagated = P_
+    if (t < XLEN) { const double v = x26[t]; ctl->x[t] = v; ctl->x_prop[t] = v; ctl->x_search[t] = 0.0; }                 // x_propagated = x_
+    if (t < NDOF) ctl->limit[t] = s.limit[t];
+    if (t < 16) ctl->prof[t] = 0;
+    if (t < PUB_WORDS) pub[t] = 0ull;              // tag 0 is never current: pub_tag(nonce, pass) has pass >= 1 there
+    if (t == 0) {
+        // esekfom.hpp:1621-1631, as upload_state
+        ctl->iter = -1; ctl->t = 0; ctl->converge = 1; ctl->done = 0; ctl->n_pass = 0; ctl->error = 0; ctl->ticket = 0; ctl->gen = 0;
+        ctl->max_iter = s.max_iter; ctl->extrinsic_est = s.extrinsic_est; ctl->R = s.R;
+        ctl->host_mirror = nullptr;
+        mirror->done = 0;
+    }
+}
+
+// x26 / P receive the result only when the update succeeded; status2 = (FL_OK or the error download_state reports, passes run)
+__global__ void __launch_bounds__(STATE_THREADS) k_state_out(const FilterCtl* __restrict__ ctl, double* __restrict__ x26,
+                                                             double* __restrict__ P, int* __restrict__ status2) {
+    const int t = threadIdx.x;
+    const int e = ctl->error;
+    if (e == 0) {
+        for (int i = t; i < NDOF * NDOF; i += STATE_THREADS) P[i] = ctl->P[i];
+        if (t < XLEN) x26[t] = ctl->x[t];
+    }
+    if (t == 0) { status2[0] = e == 0 ? FL_OK : (e == 2 ? FL_ERR_NCCL : FL_ERR_STATE); status2[1] = ctl->n_pass; }
+}
+
 // ============================================================================= NCCL (lazy)
 struct NcclUniqueId { char internal[128]; };
 struct NcclApi {
@@ -1323,7 +1366,7 @@ int Filter::run_passes() {
 }
 
 // the fused persistent kernel: blockIdx 0 solves, the others measure; every block must be co-resident (they wait for each other)
-int Filter::launch_update(int max_passes, int mode, int search_only) {
+int Filter::launch_update(int max_passes, int mode, int search_only, cudaStream_t st) {
     FL_CUDA(cudaSetDevice(map_->device()));
     const int nq = scan_.q_end - scan_.q_begin;
     UpdArgs a;
@@ -1340,7 +1383,7 @@ int Filter::launch_update(int max_passes, int mode, int search_only) {
     // one thread per point: full warps (the search is bound by a thread's own chain of loads, not by the number of SMs)
     int workers = mode == 3 ? 0 : std::min(cap - 1, (nq + UPD_THREADS - 1) / UPD_THREADS);
     if (workers < 0) workers = 0;
-    FL_CUDA(launch_upd(workers, pdl_, a, upd_pair(nq)));
+    FL_CUDA(launch_upd(workers, pdl_, a, upd_pair(nq), st));
     return FL_OK;
 }
 
@@ -1352,12 +1395,12 @@ int Filter::upd_pair(int nq) const {
     const int tiles = (nq + UPD_THREADS - 1) / UPD_THREADS;
     return tiles >= 1 && tiles <= upd_capacity_[extrinsic_est_ ? 1 : 0][1] - 1 ? 2 : 1;
 }
-cudaError_t Filter::launch_upd(int workers, bool pdl, const UpdArgs& a, int pair) {
+cudaError_t Filter::launch_upd(int workers, bool pdl, const UpdArgs& a, int pair, cudaStream_t st) {
     const int block = pair * UPD_THREADS;
-    if (extrinsic_est_) return pair == 2 ? launch_pdl(k_update<true, 2>, workers + 1, block, stream(), pdl, a)
-                                         : launch_pdl(k_update<true, 1>, workers + 1, block, stream(), pdl, a);
-    return pair == 2 ? launch_pdl(k_update<false, 2>, workers + 1, block, stream(), pdl, a)
-                     : launch_pdl(k_update<false, 1>, workers + 1, block, stream(), pdl, a);
+    if (extrinsic_est_) return pair == 2 ? launch_pdl(k_update<true, 2>, workers + 1, block, st, pdl, a)
+                                         : launch_pdl(k_update<true, 1>, workers + 1, block, st, pdl, a);
+    return pair == 2 ? launch_pdl(k_update<false, 2>, workers + 1, block, st, pdl, a)
+                     : launch_pdl(k_update<false, 1>, workers + 1, block, st, pdl, a);
 }
 
 int Filter::launch_search_only() {
@@ -1454,6 +1497,92 @@ int Filter::update_any(const float* body_xyzi, const float4* d_body, int nq, dou
         *solve_time_s += ms * 1e-3;                       // the reference accumulates into solve_time (esekfom.hpp:1926)
     }
     return FL_OK;
+}
+
+// ----------------------------------------------------------------------------- device-buffer forms
+int Filter::capacity() const {
+    size_t c = body_.bytes / sizeof(float4);
+    c = std::min(c, nearest_.bytes / (sizeof(float4) * KNN_K));
+    c = std::min(c, nearest_cnt_.bytes / sizeof(int));
+    c = std::min(c, selected_.bytes);
+    c = std::min(c, normvec_.bytes / sizeof(float4));
+    c = std::min(c, plane_.bytes / sizeof(float4));
+    c = std::min(c, srange_.bytes / sizeof(double));
+    return (int)std::min<size_t>(c, INT_MAX);
+}
+
+int Filter::device_form_scope(const char* what, bool update) const {
+    if (shard_set_ || nranks_ > 1 || p2p_on_) {
+        set_last_error("%s: a sharded filter (set_shard / comm_init / p2p_connect) has no device-buffer form", what);
+        return FL_ERR_STATE;
+    }
+    if (update && !fused()) {
+        set_last_error("%s: the device-buffer form runs k_update only; this filter uses %s", what,
+                       solver_ != 1 ? "solver mode 0" : "the two-kernels-per-pass chain (fused 0)");
+        return FL_ERR_STATE;
+    }
+    return FL_OK;
+}
+
+int Filter::update_on_stream(const float* d_body, int nq, double* d_x26, double* d_P, double R, int* d_status2, cudaStream_t st) {
+    const int dev = map_->device();
+    if (nq < 0 || (nq > 0 && !device_ptr(d_body, dev, 16)) || !device_ptr(d_x26, dev, 8) || !device_ptr(d_P, dev, 8) ||
+        !device_ptr(d_status2, dev, 4)) {
+        set_last_error("update_device: nq < 0, or a buffer is not device memory on device %d (scan 16-byte, x and P 8-byte, "
+                       "status 4-byte aligned)", dev);
+        return FL_ERR_ARG;
+    }
+    FL_CHECK(device_form_scope("update_device", true));
+    if (nq > capacity()) {
+        set_last_error("update_device: %d points exceed the filter's capacity of %d (max_points, or the largest scan so far)", nq, capacity());
+        return FL_ERR_CAPACITY;
+    }
+    FL_CUDA(cudaSetDevice(dev));
+    FL_CHECK(set_scan_device(body_.as<float4>(), nq));       // within capacity: binds, allocates nothing
+    bool joined = false;
+    FL_CHECK(map_->query_begin(st, &joined));
+    if (nq > 0) FL_CUDA(cudaMemcpyAsync(body_.ptr, d_body, sizeof(float4) * (size_t)nq, cudaMemcpyDeviceToDevice, st));
+    StateIn s;
+    for (int i = 0; i < NDOF; i++) s.limit[i] = limit_[i];
+    s.R = R; s.max_iter = max_iter_; s.extrinsic_est = extrinsic_est_;
+    k_state_in<<<1, STATE_THREADS, 0, st>>>(ctl_.as<FilterCtl>(), pub_.as<unsigned long long>(), h_ctl_, d_x26, d_P, s);
+    FL_CUDA(cudaGetLastError());
+    // run_passes's fused single-rank branch, on `st`
+    neighbours_complete_ = false;
+    FL_CHECK(launch_update(max_iter_ + 1, 0, 0, st));
+    launches_ = 1;
+    k_state_out<<<1, STATE_THREADS, 0, st>>>(ctl_.as<FilterCtl>(), d_x26, d_P, d_status2);
+    return map_->query_end(st, joined);
+}
+
+int Filter::get_nearest_on_stream(float* d_pts, int* d_cnt, int nq, cudaStream_t st) {
+    const int dev = map_->device();
+    if (nq < 0 || nq > scan_.Q) { set_last_error("get_nearest_device: nq must be in [0, %d] (the bound scan)", scan_.Q); return FL_ERR_ARG; }
+    if (nq > 0 && (!device_ptr(d_pts, dev, 16) || !device_ptr(d_cnt, dev, 4))) {
+        set_last_error("get_nearest_device: the buffers must be device memory on device %d (points 16-byte aligned)", dev);
+        return FL_ERR_ARG;
+    }
+    FL_CHECK(device_form_scope("get_nearest_device", false));
+    if (nq == 0) return FL_OK;
+    FL_CUDA(cudaSetDevice(dev));
+    bool joined = false;
+    FL_CHECK(map_->query_begin(st, &joined));
+    FL_CUDA(cudaMemcpyAsync(d_pts, scan_.nearest, sizeof(float4) * KNN_K * (size_t)nq, cudaMemcpyDeviceToDevice, st));
+    FL_CUDA(cudaMemcpyAsync(d_cnt, scan_.nearest_cnt, sizeof(int) * (size_t)nq, cudaMemcpyDeviceToDevice, st));
+    return map_->query_end(st, joined);
+}
+
+int Filter::get_selected_on_stream(unsigned char* d_out, int nq, cudaStream_t st) {
+    const int dev = map_->device();
+    if (nq < 0 || nq > scan_.Q) { set_last_error("get_selected_device: nq must be in [0, %d] (the bound scan)", scan_.Q); return FL_ERR_ARG; }
+    if (nq > 0 && !device_ptr(d_out, dev, 1)) { set_last_error("get_selected_device: the buffer must be device memory on device %d", dev); return FL_ERR_ARG; }
+    FL_CHECK(device_form_scope("get_selected_device", false));
+    if (nq == 0) return FL_OK;
+    FL_CUDA(cudaSetDevice(dev));
+    bool joined = false;
+    FL_CHECK(map_->query_begin(st, &joined));
+    FL_CUDA(cudaMemcpyAsync(d_out, scan_.selected, (size_t)nq, cudaMemcpyDeviceToDevice, st));
+    return map_->query_end(st, joined);
 }
 
 int Filter::map_incremental(double fsm, int ekf_inited, int* n_to_add, int* n_no_downsample, int* added) {

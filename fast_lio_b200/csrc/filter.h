@@ -92,6 +92,15 @@ public:
     int launch_residual_only();
     int download_state(double* x26, double* P, int* n_pass);
     int sync();
+    // the whole update on caller device buffers, enqueued on the caller's stream `st` (fl_filter_update_device): the scan is
+    // copied into body_, a state-in kernel sets the control block up from x26 / P, k_update runs the passes and a state-out
+    // kernel writes x26 / P (on success) and status2 = (status, passes).  No host synchronisation, no allocation.
+    int update_on_stream(const float* d_body, int nq, double* d_x26, double* d_P, double R, int* d_status2, cudaStream_t st);
+    // Nearest_Points / point_selected_surf of the last update into caller device buffers, on `st`
+    int get_nearest_on_stream(float* d_pts, int* d_cnt, int nq, cudaStream_t st);
+    int get_selected_on_stream(unsigned char* d_out, int nq, cudaStream_t st);
+    // the largest scan the per-point buffers hold without growing (max_points at create, or the largest scan since)
+    int capacity() const;
 
     // map_incremental (laserMapping.cpp:427-474) on the device: classify every scan point with the final
     // state and its cached neighbours, then Add_Points(PointToAdd, true) + Add_Points(PointNoNeedDownsample, false)
@@ -146,9 +155,13 @@ private:
     DeviceBuffer pub_;                 // k_update's publication block
     unsigned launch_nonce_ = 0;
     int upd_capacity_[2][2] = {{0, 0}, {0, 0}};   // co-resident k_update<EXTR, PAIR> blocks on this device, [EXTR][PAIR - 1]
-    int launch_update(int max_passes, int mode, int search_only);
+    int launch_update(int max_passes, int mode, int search_only) { return launch_update(max_passes, mode, search_only, stream()); }
+    int launch_update(int max_passes, int mode, int search_only, cudaStream_t st);
     int upd_pair(int nq) const;                   // 2: the shard's tiles fit the 512-thread grid (two threads per point), else 1
-    cudaError_t launch_upd(int workers, bool pdl, const UpdArgs& a, int pair);
+    cudaError_t launch_upd(int workers, bool pdl, const UpdArgs& a, int pair) { return launch_upd(workers, pdl, a, pair, stream()); }
+    cudaError_t launch_upd(int workers, bool pdl, const UpdArgs& a, int pair, cudaStream_t st);
+    // the device forms cover a single-rank filter (and the update a fused, solver-1 one); FL_ERR_STATE otherwise
+    int device_form_scope(const char* what, bool update) const;
     int launches_ = 0;
     long long host_ns_[4] = {0, 0, 0, 0};
     bool shard_set_ = false;

@@ -1373,8 +1373,7 @@ int Map::range_search(bool radius, const float* queries, int nq, int* out_offset
 }
 
 // ----------------------------------------------------------------------------- device-buffer forms
-// true: p is device memory of `device` (or managed memory allocated against it), aligned to `align` bytes
-static bool device_ptr(const void* p, int device, size_t align) {
+bool device_ptr(const void* p, int device, size_t align) {
     if (!p || (reinterpret_cast<uintptr_t>(p) % align) != 0) return false;
     cudaPointerAttributes a;
     if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }

@@ -16,6 +16,9 @@ struct DeviceBuffer {
     template <class T> T* as() const { return static_cast<T*>(ptr); }
 };
 
+// true: p is device memory of `device` (or managed memory allocated against it), aligned to `align` bytes
+bool device_ptr(const void* p, int device, size_t align);
+
 class Map {
 public:
     Map(int device, float downsample_size);
@@ -55,6 +58,10 @@ public:
     int add_points_from_caller(const float* d_pts_xyzi, int n, bool downsample_on, cudaStream_t st, int* added);
     // every call that may enqueue work on the handle's stream marks it, so the next device query joins that work
     void touch() { front_stale_ = true; }
+    // the join of every device-buffer call on a caller's stream `st` (map queries, fl_filter_update_device): outside capture,
+    // query_begin makes `st` wait for the handle's stream and query_end makes the handle's stream wait for `st`
+    int query_begin(cudaStream_t st, bool* joined);
+    int query_end(cudaStream_t st, bool joined);
     // re-sort every valid point into fresh, evenly filled leaves (ikd-Tree's Rebuild, ikd_Tree.cpp:736-764)
     int rebuild();
     // re-list every live slot in the hashed cell directory (map.cuh); done by build / rebuild, and when inserts crowd it
@@ -93,8 +100,6 @@ private:
     // the kernel and grid of every nearest search; knn_host runs it on host buffers
     void launch_knn(bool gated, const float4* q, int nq, int k, float md2, float4* p, float* d2, int* cnt, cudaStream_t st);
     int knn_host(bool gated, const float* q_xyzi, int nq, int k, float md2, float* out_pts, float* out_d2, int* out_cnt);
-    int query_begin(cudaStream_t st, bool* joined);
-    int query_end(cudaStream_t st, bool joined);
     int wait_for_caller(cudaStream_t st, const char* what);
 
     int ensure_capacity(int n_points);

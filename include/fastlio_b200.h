@@ -224,6 +224,34 @@ int fl_filter_gpu_launches(fl_filter_t* f);
 /* clock64() stamps of the last on-device Kalman step (tuning aid; layout in scripts/profile_once.py) */
 int fl_filter_debug_prof(fl_filter_t* f, long long* out16);
 
+/* ---- device-buffer form of the update (the conventions of the map's *_device block above)
+ * esekf::update_iterated_dyn_share_modified on device buffers      esekfom.hpp:1619-1931, laserMapping.cpp:638-754
+ * x26_device (26 doubles) and P_device (23 x 23, row-major) are read when the update starts and overwritten when it ends, like
+ * the reference's x_ / P_, but only when it succeeds.  status2_device[0] receives FL_OK, or FL_ERR_STATE for a singular system
+ * or a block that gave up waiting; status2_device[1] the number of passes run.  On success x and P hold exactly the bytes
+ * fl_filter_update returns for the same map, scan, prior, R and parameters; fl_filter_get_pass_logs, get_nearest,
+ * get_selected, download_state and map_incremental afterwards see this update as they would see fl_filter_update's.
+ * The scan is copied into the filter's own buffer on `stream`: the caller may reuse or free body_xyzi_device once `stream`
+ * has passed the call.  The call never synchronises the host, never allocates and never sizes a launch from a device value;
+ * nq above the filter's capacity (max_points at create, or the largest scan it has bound since) is FL_ERR_CAPACITY and
+ * enqueues nothing.  solve_time is not reported: time the call with events on `stream`.
+ * Ordering: outside stream capture, `stream` first waits for everything enqueued on the handle's stream (including an
+ * earlier device-form update of this filter on another stream), and the handle's stream then waits for the update, so a
+ * later host-form call on the filter or the map (map_incremental, get_pass_logs, Add_Points, Delete_Point_Boxes) sees its
+ * result and cannot change the map under it.  While `stream` is capturing nothing is joined: order replays against other
+ * calls on the filter and the map yourself (synchronise a replay before a host-form call on the filter).  A captured graph
+ * keeps the map's layout, the filter's buffers, nq and the parameters (max_iter, limit, extrinsic_est_en, R) of capture time;
+ * capture again after any of them changes.
+ * A host pointer, a pointer to another device, a null pointer (the scan may be null when nq = 0) or a misaligned one (scan
+ * 16 bytes, x and P 8, status 4) is FL_ERR_ARG; a sharded filter (set_shard, comm_init with nranks > 1, p2p_connect), solver
+ * mode 0 or fused 0 is FL_ERR_STATE: the device form runs k_update only.  Nothing is enqueued on a refusal. */
+int fl_filter_update_device(fl_filter_t* f, const float* body_xyzi_device, int nq, double* x26_device, double* P_device, double R,
+                            int* status2_device, void* stream);
+/* Nearest_Points / point_selected_surf of the last update (the bytes of fl_filter_get_nearest / get_selected), copied into
+ * device buffers on `stream` with the update's ordering rules; 0 <= nq <= the bound scan's size.  Not for sharded filters. */
+int fl_filter_get_nearest_device(fl_filter_t* f, float* out_pts_device, int* out_cnt_device, int nq, void* stream);
+int fl_filter_get_selected_device(fl_filter_t* f, unsigned char* out_device, int nq, void* stream);
+
 /* ------------------------------------------------------------------ scan front end (SURVEY.md §8f rows 3-4)
  * The two steps that produce feats_down_body, kept in HBM on the map's device and stream so that a scan goes
  * raw -> de-skewed -> down-sampled -> update -> map_incremental with one upload. */
