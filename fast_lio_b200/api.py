@@ -50,6 +50,7 @@ SYMBOLS = [
     "fl_filter_update_scan", "fl_localmap_create", "fl_localmap_destroy", "fl_localmap_segment", "fl_localmap_get",
     "fl_comm_unique_id", "fl_filter_comm_init", "fl_filter_set_shard", "fl_filter_p2p_handle", "fl_filter_p2p_connect",
     "fl_filter_update_device", "fl_filter_get_nearest_device", "fl_filter_get_selected_device",
+    "fl_map_add_points_async", "fl_map_maintain", "fl_filter_map_incremental_device",
 ]
 
 
@@ -97,6 +98,9 @@ def load():
         fn.argtypes = [_vp, _vp, C.c_int, _vp, _vp, C.c_longlong, _vp, C.c_ulonglong, _vp, _vp]
     L.fl_map_build_device.argtypes = [_vp, _vp, C.c_int, _vp]
     L.fl_map_add_points_device.argtypes = [_vp, _vp, C.c_int, C.c_int, _vp]
+    L.fl_map_add_points_async.argtypes = [_vp, _vp, _vp, C.c_int, C.c_int, _vp, _vp]
+    L.fl_map_maintain.argtypes = [_vp, C.POINTER(C.c_int)]
+    L.fl_filter_map_incremental_device.argtypes = [_vp, C.c_double, C.c_int, _vp, _vp]
     L.fl_filter_update_device.argtypes = [_vp, _vp, C.c_int, _vp, _vp, C.c_double, _vp, _vp]
     L.fl_filter_get_nearest_device.argtypes = [_vp, _vp, _vp, C.c_int, _vp]
     L.fl_filter_get_selected_device.argtypes = [_vp, _vp, C.c_int, _vp]
@@ -376,6 +380,28 @@ class KdTree:
         return _check(self._L.fl_map_add_points_device(self.h, pts.data_ptr() if len(pts) else None, len(pts), int(downsample_on),
                                                        self._stream()))
 
+    def add_points_async(self, pts, n, n_max: int, downsample_on: bool, status=None):
+        """fl_map_add_points_async: Add_Points of the first *n rows of pts ((>= n_max, 4) float32), n an int32 CUDA tensor of one
+        element read when the current stream reaches the call.  Returns status, an int32 tensor (2,) = (FL_OK, 1 = maintenance
+        due, or FL_ERR_CAPACITY = nothing changed; the reference's return value), written on the current stream."""
+        import torch
+        pts = self._tensor(pts, "pts", 4)
+        if pts.shape[0] < n_max:
+            raise ValueError(f"pts: {pts.shape[0]} rows, fewer than n_max = {n_max}")
+        n = self._tensor(n, "n", None, torch.int32, (1,))
+        if status is None:
+            status = torch.empty(2, dtype=torch.int32, device=pts.device)
+        status = self._tensor(status, "status", None, torch.int32, (2,))
+        _check(self._L.fl_map_add_points_async(self.h, pts.data_ptr() if n_max > 0 else None, n.data_ptr(), n_max,
+                                               int(downsample_on), status.data_ptr(), self._stream()))
+        return status
+
+    def maintain(self) -> bool:
+        """fl_map_maintain: settle the map and run the deferred re-pack / re-list; True when graphs must be captured again."""
+        changed = C.c_int(0)
+        _check(self._L.fl_map_maintain(self.h, C.byref(changed)))
+        return bool(changed.value)
+
     def tree_range(self) -> np.ndarray:
         box = np.zeros(6, dtype=np.float32)
         _check(self._L.fl_map_tree_range(self.h, box))
@@ -480,6 +506,17 @@ class Esekf:
         _check(self._L.fl_filter_update_device(self.h, scan.data_ptr() if nq else None, nq, x.data_ptr(), P.data_ptr(), R,
                                                status.data_ptr(), t._stream()))
         return status
+
+    def map_incremental_device(self, filter_size_map_min: float = 0.5, flg_EKF_inited: bool = True, out4=None):
+        """fl_filter_map_incremental_device on the current stream.  Returns out4, an int32 tensor (4,) = (|PointToAdd|,
+        |PointNoNeedDownsample|, Add_Points return, status), written without a host synchronisation (capturable)."""
+        import torch
+        t = self.tree
+        if out4 is None:
+            out4 = torch.empty(4, dtype=torch.int32, device=f"cuda:{t.device}")
+        out4 = t._tensor(out4, "out4", None, torch.int32, (4,))
+        _check(self._L.fl_filter_map_incremental_device(self.h, filter_size_map_min, int(flg_EKF_inited), out4.data_ptr(), t._stream()))
+        return out4
 
     def nearest_device(self, nq: int):
         """Nearest_Points of the last update as tensors (pts [nq, 5, 4] float32, cnt [nq] int32), copied on the current stream."""

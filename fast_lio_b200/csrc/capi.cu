@@ -96,59 +96,67 @@ int fl_map_destroy(fl_map_t* m) {
 #define MAP_QUERY_GUARD(m)                                                       \
     if (!(m) || !(m)->impl) { fl::set_last_error("null map handle"); return FL_ERR_ARG; } \
     std::lock_guard<std::mutex> _lk((m)->mu)
+// host forms settle the device forms' mutations first (Map::settle): a read-only call refreshes the host's view of the map, any
+// other call also runs the re-pack / re-list they deferred
+#define MAP_READ_GUARD(m)                                                        \
+    MAP_GUARD(m);                                                                \
+    { const int _rc = (m)->impl->settle(false); if (_rc != FL_OK) return _rc; }
+#define MAP_MUTATE_GUARD(m)                                                      \
+    MAP_GUARD(m);                                                                \
+    { const int _rc = (m)->impl->settle(true); if (_rc != FL_OK) return _rc; }
 
 int fl_map_set_downsample(fl_map_t* m, float v) { MAP_GUARD(m); m->impl->set_downsample(v); return FL_OK; }
-int fl_map_build(fl_map_t* m, const float* pts, int n) { MAP_GUARD(m); return m->impl->build(pts, n); }
-int fl_map_size(fl_map_t* m) { MAP_GUARD(m); return m->impl->size(); }
-int fl_map_validnum(fl_map_t* m) { MAP_GUARD(m); return m->impl->validnum(); }
+int fl_map_build(fl_map_t* m, const float* pts, int n) { MAP_MUTATE_GUARD(m); return m->impl->build(pts, n); }
+int fl_map_size(fl_map_t* m) { MAP_READ_GUARD(m); return m->impl->size(); }
+int fl_map_validnum(fl_map_t* m) { MAP_READ_GUARD(m); return m->impl->validnum(); }
 int fl_map_knn(fl_map_t* m, const float* q, int nq, int k, float* out_pts, float* out_d2, int* out_cnt) {
-    MAP_GUARD(m);
+    MAP_READ_GUARD(m);
     if (nq > 0 && (!q || !out_pts || !out_d2 || !out_cnt)) { fl::set_last_error("fl_map_knn: null buffer"); return FL_ERR_ARG; }
     return m->impl->knn(q, nq, k, out_pts, out_d2, out_cnt);
 }
 int fl_map_nearest_search(fl_map_t* m, const float* q, int nq, int k, float max_dist, float* out_pts, float* out_d2, int* out_cnt) {
-    MAP_GUARD(m);
+    MAP_READ_GUARD(m);
     if (nq > 0 && (!q || !out_pts || !out_d2 || !out_cnt)) { fl::set_last_error("fl_map_nearest_search: null buffer"); return FL_ERR_ARG; }
     return m->impl->nearest_search(q, nq, k, max_dist, out_pts, out_d2, out_cnt);
 }
 int fl_map_add_points(fl_map_t* m, const float* pts, int n, int downsample_on) {
-    MAP_GUARD(m);
+    MAP_MUTATE_GUARD(m);
     int added = 0;
     int rc = m->impl->add_points(pts, n, downsample_on != 0, &added);
     return rc == FL_OK ? added : rc;
 }
 int fl_map_delete_boxes(fl_map_t* m, const float* boxes6, int nb) {
-    MAP_GUARD(m);
+    MAP_MUTATE_GUARD(m);
     int deleted = 0;
     int rc = m->impl->delete_boxes(boxes6, nb, &deleted);
     return rc == FL_OK ? deleted : rc;
 }
 int fl_map_add_boxes(fl_map_t* m, const float* boxes6, int nb) {
-    MAP_GUARD(m);
+    MAP_MUTATE_GUARD(m);
     int revived = 0;
     int rc = m->impl->add_boxes(boxes6, nb, &revived);
     return rc == FL_OK ? revived : rc;
 }
 int fl_map_acquire_removed(fl_map_t* m, float* out, int cap) {
-    MAP_GUARD(m);
+    MAP_READ_GUARD(m);
     int n = 0;
     int rc = m->impl->acquire_removed(out, cap, &n);
     return rc == FL_OK ? n : rc;
 }
 int fl_map_flatten(fl_map_t* m, float* out, int cap) {
-    MAP_GUARD(m);
+    MAP_READ_GUARD(m);
     int n = 0;
     int rc = m->impl->flatten(out, cap, &n);
     return rc == FL_OK ? n : rc;
 }
 int fl_map_box_search(fl_map_t* m, const float* boxes6, int nb, int* out_offsets, float* out_xyzi, int cap) {
-    MAP_GUARD(m);
+    MAP_READ_GUARD(m);
     long long total = 0;
     int rc = m->impl->range_search(false, boxes6, nb, out_offsets, out_xyzi, cap, &total);
     return rc == FL_OK ? (int)total : rc;
 }
 int fl_map_radius_search(fl_map_t* m, const float* centers_xyzr, int nq, int* out_offsets, float* out_xyzi, int cap) {
-    MAP_GUARD(m);
+    MAP_READ_GUARD(m);
     long long total = 0;
     int rc = m->impl->range_search(true, centers_xyzr, nq, out_offsets, out_xyzi, cap, &total);
     return rc == FL_OK ? (int)total : rc;
@@ -178,19 +186,33 @@ int fl_map_radius_search_device(fl_map_t* m, const float* centers_xyzr_device, i
                                         workspace_bytes, status2_device, static_cast<cudaStream_t>(stream));
 }
 int fl_map_build_device(fl_map_t* m, const float* pts_xyzi_device, int n, void* stream) {
-    MAP_GUARD(m);
+    MAP_MUTATE_GUARD(m);
     return m->impl->build_from_caller(pts_xyzi_device, n, static_cast<cudaStream_t>(stream));
 }
 int fl_map_add_points_device(fl_map_t* m, const float* pts_xyzi_device, int n, int downsample_on, void* stream) {
-    MAP_GUARD(m);
+    MAP_MUTATE_GUARD(m);
     int added = 0;
     int rc = m->impl->add_points_from_caller(pts_xyzi_device, n, downsample_on != 0, static_cast<cudaStream_t>(stream), &added);
     return rc == FL_OK ? added : rc;
 }
-int fl_map_tree_range(fl_map_t* m, float* box6) { MAP_GUARD(m); if (!box6) return FL_ERR_ARG; return m->impl->tree_range(box6); }
-int fl_map_rebuild(fl_map_t* m) { MAP_GUARD(m); return m->impl->rebuild(); }
-int fl_map_stats(fl_map_t* m, int* out4) {
+// Device form: never settles (the host's view catches up at the next host-form call or fl_map_maintain)
+int fl_map_add_points_async(fl_map_t* m, const float* pts_xyzi_device, const int* n_device, int n_max, int downsample_on,
+                            int* status2_device, void* stream) {
     MAP_GUARD(m);
+    return m->impl->add_points_async_checked(pts_xyzi_device, n_device, n_max, downsample_on != 0, status2_device,
+                                             static_cast<cudaStream_t>(stream));
+}
+int fl_map_maintain(fl_map_t* m, int* layout_changed) {
+    MAP_GUARD(m);
+    int changed = 0;
+    const int rc = m->impl->settle(true, &changed);
+    if (layout_changed) *layout_changed = changed;
+    return rc;
+}
+int fl_map_tree_range(fl_map_t* m, float* box6) { MAP_READ_GUARD(m); if (!box6) return FL_ERR_ARG; return m->impl->tree_range(box6); }
+int fl_map_rebuild(fl_map_t* m) { MAP_MUTATE_GUARD(m); return m->impl->rebuild(); }
+int fl_map_stats(fl_map_t* m, int* out4) {
+    MAP_READ_GUARD(m);
     if (!out4) return FL_ERR_ARG;
     out4[0] = m->impl->view().n_main; out4[1] = m->impl->overflow_leaves();
     out4[2] = m->impl->view().n_levels; out4[3] = m->impl->rebuild_count();
@@ -198,12 +220,12 @@ int fl_map_stats(fl_map_t* m, int* out4) {
 }
 
 int fl_map_set_cell_directory(fl_map_t* m, int on, float cell_size) {
-    MAP_GUARD(m);
+    MAP_MUTATE_GUARD(m);
     m->impl->set_cell_directory(on != 0, cell_size > 0.f ? cell_size : 0.f);
     return m->impl->build_directory();
 }
 int fl_map_dir_stats(fl_map_t* m, int* out6) {
-    MAP_GUARD(m);
+    MAP_READ_GUARD(m);
     if (!out6) return FL_ERR_ARG;
     return m->impl->dir_stats(out6);
 }
@@ -213,6 +235,10 @@ int fl_map_dir_stats(fl_map_t* m, int* out6) {
     if (!(f) || !(f)->impl) { fl::set_last_error("null filter handle"); return FL_ERR_ARG; }   \
     std::lock_guard<std::mutex> _lk((f)->map->mu);                                             \
     (f)->map->impl->touch()
+// the filter's host forms settle the map first, with its deferred re-pack / re-list (Map::settle)
+#define FILTER_HOST_GUARD(f)                                                                   \
+    FILTER_GUARD(f);                                                                           \
+    { const int _rc = (f)->map->impl->settle(true); if (_rc != FL_OK) return _rc; }
 
 int fl_filter_create(fl_filter_t** out, fl_map_t* map, int max_points) {
     if (!out || !map || !map->impl) { fl::set_last_error("fl_filter_create: null argument"); return FL_ERR_ARG; }
@@ -241,15 +267,19 @@ int fl_filter_set_solver(fl_filter_t* f, int mode) { FILTER_GUARD(f); if (mode <
 int fl_filter_set_fused(fl_filter_t* f, int on) { FILTER_GUARD(f); f->impl->set_fused(on != 0); return FL_OK; }
 int fl_filter_set_search(fl_filter_t* f, int mode) { FILTER_GUARD(f); if (mode < 0 || mode > 1) return FL_ERR_ARG; f->impl->set_search_mode(mode); return FL_OK; }
 int fl_filter_update(fl_filter_t* f, const float* body, int nq, double* x26, double* P, double R, double* solve_time_s) {
-    FILTER_GUARD(f);
+    FILTER_HOST_GUARD(f);
     return f->impl->update(body, nq, x26, P, R, solve_time_s);
 }
 int fl_filter_map_incremental(fl_filter_t* f, double fsm, int ekf_inited, int* out3) {
-    FILTER_GUARD(f);
+    FILTER_HOST_GUARD(f);
     int a = 0, b = 0, c = 0;
     int rc = f->impl->map_incremental(fsm, ekf_inited, &a, &b, &c);
     if (out3) { out3[0] = a; out3[1] = b; out3[2] = c; }
     return rc;
+}
+int fl_filter_map_incremental_device(fl_filter_t* f, double fsm, int ekf_inited, int* out4_device, void* stream) {
+    FILTER_GUARD(f);
+    return f->impl->map_incremental_on_stream(fsm, ekf_inited, out4_device, static_cast<cudaStream_t>(stream));
 }
 int fl_filter_get_nearest(fl_filter_t* f, float* out_pts, int* out_cnt, int nq) { FILTER_GUARD(f); return f->impl->get_nearest(out_pts, out_cnt, nq); }
 int fl_filter_get_selected(fl_filter_t* f, unsigned char* out, int nq) { FILTER_GUARD(f); if (!out) return FL_ERR_ARG; return f->impl->get_selected(out, nq); }
@@ -281,7 +311,7 @@ int fl_filter_upload_state(fl_filter_t* f, const double* x26, const double* P, d
     if (!x26 || !P) return FL_ERR_ARG;
     return f->impl->upload_state(x26, P, R);
 }
-int fl_filter_run(fl_filter_t* f) { FILTER_GUARD(f); return f->impl->run_passes(); }
+int fl_filter_run(fl_filter_t* f) { FILTER_HOST_GUARD(f); return f->impl->run_passes(); }
 int fl_filter_download_state(fl_filter_t* f, double* x26, double* P, int* n_pass) { FILTER_GUARD(f); return f->impl->download_state(x26, P, n_pass); }
 int fl_filter_sync(fl_filter_t* f) { FILTER_GUARD(f); return f->impl->sync(); }
 int fl_filter_debug_prof(fl_filter_t* f, long long* out16) {
@@ -423,7 +453,7 @@ int fl_scan_download(fl_scan_t* s, int which, float* out_xyzi, int cap) {
     return rc == FL_OK ? n : rc;
 }
 int fl_filter_update_scan(fl_filter_t* f, fl_scan_t* s, double* x26, double* P, double R, double* solve_time_s) {
-    FILTER_GUARD(f);
+    FILTER_HOST_GUARD(f);
     if (!s || !s->impl || s->map != f->map) { fl::set_last_error("fl_filter_update_scan: the scan must live on the filter's map"); return FL_ERR_ARG; }
     return f->impl->update_device(s->impl->down_device(), s->impl->down_count(), x26, P, R, solve_time_s);
 }

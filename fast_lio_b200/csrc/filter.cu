@@ -1217,6 +1217,16 @@ int Filter::reserve(int nq) {
     scan_.plane = plane_.as<float4>();
     FL_CHECK(srange_.reserve(sizeof(double) * (size_t)nq));
     scan_.srange = srange_.as<double>();
+    // map_incremental's buffers, so that its device form never allocates for a scan within capacity()
+    FL_CHECK(mi_world_.reserve(sizeof(float4) * (size_t)nq));
+    FL_CHECK(mi_flag_add_.reserve((size_t)nq));
+    FL_CHECK(mi_flag_no_.reserve((size_t)nq));
+    FL_CHECK(mi_list_add_.reserve(sizeof(float4) * (size_t)nq));
+    FL_CHECK(mi_list_no_.reserve(sizeof(float4) * (size_t)nq));
+    FL_CHECK(mi_counts_.reserve(sizeof(int) * 2));
+    size_t tmp = 0;
+    FL_CUDA(cub::DeviceSelect::Flagged(nullptr, tmp, (const float4*)nullptr, (const unsigned char*)nullptr, (float4*)nullptr, (int*)nullptr, nq));
+    FL_CHECK(mi_tmp_.reserve(tmp));
     return FL_OK;
 }
 
@@ -1508,6 +1518,9 @@ int Filter::capacity() const {
     c = std::min(c, normvec_.bytes / sizeof(float4));
     c = std::min(c, plane_.bytes / sizeof(float4));
     c = std::min(c, srange_.bytes / sizeof(double));
+    c = std::min(c, mi_world_.bytes / sizeof(float4));
+    c = std::min(c, std::min(mi_flag_add_.bytes, mi_flag_no_.bytes));
+    c = std::min(c, std::min(mi_list_add_.bytes, mi_list_no_.bytes) / sizeof(float4));
     return (int)std::min<size_t>(c, INT_MAX);
 }
 
@@ -1625,6 +1638,42 @@ int Filter::map_incremental(double fsm, int ekf_inited, int* n_to_add, int* n_no
     FL_CHECK(map_->add_points_device(mi_list_no_.as<float4>(), counts[1], false, &b));      // :471
     if (added) *added = a;
     return FL_OK;
+}
+
+int Filter::map_incremental_on_stream(double fsm, int ekf_inited, int* d_out4, cudaStream_t st) {
+    const int dev = map_->device();
+    if (!device_ptr(d_out4, dev, 4)) { set_last_error("map_incremental_device: out4 must be 4-byte aligned device memory on device %d", dev); return FL_ERR_ARG; }
+    if (!(fsm > 0.0)) { set_last_error("map_incremental_device: filter_size_map_min must be > 0"); return FL_ERR_ARG; }
+    FL_CHECK(device_form_scope("map_incremental_device", false));
+    const int nq = scan_.Q;
+    FL_CUDA(cudaSetDevice(dev));
+    size_t tmp = 0;
+    FL_CUDA(cub::DeviceSelect::Flagged(nullptr, tmp, (const float4*)nullptr, (const unsigned char*)nullptr, (float4*)nullptr, (int*)nullptr, nq, st));
+    if (nq > capacity() || tmp > mi_tmp_.bytes) {
+        set_last_error("map_incremental_device: the bound scan of %d points exceeds the filter's capacity of %d", nq, capacity());
+        return FL_ERR_CAPACITY;
+    }
+    if (nq <= 0) {                                      // the host form inserts nothing either: (0, 0, 0, FL_OK)
+        bool joined = false;
+        FL_CHECK(map_->query_begin(st, &joined));
+        FL_CUDA(cudaMemsetAsync(d_out4, 0, 4 * sizeof(int), st));
+        return map_->query_end(st, joined);
+    }
+    FL_CHECK(map_->async_prepare(nq, st, "map_incremental_device"));
+    bool joined = false;
+    FL_CHECK(map_->mutation_begin(st, &joined));
+    k_map_incremental<<<(nq + 255) / 256, 256, 0, st>>>(scan_, ctl_.as<FilterCtl>(), fsm, ekf_inited, mi_world_.as<float4>(),
+                                                       mi_flag_add_.as<unsigned char>(), mi_flag_no_.as<unsigned char>());
+    FL_CUDA(cudaGetLastError());
+    tmp = mi_tmp_.bytes;
+    FL_CUDA(cub::DeviceSelect::Flagged(mi_tmp_.ptr, tmp, mi_world_.as<float4>(), mi_flag_add_.as<unsigned char>(), mi_list_add_.as<float4>(),
+                                       mi_counts_.as<int>(), nq, st));
+    tmp = mi_tmp_.bytes;
+    FL_CUDA(cub::DeviceSelect::Flagged(mi_tmp_.ptr, tmp, mi_world_.as<float4>(), mi_flag_no_.as<unsigned char>(), mi_list_no_.as<float4>(),
+                                       mi_counts_.as<int>() + 1, nq, st));
+    const int* counts = mi_counts_.as<int>();
+    FL_CHECK(map_->add_points_async(mi_list_add_.as<float4>(), counts, true, mi_list_no_.as<float4>(), counts + 1, nq, counts, d_out4, st));   // :470-471
+    return map_->mutation_end(st, joined);
 }
 
 int Filter::get_nearest(float* out_pts, int* out_cnt, int nq) {

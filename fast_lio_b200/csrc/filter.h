@@ -105,6 +105,10 @@ public:
     // map_incremental (laserMapping.cpp:427-474) on the device: classify every scan point with the final
     // state and its cached neighbours, then Add_Points(PointToAdd, true) + Add_Points(PointNoNeedDownsample, false)
     int map_incremental(double filter_size_map_min, int ekf_inited, int* n_to_add, int* n_no_downsample, int* added);
+    // the same on the caller's stream `st` (fl_filter_map_incremental_device): the classification and the compaction of the bound
+    // scan, then both Add_Points as one all-or-nothing device-form call of the map (Map::add_points_async, n_max = the scan's
+    // size); out4 = (|PointToAdd|, |PointNoNeedDownsample|, Add_Points(PointToAdd, true), status).  No host synchronisation.
+    int map_incremental_on_stream(double filter_size_map_min, int ekf_inited, int* d_out4, cudaStream_t st);
     int get_nearest(float* out_pts, int* out_cnt, int nq);
     // multi-GPU: Nearest_Points of the points outside this rank's shard (searched by their own rank during the update) are
     // recomputed here, with the state of the last searching pass, before anything reads the whole scan's neighbours

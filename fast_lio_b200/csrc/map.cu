@@ -43,7 +43,12 @@ void DeviceBuffer::release() {
 
 // counters_ layout
 enum Counter { C_LEAF_USED = 0, C_DELETED, C_ADDED, C_GROUPS, C_NINSERT, C_TOMB, C_ERROR, C_COMPACT,
-               C_DIR_CELLS, C_DIR_POOL, C_DIR_CROWDED, C_DIR_ERROR, C_DIR_WALKED, C_REMOVED, C_REVIVED, C_NFIX, C_COUNT = 16 };
+               C_DIR_CELLS, C_DIR_POOL, C_DIR_CROWDED, C_DIR_ERROR, C_DIR_WALKED, C_REMOVED, C_REVIVED, C_NFIX,
+               // device forms of Add_Points: validnum / lazily deleted points (n_valid_, n_tomb_ on the device), the batch
+               // sizes as read (RA, RB) and as applied (NA, NB: 0 when the plan refused), the plan's counts, its verdict, and
+               // "maintenance due" (the host form would have re-packed or re-listed); C_REFUSED: a call was refused since the last
+               // fl_map_maintain (sticky, unlike C_SKIP), C_NEED: the list-pool need the plan last computed
+               C_VALID, C_TOMBS, C_RA, C_RB, C_NA, C_NB, C_MISS, C_FIXES, C_SKIP, C_DUE, C_REFUSED, C_NEED, C_COUNT = 32 };
 
 // ============================================================================= kernels
 // ----------------------------------------------------------------------------- k-d partition build
@@ -302,11 +307,18 @@ __global__ void k_halo_fill(MapView m, int n_leaf_used) {
         }
     }
 }
+// The batch size of a kernel of Add_Points: n (host form), or *n_dev clamped to [0, n] (device forms: n is the n_max the grid
+// was sized from, *n_dev the count some earlier kernel of the call left in device memory).
+__device__ __forceinline__ int batch_count(int n, const int* __restrict__ n_dev) {
+    return n_dev ? min(max(*n_dev, 0), n) : n;
+}
 // incremental, two kernels (claim, then append) so that nobody waits for a list that is still being set up.
 // One warp per inserted point, lane t < 27 its t-th cell.  slots[i] < 0: the point could not be placed.
-__global__ void __launch_bounds__(256) k_halo_claim(MapView m, const float4* __restrict__ pts, const int* __restrict__ slots, int n, int* counters) {
+__global__ void __launch_bounds__(256) k_halo_claim(MapView m, const float4* __restrict__ pts, const int* __restrict__ slots, int n,
+                                                     const int* __restrict__ n_dev, int* counters) {
     const int lane = threadIdx.x & 31;
     const int warps = (gridDim.x * blockDim.x) >> 5;
+    n = batch_count(n, n_dev);
     for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
         if (slots[i] < 0 || lane >= 27) continue;
         bool fresh = false;
@@ -319,10 +331,11 @@ __global__ void __launch_bounds__(256) k_halo_claim(MapView m, const float4* __r
         E.cnt_cap = (unsigned)HALO_NEW_CAP << 16;
     }
 }
-__global__ void __launch_bounds__(256) k_halo_append(MapView m, const float4* __restrict__ pts, const int* __restrict__ slots, int n, int* counters,
-                                                      unsigned* __restrict__ fix, int fix_cap) {
+__global__ void __launch_bounds__(256) k_halo_append(MapView m, const float4* __restrict__ pts, const int* __restrict__ slots, int n,
+                                                      const int* __restrict__ n_dev, int* counters, unsigned* __restrict__ fix, int fix_cap) {
     const int lane = threadIdx.x & 31;
     const int warps = (gridDim.x * blockDim.x) >> 5;
+    n = batch_count(n, n_dev);
     for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
         const int slot = slots[i];
         if (slot < 0 || lane >= 27) continue;
@@ -569,13 +582,18 @@ __device__ __forceinline__ unsigned long long voxel_key(const float4& p, float d
     }
     return key;
 }
+// Real keys use bits 0-62 (and reach 2^63 - 1 where the coordinates clamp).  Device forms sort all n_max rows: rows past the
+// batch get PAD_KEY, which sorts after every real key, so the first n sorted rows are those of the host form's sort of n rows.
+constexpr unsigned long long PAD_KEY = 1ull << 63;
 __global__ void k_voxel_keys(const float4* __restrict__ pts, int n, float ds, unsigned long long* __restrict__ keys,
-                             unsigned* __restrict__ vals) {
+                             unsigned* __restrict__ vals, const int* __restrict__ n_dev) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) { keys[i] = voxel_key(pts[i], ds); vals[i] = (unsigned)i; }
+    if (i < n) { keys[i] = i < batch_count(n, n_dev) ? voxel_key(pts[i], ds) : PAD_KEY; vals[i] = (unsigned)i; }
 }
-__global__ void k_group_heads(const unsigned long long* __restrict__ keys, int n, int* __restrict__ group_start, int* counters) {
+__global__ void k_group_heads(const unsigned long long* __restrict__ keys, int n, int* __restrict__ group_start, int* counters,
+                              const int* __restrict__ n_dev) {
     int r = blockIdx.x * blockDim.x + threadIdx.x;
+    n = batch_count(n, n_dev);
     if (r < n && (r == 0 || keys[r] != keys[r - 1])) group_start[atomicAdd(&counters[C_GROUPS], 1)] = r;
 }
 
@@ -620,7 +638,8 @@ __device__ __forceinline__ bool same_point(const float4& a, const float4& b) {  
     return fabs((double)a.x - (double)b.x) < 1e-6 && fabs((double)a.y - (double)b.y) < 1e-6 && fabs((double)a.z - (double)b.z) < 1e-6;
 }
 
-// One warp per touched voxel.  Reproduces the sequential per-point semantics of
+// One warp per touched voxel (device forms: rows past the batch carry PAD_KEY, which no group's key equals, so a group never
+// runs into them and n may be n_max).  Reproduces the sequential per-point semantics of
 // Add_Points(downsample_on = true) (ikd_Tree.cpp:489-521) for all batch points that fall
 // into the voxel, in their original order (the sort is stable).
 __global__ void __launch_bounds__(256) k_downsample_resolve(MapView m, const float4* __restrict__ batch,
@@ -678,9 +697,11 @@ __global__ void __launch_bounds__(256) k_downsample_resolve(MapView m, const flo
 // One warp per new point: descend towards the nearest child box to the home leaf, claim a free slot there or
 // in its overflow chain (allocating a chain leaf from the pool if needed), publish the point
 // and grow the AABBs on the root path with float atomics ("partial refit").
-__global__ void __launch_bounds__(256) k_insert(MapView m, const float4* __restrict__ pts, int n, int* counters, int* __restrict__ slot_out) {
+__global__ void __launch_bounds__(256) k_insert(MapView m, const float4* __restrict__ pts, int n, const int* __restrict__ n_dev, int* counters,
+                                                 int* __restrict__ slot_out) {
     const int lane = threadIdx.x & 31;
     const int warps = (gridDim.x * blockDim.x) >> 5;
+    n = batch_count(n, n_dev);
     for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
         const float4 p = pts[i];
         int node = 0;
@@ -753,6 +774,114 @@ __global__ void __launch_bounds__(256) k_insert(MapView m, const float4* __restr
             e /= FAN;
         }
     }
+}
+
+// ----------------------------------------------------------------------------- Add_Points on the caller's stream
+// The device forms cannot re-pack or re-list after the fact (the pinned searches would answer from incomplete halo lists in
+// between), so a plan decides before anything is written whether the whole call fits the room left, and every kernel of the call
+// then runs over the count the plan let through: 0 when it refused.
+constexpr int HALO_FIX_MAX = (HALO_MAX + HALO_MAX / 2 + 3) & ~3;      // the largest list k_halo_fix makes
+
+__global__ void k_plan_begin(int* counters, const int* __restrict__ na, const int* __restrict__ nb, int n_max) {
+    counters[C_RA] = min(max(*na, 0), n_max);
+    counters[C_RB] = nb ? min(max(*nb, 0), n_max) : 0;
+    counters[C_MISS] = 0;
+    counters[C_FIXES] = 0;
+}
+// The list-pool need of a batch, counted over every (point, halo cell) pair of the batch (a superset of what the inserts append).
+// k_plan_count: a pair whose cell has no entry yet may claim a fresh list (HALO_NEW_CAP); the pairs of a listed cell are counted
+// in cellcnt (one int per table entry, all zero between calls).  k_plan_reset, after the counts of both lists: the first pair of
+// a cell to take its count back to zero judges the cell.  Its list overflows when the count exceeds the free places; k_halo_fix
+// then makes one new list (per insert) for the live points of the block, which are all listed already or in this batch, so at
+// most L = listed + count of them.  C_FIXES: the need of those lists, in units of 16 ints.
+__global__ void __launch_bounds__(256) k_plan_count(MapView m, const float4* __restrict__ pts, int n, const int* __restrict__ n_dev,
+                                                     int* counters, int* __restrict__ cellcnt) {
+    const int lane = threadIdx.x & 31;
+    const int warps = (gridDim.x * blockDim.x) >> 5;
+    n = batch_count(n, n_dev);
+    for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
+        bool miss = false;
+        if (lane < 27) {
+            const unsigned e = dir_find(m.dir, halo_key(m.dir, pts[i], lane));
+            if (e == 0xffffffffu) miss = true;
+            else if (m.dir.tab[e].start >= 0) atomicAdd(&cellcnt[e], 1);
+        }
+        const unsigned mm = __ballot_sync(FULL, miss);
+        if (lane == 0 && mm) atomicAdd(&counters[C_MISS], __popc(mm));
+    }
+}
+__global__ void __launch_bounds__(256) k_plan_reset(MapView m, const float4* __restrict__ pts, int n, const int* __restrict__ n_dev,
+                                                     int* counters, int* __restrict__ cellcnt, int inserts) {
+    const int lane = threadIdx.x & 31;
+    const int warps = (gridDim.x * blockDim.x) >> 5;
+    n = batch_count(n, n_dev);
+    for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
+        if (lane >= 27) continue;
+        const unsigned e = dir_find(m.dir, halo_key(m.dir, pts[i], lane));
+        if (e == 0xffffffffu) continue;
+        const int t = atomicExch(&cellcnt[e], 0);
+        const CellEntry E = m.dir.tab[e];
+        if (t == 0 || E.start < 0) continue;
+        const int listed = (int)(E.cnt_cap & 0xffffu), free_ = (int)(E.cnt_cap >> 16) - listed;
+        if (t <= free_) continue;
+        const int L = listed + t;
+        const int room = min(HALO_FIX_MAX, (L + max(16, L / 2) + 3) & ~3);
+        const int fixes = 1 + (inserts > 1 && t > free_ + 16);            // a second insert overflows the new list's >= 16 free places
+        atomicAdd(&counters[C_FIXES], fixes * ((room + 15) / 16));
+    }
+}
+// The host form's guards before an insert, for the whole call at once, in terms of the batch size (nothing is tombstoned yet):
+// overflow leaves for one fresh leaf per point, the table below 90 % load, the list pool for the counted need.  The fix list is
+// sized for 27 entries per point and cannot overflow.
+__global__ void k_plan(MapView m, int* counters) {
+    const long long n = (long long)counters[C_RA] + counters[C_RB];
+    bool ok = counters[C_LEAF_USED] + n <= m.leaf_cap;
+    if (m.dir.cap) {
+        ok = ok && ((long long)counters[C_DIR_CELLS] + 27 * n) * 10 <= (long long)m.dir.cap * 9;
+        const long long miss = counters[C_MISS];
+        // fresh cells: a fresh list of HALO_NEW_CAP each, and a new list for each (per insert) that more than HALO_NEW_CAP pairs hit
+        const long long need = miss * HALO_NEW_CAP + 16ll * counters[C_FIXES] + 2 * (miss / (HALO_NEW_CAP + 1)) * HALO_FIX_MAX;
+        ok = ok && counters[C_DIR_POOL] + need <= m.dir.lists_cap;
+        counters[C_NEED] = (int)min(need, (long long)INT_MAX);
+    }
+    counters[C_SKIP] = !ok;
+    if (!ok) counters[C_REFUSED] = 1;
+    counters[C_NA] = ok ? counters[C_RA] : 0;
+    counters[C_NB] = ok ? counters[C_RB] : 0;
+    counters[C_ADDED] = counters[C_GROUPS] = counters[C_NINSERT] = counters[C_TOMB] = 0;
+}
+// After one Add_Points of the call: the host form's bookkeeping of n_valid_ / n_tomb_ (add_points_host) and its decisions after
+// the insert (insert_device's re-list of a full or crowded directory, maybe_rebuild), which here only mark maintenance as due.
+__global__ void k_async_account(MapView m, int* counters, int slot, bool downsample_on, int chain_limit) {
+    const int batch = counters[slot];
+    if (batch == 0) return;
+    int inserted = batch;
+    if (downsample_on) {
+        const int tomb = counters[C_TOMB];
+        inserted = counters[C_NINSERT];
+        counters[C_VALID] -= tomb;
+        counters[C_TOMBS] += tomb;
+    }
+    counters[C_VALID] += inserted;
+    bool due = false;
+    if (inserted > 0 && m.dir.cap) due = counters[C_DIR_ERROR] || counters[C_DIR_CROWDED] > max(64, counters[C_DIR_CELLS] / 1024);
+    if (downsample_on) counters[C_TOMBS] = max(0, counters[C_TOMBS] - inserted);
+    const int tombs = counters[C_TOMBS];
+    due = due || counters[C_LEAF_USED] - m.n_main > chain_limit || (tombs > 1024 && tombs > counters[C_VALID]) || counters[C_ERROR];
+    if (due) counters[C_DUE] = 1;
+}
+// status2 = (status, added), or out4 = (list_counts[0], list_counts[1], added, status)
+__global__ void k_async_status(const int* __restrict__ counters, const int* __restrict__ list_counts, int* __restrict__ out) {
+    const bool skip = counters[C_SKIP] != 0;
+    const int st = skip ? FL_ERR_CAPACITY : (counters[C_DUE] ? 1 : FL_OK);
+    const int added = skip ? 0 : counters[C_ADDED];
+    if (list_counts) { out[0] = list_counts[0]; out[1] = list_counts[1]; out[2] = added; out[3] = st; }
+    else { out[0] = st; out[1] = added; }
+}
+__global__ void k_set_counts(int* counters, int valid, int tomb, int due) {
+    counters[C_VALID] = valid;
+    counters[C_TOMBS] = tomb;
+    counters[C_DUE] = due;
 }
 
 // ----------------------------------------------------------------------------- Box_Search / Radius_Search
@@ -991,6 +1120,8 @@ Map::~Map() {
     src_.release(); keys_in_.release(); keys_out_.release(); vals_in_.release(); vals_out_.release();
     cub_tmp_.release(); scratch_.release(); scratch2_.release(); scratch3_.release();
     range_ws_.release(); range_out_.release();
+    a_keys_in_.release(); a_keys_out_.release(); a_vals_in_.release(); a_vals_out_.release(); a_groups_.release(); a_ins_.release();
+    a_slots_.release(); a_fix_.release(); a_cub_.release(); cellcnt_.release();
     if (h_counters_) cudaFreeHost(h_counters_);
     if (ev_front_) cudaEventDestroy(ev_front_);
     if (ev_caller_) cudaEventDestroy(ev_caller_);
@@ -1112,6 +1243,8 @@ int Map::build_from_sorted(const float4* d_src, int n) {
     n_valid_ = n;
     n_tomb_ = 0;
     built_ = true;
+    layout_dirty_ = true;
+    FL_CHECK(publish_counts());
     return build_directory();
 }
 
@@ -1155,6 +1288,11 @@ int Map::build_directory() {
         FL_CUDA(cudaMemcpyAsync(&h_counters_[C_DIR_CELLS], &d_cnt[C_DIR_CELLS], sizeof(int) * 4, cudaMemcpyDeviceToHost, stream_));
         FL_CUDA(cudaStreamSynchronize(stream_));
         if (h_counters_[C_DIR_ERROR]) { dir_min_pool_ = std::max<size_t>(dir_min_pool_ * 2, (size_t)HALO_NEW_CAP * 262144); continue; }
+        layout_dirty_ = true;
+        if (async_used_) {          // the plan's per-entry counters (k_plan_count): one int per table entry, all zero
+            FL_CHECK(cellcnt_.reserve(sizeof(int) * (size_t)v_.dir.cap));
+            FL_CUDA(cudaMemsetAsync(cellcnt_.ptr, 0, cellcnt_.bytes, stream_));
+        }
         return FL_OK;
     }
     set_last_error("cell directory: could not size the table");
@@ -1259,6 +1397,7 @@ int Map::delete_boxes(const float* boxes6, int nb, int* deleted) {
         n_valid_ -= d; n_tomb_ += d;
         FL_CHECK(refit());          // tighten every AABB ("box-delete by refit")
         FL_CHECK(maybe_rebuild());
+        FL_CHECK(publish_counts());
     }
     if (deleted) *deleted = d;
     return FL_OK;
@@ -1301,6 +1440,7 @@ int Map::add_boxes(const float* boxes6, int nb, int* revived) {
     if (r > 0) {
         n_valid_ += r; n_tomb_ = std::max(0, n_tomb_ - r);
         FL_CHECK(refit());          // the boxes were tightened when the points went away
+        FL_CHECK(publish_counts());
     }
     if (revived) *revived = r;
     return FL_OK;
@@ -1611,12 +1751,12 @@ int Map::insert_device(const float4* d_pts, int n) {
         }
     }
     FL_CHECK(ins_slots_.reserve(sizeof(int) * (size_t)n));
-    k_insert<<<blocks_for((long long)n * 32, 256), 256, 0, stream_>>>(v_, d_pts, n, counters_.as<int>(), ins_slots_.as<int>());
+    k_insert<<<blocks_for((long long)n * 32, 256), 256, 0, stream_>>>(v_, d_pts, n, nullptr, counters_.as<int>(), ins_slots_.as<int>());
     if (v_.dir.cap) {
-        k_halo_claim<<<blocks_for((long long)n * 32, 256), 256, 0, stream_>>>(v_, d_pts, ins_slots_.as<int>(), n, counters_.as<int>());
+        k_halo_claim<<<blocks_for((long long)n * 32, 256), 256, 0, stream_>>>(v_, d_pts, ins_slots_.as<int>(), n, nullptr, counters_.as<int>());
         FL_CHECK(dir_fix_.reserve(sizeof(unsigned) * 65536));
         FL_CUDA(cudaMemsetAsync(&counters_.as<int>()[C_NFIX], 0, sizeof(int), stream_));
-        k_halo_append<<<blocks_for((long long)n * 32, 256), 256, 0, stream_>>>(v_, d_pts, ins_slots_.as<int>(), n, counters_.as<int>(),
+        k_halo_append<<<blocks_for((long long)n * 32, 256), 256, 0, stream_>>>(v_, d_pts, ins_slots_.as<int>(), n, nullptr, counters_.as<int>(),
                                                                                  dir_fix_.as<unsigned>(), 65536);
         k_halo_fix<<<296, 256, 0, stream_>>>(v_, dir_fix_.as<unsigned>(), 65536, counters_.as<int>());
     }
@@ -1638,6 +1778,11 @@ int Map::insert_device(const float4* d_pts, int n) {
 }
 
 int Map::add_points_device(const float4* d_pts, int n, bool downsample_on, int* added) {
+    FL_CHECK(add_points_host(d_pts, n, downsample_on, added));
+    return publish_counts();
+}
+
+int Map::add_points_host(const float4* d_pts, int n, bool downsample_on, int* added) {
     if (added) *added = 0;
     if (n < 0) { set_last_error("add_points: n < 0"); return FL_ERR_ARG; }
     if (n == 0) return FL_OK;
@@ -1654,7 +1799,7 @@ int Map::add_points_device(const float4* d_pts, int n, bool downsample_on, int* 
     FL_CHECK(scratch3_.reserve(sizeof(float4) * (size_t)n));       // insert list
     int* d_cnt = counters_.as<int>();
     FL_CUDA(cudaMemsetAsync(&d_cnt[C_ADDED], 0, sizeof(int) * 4, stream_));   // ADDED, GROUPS, NINSERT, TOMB
-    k_voxel_keys<<<blocks_for(n, 256, 1 << 30), 256, 0, stream_>>>(d_pts, n, downsample_, keys_in_.as<unsigned long long>(), vals_in_.as<unsigned>());
+    k_voxel_keys<<<blocks_for(n, 256, 1 << 30), 256, 0, stream_>>>(d_pts, n, downsample_, keys_in_.as<unsigned long long>(), vals_in_.as<unsigned>(), nullptr);
     size_t tmp = 0;
     FL_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp, keys_in_.as<unsigned long long>(), keys_out_.as<unsigned long long>(),
                                             vals_in_.as<unsigned>(), vals_out_.as<unsigned>(), n, 0, 63, stream_));
@@ -1662,7 +1807,7 @@ int Map::add_points_device(const float4* d_pts, int n, bool downsample_on, int* 
     tmp = cub_tmp_.bytes;
     FL_CUDA(cub::DeviceRadixSort::SortPairs(cub_tmp_.ptr, tmp, keys_in_.as<unsigned long long>(), keys_out_.as<unsigned long long>(),
                                             vals_in_.as<unsigned>(), vals_out_.as<unsigned>(), n, 0, 63, stream_));
-    k_group_heads<<<blocks_for(n, 256, 1 << 30), 256, 0, stream_>>>(keys_out_.as<unsigned long long>(), n, scratch2_.as<int>(), d_cnt);
+    k_group_heads<<<blocks_for(n, 256, 1 << 30), 256, 0, stream_>>>(keys_out_.as<unsigned long long>(), n, scratch2_.as<int>(), d_cnt, nullptr);
     k_downsample_resolve<<<blocks_for((long long)n * 32, 256), 256, 0, stream_>>>(
         v_, d_pts, keys_out_.as<unsigned long long>(), vals_out_.as<unsigned>(), n, scratch2_.as<int>(), downsample_,
         scratch3_.as<float4>(), d_cnt);
@@ -1686,6 +1831,222 @@ int Map::add_points(const float* pts_xyzi, int n, bool downsample_on, int* added
     FL_CHECK(scratch_.reserve(sizeof(float4) * (size_t)n));
     FL_CUDA(cudaMemcpyAsync(scratch_.ptr, pts_xyzi, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, stream_));
     return add_points_device(scratch_.as<float4>(), n, downsample_on, added);
+}
+
+// ----------------------------------------------------------------------------- device forms of Add_Points
+int Map::publish_counts() {
+    k_set_counts<<<1, 1, 0, stream_>>>(counters_.as<int>(), n_valid_, n_tomb_, due_ ? 1 : 0);
+    FL_CUDA(cudaGetLastError());
+    return FL_OK;
+}
+
+int Map::settle(bool full, int* layout_changed) {
+    FL_CUDA(cudaSetDevice(device_));
+    if (pending_ || captured_) {
+        // the device forms' work reached the handle's stream through mutation_end; graph replays the caller has synchronised
+        FL_CUDA(cudaMemcpyAsync(h_counters_, counters_.ptr, sizeof(int) * C_COUNT, cudaMemcpyDeviceToHost, stream_));
+        FL_CUDA(cudaStreamSynchronize(stream_));
+        n_valid_ = h_counters_[C_VALID];
+        n_tomb_ = h_counters_[C_TOMBS];
+        ub_n_ = 0;
+        // what is owed survives read-only settles: only a full settle does it and clears it
+        due_ = due_ || h_counters_[C_DUE] != 0;
+        refused_ = refused_ || h_counters_[C_REFUSED] != 0;
+        pending_ = false;
+    }
+    if (full && (due_ || refused_)) {
+        // what the host form would have done after its inserts (insert_device, maybe_rebuild), then room for a refused call
+        if (v_.dir.cap) {
+            const bool crowded = h_counters_[C_DIR_CROWDED] > std::max(64, h_counters_[C_DIR_CELLS] / 1024);
+            if (h_counters_[C_DIR_ERROR]) {
+                dir_min_cap_ = std::max(dir_min_cap_, (size_t)v_.dir.cap + (size_t)v_.dir.cap / 2);
+                dir_min_pool_ = std::max<size_t>(dir_min_pool_ * 2, (size_t)HALO_NEW_CAP * 262144);
+            }
+            if (h_counters_[C_DIR_ERROR] || crowded) { n_dir_rebuilds_++; FL_CHECK(build_directory()); }
+        }
+        FL_CHECK(maybe_rebuild());
+        if (refused_) FL_CHECK(async_grow(async_n_max_, true));
+        due_ = refused_ = false;
+        h_counters_[C_REFUSED] = 0;
+        FL_CUDA(cudaMemsetAsync(&counters_.as<int>()[C_REFUSED], 0, sizeof(int), stream_));
+        FL_CHECK(publish_counts());          // C_DUE = 0
+        FL_CUDA(cudaStreamSynchronize(stream_));
+    }
+    if (layout_changed) { *layout_changed = layout_dirty_ ? 1 : 0; layout_dirty_ = false; }
+    return FL_OK;
+}
+
+// the host's bound: the call fits when the points of every device-form call since the last settle and n_max more could each take
+// one fresh leaf and claim 27 fresh cells with the table below 90 % load -- insert_device's two guards.  The list pool's need
+// has no useful bound on the host (up to 27 fresh lists per point); the plan kernel checks it on the device.
+bool Map::async_fits(long long n_max) const {
+    const long long n = ub_n_ + n_max;
+    if (h_counters_[C_LEAF_USED] + n > v_.leaf_cap) return false;
+    return !v_.dir.cap || (h_counters_[C_DIR_CELLS] + 27 * n) * 10 <= (long long)v_.dir.cap * 9;
+}
+
+// Room for one call of n_max points, by insert_device's rules (a re-pack with a larger overflow pool, a re-list with a larger
+// table); after a refused call (pool = true) also a re-list with a larger list pool when the need the plan last computed does
+// not fit it.  Synchronous; the map must be settled.
+int Map::async_grow(int n_max, bool pool) {
+    const long long n = std::max(n_max, 1);
+    if (h_counters_[C_LEAF_USED] + n > v_.leaf_cap) {
+        min_pool_ = (int)std::min<long long>(std::max<long long>(min_pool_, n + 1024), INT_MAX / 2);
+        FL_CHECK(rebuild());
+    }
+    if (v_.dir.cap) {
+        const long long cells = (long long)h_counters_[C_DIR_CELLS] + 27 * n;
+        const bool grow_cap = cells * 10 > (long long)v_.dir.cap * 9;
+        const long long need = std::max<long long>(h_counters_[C_NEED], 0);
+        const bool grow_pool = pool && (long long)h_counters_[C_DIR_POOL] + need > v_.dir.lists_cap;
+        if (grow_cap) dir_min_cap_ = std::max(dir_min_cap_, (size_t)cells * 2 + 16384);
+        if (grow_pool) dir_min_pool_ = std::max<size_t>(dir_min_pool_ * 2, 2 * (size_t)need);
+        if (grow_cap || grow_pool) { n_dir_rebuilds_++; FL_CHECK(build_directory()); }
+    }
+    FL_CUDA(cudaStreamSynchronize(stream_));
+    return publish_counts();
+}
+
+// Scratch of a device-form call of n_max points (its own buffers: a host-form call never moves what a graph captured)
+int Map::async_scratch(int n_max, bool may_allocate) {
+    const size_t n = (size_t)std::max(n_max, 1);
+    size_t sort_bytes = 0;
+    FL_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                            (unsigned*)nullptr, (unsigned*)nullptr, (int)n, 0, 64, stream_));
+    struct Want { DeviceBuffer* b; size_t bytes; } want[] = {
+        {&a_keys_in_, sizeof(unsigned long long) * n}, {&a_keys_out_, sizeof(unsigned long long) * n}, {&a_vals_in_, sizeof(unsigned) * n},
+        {&a_vals_out_, sizeof(unsigned) * n}, {&a_groups_, sizeof(int) * n}, {&a_ins_, sizeof(float4) * n}, {&a_slots_, sizeof(int) * n},
+        {&a_fix_, sizeof(unsigned) * 27 * n}, {&a_cub_, sort_bytes}, {&cellcnt_, sizeof(int) * (size_t)v_.dir.cap}};
+    bool short_ = false;
+    for (const Want& w : want) short_ = short_ || w.b->bytes < w.bytes;
+    if (!short_) return FL_OK;
+    if (!may_allocate) return FL_ERR_CAPACITY;
+    FL_CUDA(cudaStreamSynchronize(stream_));          // nothing in flight may still use a buffer that moves
+    for (const Want& w : want) {
+        if (w.b->bytes >= w.bytes) continue;
+        if (w.b->ptr) layout_dirty_ = true;
+        FL_CHECK(w.b->reserve(w.bytes));
+        if (w.b == &cellcnt_) FL_CUDA(cudaMemsetAsync(cellcnt_.ptr, 0, cellcnt_.bytes, stream_));
+    }
+    return FL_OK;
+}
+
+int Map::async_prepare(int n_max, cudaStream_t st, const char* what) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    FL_CUDA(cudaStreamGetCaptureInfo(st, &cs));
+    const bool capturing = cs != cudaStreamCaptureStatusNone;
+    async_used_ = true;
+    async_n_max_ = std::max(async_n_max_, n_max);
+    if (capturing) {
+        if (!async_fits(n_max)) {
+            set_last_error("%s: %d points might not fit the map's headroom; call fl_map_maintain (or the call once outside capture) first", what, n_max);
+            return FL_ERR_CAPACITY;
+        }
+        if (async_scratch(n_max, false) != FL_OK) {
+            set_last_error("%s: no scratch for %d points yet; make the call once outside capture first", what, n_max);
+            return FL_ERR_CAPACITY;
+        }
+        return FL_OK;
+    }
+    if (!async_fits(n_max)) {                  // the one synchronous case: settle, and grow when the settled map has no room either
+        FL_CHECK(settle(false));
+        if (!async_fits(n_max)) FL_CHECK(async_grow(n_max, false));
+    }
+    return async_scratch(n_max, true);
+}
+
+int Map::mutation_begin(cudaStream_t st, bool* joined) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    FL_CUDA(cudaStreamGetCaptureInfo(st, &cs));
+    *joined = cs == cudaStreamCaptureStatusNone;
+    if (!*joined) { captured_ = true; return FL_OK; }
+    // a mutation waits for everything enqueued on the handle so far, device queries joined from other streams included
+    FL_CUDA(cudaEventRecord(ev_front_, stream_));
+    FL_CUDA(cudaStreamWaitEvent(st, ev_front_, 0));
+    return FL_OK;
+}
+int Map::mutation_end(cudaStream_t st, bool joined) {
+    pending_ = true;
+    touch();
+    return query_end(st, joined);
+}
+
+int Map::enqueue_insert(const float4* pts, const int* n_dev, int n_max, cudaStream_t st) {
+    const int g = blocks_for((long long)n_max * 32, 256);
+    int* d_cnt = counters_.as<int>();
+    k_insert<<<g, 256, 0, st>>>(v_, pts, n_max, n_dev, d_cnt, a_slots_.as<int>());
+    if (v_.dir.cap) {
+        const int fix_cap = (int)std::min<long long>(27ll * n_max, INT_MAX);
+        k_halo_claim<<<g, 256, 0, st>>>(v_, pts, a_slots_.as<int>(), n_max, n_dev, d_cnt);
+        FL_CUDA(cudaMemsetAsync(&d_cnt[C_NFIX], 0, sizeof(int), st));
+        k_halo_append<<<g, 256, 0, st>>>(v_, pts, a_slots_.as<int>(), n_max, n_dev, d_cnt, a_fix_.as<unsigned>(), fix_cap);
+        k_halo_fix<<<296, 256, 0, st>>>(v_, a_fix_.as<unsigned>(), fix_cap, d_cnt);
+    }
+    FL_CUDA(cudaGetLastError());
+    return FL_OK;
+}
+
+// add_points_host on the device: the batch's count at counters_[slot]
+int Map::enqueue_add(const float4* pts, int slot, bool downsample_on, int n_max, cudaStream_t st) {
+    int* d_cnt = counters_.as<int>();
+    const int chain_limit = std::max(64, (int)(rebuild_overflow_frac_ * v_.n_main));
+    if (downsample_on) {
+        unsigned long long* ki = a_keys_in_.as<unsigned long long>();
+        unsigned long long* ko = a_keys_out_.as<unsigned long long>();
+        k_voxel_keys<<<blocks_for(n_max, 256, 1 << 30), 256, 0, st>>>(pts, n_max, downsample_, ki, a_vals_in_.as<unsigned>(), &d_cnt[slot]);
+        size_t tmp = a_cub_.bytes;
+        FL_CUDA(cub::DeviceRadixSort::SortPairs(a_cub_.ptr, tmp, ki, ko, a_vals_in_.as<unsigned>(), a_vals_out_.as<unsigned>(), n_max, 0, 64, st));
+        k_group_heads<<<blocks_for(n_max, 256, 1 << 30), 256, 0, st>>>(ko, n_max, a_groups_.as<int>(), d_cnt, &d_cnt[slot]);
+        k_downsample_resolve<<<blocks_for((long long)n_max * 32, 256), 256, 0, st>>>(
+            v_, pts, ko, a_vals_out_.as<unsigned>(), n_max, a_groups_.as<int>(), downsample_, a_ins_.as<float4>(), d_cnt);
+        FL_CHECK(enqueue_insert(a_ins_.as<float4>(), &d_cnt[C_NINSERT], n_max, st));
+    } else {
+        FL_CHECK(enqueue_insert(pts, &d_cnt[slot], n_max, st));
+    }
+    k_async_account<<<1, 1, 0, st>>>(v_, d_cnt, slot, downsample_on, chain_limit);
+    FL_CUDA(cudaGetLastError());
+    return FL_OK;
+}
+
+int Map::add_points_async(const float4* pa, const int* na, bool downsample_a, const float4* pb, const int* nb, int n_max,
+                          const int* list_counts, int* out, cudaStream_t st) {
+    int* d_cnt = counters_.as<int>();
+    k_plan_begin<<<1, 1, 0, st>>>(d_cnt, na, nb, n_max);
+    if (v_.dir.cap) {
+        const int g = blocks_for((long long)n_max * 32, 256);
+        const float4* lists[2] = {pa, pb};
+        for (int l = 0; l < 2; l++)
+            if (lists[l]) k_plan_count<<<g, 256, 0, st>>>(v_, lists[l], n_max, &d_cnt[l ? C_RB : C_RA], d_cnt, cellcnt_.as<int>());
+        for (int l = 0; l < 2; l++)
+            if (lists[l]) k_plan_reset<<<g, 256, 0, st>>>(v_, lists[l], n_max, &d_cnt[l ? C_RB : C_RA], d_cnt, cellcnt_.as<int>(), pb ? 2 : 1);
+    }
+    k_plan<<<1, 1, 0, st>>>(v_, d_cnt);
+    FL_CHECK(enqueue_add(pa, C_NA, downsample_a, n_max, st));
+    if (pb) FL_CHECK(enqueue_add(pb, C_NB, false, n_max, st));
+    k_async_status<<<1, 1, 0, st>>>(d_cnt, list_counts, out);
+    FL_CUDA(cudaGetLastError());
+    ub_n_ += n_max;
+    return FL_OK;
+}
+
+int Map::add_points_async_checked(const float* d_pts, const int* d_n, int n_max, bool downsample_on, int* d_status2, cudaStream_t st) {
+    if (n_max < 0 || !device_ptr(d_n, device_, 4) || !device_ptr(d_status2, device_, 4) || (n_max > 0 && !device_ptr(d_pts, device_, 16))) {
+        set_last_error("add_points_async: n_max < 0, or a buffer is not device memory on device %d (points 16-byte, n and status "
+                       "4-byte aligned)", device_);
+        return FL_ERR_ARG;
+    }
+    FL_CUDA(cudaSetDevice(device_));
+    if (n_max == 0) {                                   // nothing can be inserted: (FL_OK, 0)
+        bool joined = false;
+        FL_CHECK(query_begin(st, &joined));
+        FL_CUDA(cudaMemsetAsync(d_status2, 0, 2 * sizeof(int), st));
+        return query_end(st, joined);
+    }
+    FL_CHECK(async_prepare(n_max, st, "add_points_async"));
+    bool joined = false;
+    FL_CHECK(mutation_begin(st, &joined));
+    FL_CHECK(add_points_async(reinterpret_cast<const float4*>(d_pts), d_n, downsample_on, nullptr, nullptr, n_max, nullptr, d_status2, st));
+    return mutation_end(st, joined);
 }
 
 int Map::tree_range(float* box6) {

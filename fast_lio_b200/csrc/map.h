@@ -62,6 +62,27 @@ public:
     // query_begin makes `st` wait for the handle's stream and query_end makes the handle's stream wait for `st`
     int query_begin(cudaStream_t st, bool* joined);
     int query_end(cudaStream_t st, bool joined);
+    // Device forms of Add_Points (fl_map_add_points_async, fl_filter_map_incremental_device): enqueued on the caller's stream `st`,
+    // the point counts read from device memory when `st` reaches them, no host synchronisation, no allocation (except the one
+    // documented case in async_prepare), grids sized from n_max.  A one-thread plan kernel checks the headroom first; when the
+    // batch might not fit, nothing is changed and the status is FL_ERR_CAPACITY.
+    //   async_prepare: the host's bound of the headroom for one more call of up to n_max points.  Outside capture a call that
+    //     might not fit settles the map and grows it first (synchronously); on a capturing stream it is FL_ERR_CAPACITY.
+    //   mutation_begin / mutation_end: the join of a device-form mutation (everything enqueued on the handle so far comes first)
+    int async_prepare(int n_max, cudaStream_t st, const char* what);
+    int mutation_begin(cudaStream_t st, bool* joined);
+    int mutation_end(cudaStream_t st, bool joined);
+    // one or two Add_Points (list a with downsample_a, then list b plain; b may be null) of up to n_max points each, counts
+    // *na / *nb in device memory (clamped to [0, n_max]), all-or-nothing together.  out: status2 = (status, added) when
+    // list_counts is null, else out4 = (list_counts[0], list_counts[1], added, status)
+    int add_points_async(const float4* pa, const int* na, bool downsample_a, const float4* pb, const int* nb, int n_max,
+                         const int* list_counts, int* out, cudaStream_t st);
+    // the public fl_map_add_points_async: argument checks, async_prepare, the join, add_points_async
+    int add_points_async_checked(const float* d_pts, const int* d_n, int n_max, bool downsample_on, int* d_status2, cudaStream_t st);
+    // Host-form calls settle first.  Read-only ones (full = false) refresh the host's mirror of the device counters (one read-back
+    // when a device-form mutation may have run); the others (full = true) also run the re-pack / re-list the device forms deferred,
+    // by the host form's rules.  *layout_changed: buffers or leaves moved since the last report (captured graphs are stale).
+    int settle(bool full, int* layout_changed = nullptr);
     // re-sort every valid point into fresh, evenly filled leaves (ikd-Tree's Rebuild, ikd_Tree.cpp:736-764)
     int rebuild();
     // re-list every live slot in the hashed cell directory (map.cuh); done by build / rebuild, and when inserts crowd it
@@ -72,7 +93,7 @@ public:
     // recompute every AABB from the valid points (after deletions)
     int refit();
 
-    int size() const { return n_valid_ + n_tomb_; }       // KD_TREE::size()  (valid + lazily deleted)
+    int size() const { return n_valid_ + n_tomb_; }       // KD_TREE::size()  (valid + lazily deleted; settle(false) first)
     int validnum() const { return n_valid_; }             // KD_TREE::validnum()
     void set_downsample(float v) { downsample_ = v; }
     float downsample() const { return downsample_; }
@@ -106,6 +127,26 @@ private:
     int build_from_sorted(const float4* d_src, int n);
     int insert_device(const float4* d_pts, int n);
     int maybe_rebuild();
+    int add_points_host(const float4* d_pts, int n, bool downsample_on, int* added);
+    // the host's n_valid_ / n_tomb_ into the device counters the device forms keep (after every host-form mutation)
+    int publish_counts();
+    // device forms: one Add_Points of the batch at pts, effective count at counters_[slot], after the plan kernel
+    int enqueue_add(const float4* pts, int slot, bool downsample_on, int n_max, cudaStream_t st);
+    int enqueue_insert(const float4* pts, const int* n_dev, int n_max, cudaStream_t st);
+    bool async_fits(long long n_max) const;
+    int async_grow(int n_max, bool pool);
+    int async_scratch(int n_max, bool may_allocate);
+
+    // device forms: pending_ = unsettled device-form mutations; captured_ = one was captured into a graph, so replays may
+    // mutate the map at any time and every settle reads back; ub_n_ = points the device forms may have inserted since the last
+    // settle (the host's bound of the headroom they used)
+    bool pending_ = false, captured_ = false, async_used_ = false, layout_dirty_ = false;
+    // owed by the next full settle (fl_map_maintain, a host-form mutation): the deferred re-pack / re-list (due_) and room for a
+    // refused call (refused_).  Read-only settles only add to them.
+    bool due_ = false, refused_ = false;
+    long long ub_n_ = 0;
+    int async_n_max_ = 0;
+    DeviceBuffer a_keys_in_, a_keys_out_, a_vals_in_, a_vals_out_, a_groups_, a_ins_, a_slots_, a_fix_, a_cub_, cellcnt_;
 
     int device_;
     float downsample_;

@@ -159,6 +159,35 @@ int fl_map_radius_search_device(fl_map_t* m, const float* centers_xyzr_device, i
  * enqueued on `stream`, and may be reused when the call returns.  Cannot be called on a capturing stream (FL_ERR_ARG). */
 int fl_map_build_device(fl_map_t* m, const float* pts_xyzi_device, int n, void* stream);
 int fl_map_add_points_device(fl_map_t* m, const float* pts_xyzi_device, int n, int downsample_on, void* stream);
+/* KD_TREE::Add_Points on the caller's stream                          ikd_Tree.cpp:478-573
+ * n is read from *n_device when `stream` reaches the call; the caller promises 0 <= *n_device <= n_max (a larger value is
+ * clamped to n_max).  status2_device[0]: FL_OK; 1 = maintenance due (the insert was applied, and the host form would have
+ * re-packed the leaves or re-listed the directory at this point: call fl_map_maintain); FL_ERR_CAPACITY = the call did not fit
+ * the map's headroom and NOTHING was changed.  status2_device[1]: the reference's return value, 0 on a refusal.
+ * Like the device-buffer queries above: never synchronises, allocates, re-packs, re-lists or sizes a launch from a device value
+ * (grids follow n_max), so it may be captured into a CUDA graph and replayed with other counts.  A plan kernel checks, before
+ * anything is written, that the batch fits the room left (overflow leaves, cell table below 90 % load, halo-list pool); every
+ * other kernel of the call then runs over the count the plan let through.  The one exception to "never synchronises": outside
+ * capture, when the host's bound of the headroom (overflow leaves and table cells for the points of every device-form call since
+ * the map was last settled, plus n_max; the list pool is checked on the device only) says the call might not fit, the call first
+ * settles the map (a wait for the stream) and grows it if it has no room either, synchronously, as the host form would.  On
+ * a capturing stream that case is FL_ERR_CAPACITY with nothing captured (so is a first call with this n_max: make the call once
+ * outside capture before capturing it).
+ * Ordering: outside capture `stream` first waits for everything enqueued on the handle (device queries joined from other
+ * streams included), and the handle's stream then waits for the call, so later calls on the map see the insert.  Inside capture
+ * nothing is joined (the rules of the queries above).  Host, wrong-device, null or misaligned pointers are FL_ERR_ARG and
+ * nothing is enqueued.  The host-form calls settle first: read-only ones (size, validnum, flatten, tree_range, the queries,
+ * fl_map_stats, fl_map_dir_stats) read the device's counters back once and change no layout, so a captured graph stays valid
+ * across them (synchronise graph replays before them); mutations and the filter's host forms also run the deferred re-pack /
+ * re-list. */
+int fl_map_add_points_async(fl_map_t* m, const float* pts_xyzi_device, const int* n_device, int n_max, int downsample_on,
+                            int* status2_device, void* stream);
+/* Settles the host's view of the map and runs the re-pack / directory re-list that device-form mutations deferred (by the host
+ * form's rules), and grows the map for a device-form call it refused (FL_ERR_CAPACITY).  *layout_changed (may be NULL) = 1 when
+ * buffers or leaves moved since the last report: graphs captured before must be captured again.  Synchronous.  A status of 1 or a
+ * refusal stays owed to this call when read-only host calls (validnum, size, ...) run in between; calls refused for lack of room
+ * keep being refused until it runs. */
+int fl_map_maintain(fl_map_t* m, int* layout_changed);
 /* KD_TREE::tree_range()                                              ikd_Tree.cpp:100-137 */
 int fl_map_tree_range(fl_map_t* m, float* box6);
 /* KD_TREE::Rebuild of the whole tree (ikd_Tree.cpp:736-764): re-sorts all valid points into fresh leaves */
@@ -251,6 +280,13 @@ int fl_filter_update_device(fl_filter_t* f, const float* body_xyzi_device, int n
  * device buffers on `stream` with the update's ordering rules; 0 <= nq <= the bound scan's size.  Not for sharded filters. */
 int fl_filter_get_nearest_device(fl_filter_t* f, float* out_pts_device, int* out_cnt_device, int nq, void* stream);
 int fl_filter_get_selected_device(fl_filter_t* f, unsigned char* out_device, int nq, void* stream);
+/* map_incremental() (laserMapping.cpp:427-474) on the caller's stream, after the last update of this filter (host or device
+ * form): out4_device = (|PointToAdd|, |PointNoNeedDownsample|, Add_Points(PointToAdd, true), status), the first three the values
+ * of fl_filter_map_incremental's out3, the status that of fl_map_add_points_async for both inserts, which are all-or-nothing
+ * together (FL_ERR_CAPACITY: neither list was inserted).  n_max is the bound scan's size.  The conventions, ordering and capture
+ * rules of fl_map_add_points_async; per scan, fl_filter_update_device then this call may be captured into one graph.  A sharded
+ * filter is FL_ERR_STATE and a null, host or misaligned out4 FL_ERR_ARG, with nothing enqueued. */
+int fl_filter_map_incremental_device(fl_filter_t* f, double filter_size_map_min, int flg_EKF_inited, int* out4_device, void* stream);
 
 /* ------------------------------------------------------------------ scan front end (SURVEY.md §8f rows 3-4)
  * The two steps that produce feats_down_body, kept in HBM on the map's device and stream so that a scan goes
