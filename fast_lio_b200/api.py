@@ -51,6 +51,8 @@ SYMBOLS = [
     "fl_comm_unique_id", "fl_filter_comm_init", "fl_filter_set_shard", "fl_filter_p2p_handle", "fl_filter_p2p_connect",
     "fl_filter_update_device", "fl_filter_get_nearest_device", "fl_filter_get_selected_device",
     "fl_map_add_points_async", "fl_map_maintain", "fl_filter_map_incremental_device",
+    "fl_scan_reserve", "fl_scan_upload_device", "fl_scan_undistort_device", "fl_scan_voxel_downsample_device",
+    "fl_filter_update_scan_device",
 ]
 
 
@@ -131,6 +133,11 @@ def load():
     L.fl_scan_voxel_downsample.argtypes = [C.c_void_p, C.c_float]
     L.fl_scan_download.argtypes = [C.c_void_p, C.c_int, _f32p, C.c_int]
     L.fl_filter_update_scan.argtypes = [C.c_void_p, C.c_void_p, _f64p, _f64p, C.c_double, C.POINTER(C.c_double)]
+    L.fl_scan_reserve.argtypes = [_vp, C.c_int, C.c_int]
+    L.fl_scan_upload_device.argtypes = [_vp, _vp, _vp, _vp, C.c_int, _vp]
+    L.fl_scan_undistort_device.argtypes = [_vp, _vp, _vp, C.c_int, _vp, _vp]
+    L.fl_scan_voxel_downsample_device.argtypes = [_vp, C.c_float, _vp, _vp]
+    L.fl_filter_update_scan_device.argtypes = [_vp, _vp, _vp, _vp, C.c_double, _vp, _vp]
     L.fl_localmap_create.argtypes = [C.POINTER(C.c_void_p), C.c_double, C.c_float]
     L.fl_localmap_destroy.argtypes = [C.c_void_p]
     L.fl_localmap_segment.argtypes = [C.c_void_p, C.c_void_p, _f64p, _f32p, C.POINTER(C.c_int)]
@@ -645,6 +652,70 @@ class Scan:
         st = C.c_double(0.0)
         _check(self._L.fl_filter_update_scan(filt.h, self.h, x, Pm, R, C.byref(st)))
         return x, Pm, st.value
+
+    # ---- device-buffer forms: CUDA tensors on the map's device, enqueued on torch.cuda.current_stream(), counts in device memory
+    def reserve(self, n_max: int, n_pose_max: int):
+        """fl_scan_reserve: size the device forms' buffers for up to n_max points and n_pose_max IMU poses (synchronous)."""
+        _check(self._L.fl_scan_reserve(self.h, n_max, n_pose_max))
+
+    def _count(self, n, default: int, name: str):
+        import torch
+        t = self.tree
+        if n is None:
+            # building the count is a host-to-device copy, which a capturing stream cannot take
+            if torch.cuda.is_current_stream_capturing():
+                raise ValueError(f"{name}: pass an int32 CUDA tensor while capturing a CUDA graph")
+            return torch.tensor([default], dtype=torch.int32, device=f"cuda:{t.device}")
+        return t._tensor(n, name, None, torch.int32, (1,))
+
+    def upload_device(self, xyzi, offset_ms, n=None, n_max: int | None = None):
+        """fl_scan_upload_device: the first *n rows of xyzi ((>= n_max, 4) float32) and offset_ms ((>= n_max,) float32).  n is an
+        int32 CUDA tensor of one element (None: the tensor's length, which is copied from the host, so pass a tensor when capturing
+        a CUDA graph); n_max defaults to the number of rows."""
+        import torch
+        t = self.tree
+        xyzi = t._tensor(xyzi, "xyzi", 4)
+        offset_ms = t._tensor(offset_ms, "offset_ms", None, torch.float32, (xyzi.shape[0],))
+        n_max = xyzi.shape[0] if n_max is None else n_max
+        if xyzi.shape[0] < n_max:
+            raise ValueError(f"xyzi: {xyzi.shape[0]} rows, fewer than n_max = {n_max}")
+        self._n = self._count(n, xyzi.shape[0], "n")           # kept alive until the stream has read it
+        _check(self._L.fl_scan_upload_device(self.h, xyzi.data_ptr() if n_max else None, offset_ms.data_ptr() if n_max else None,
+                                             self._n.data_ptr(), n_max, t._stream()))
+
+    def undistort_device(self, poses, n_pose, x_end):
+        """fl_scan_undistort_device: poses (n_pose_max, 22) float64, n_pose an int32 CUDA tensor (1,) (None: all rows, copied
+        from the host, so pass a tensor when capturing), x_end (26,) float64; all read when the current stream reaches the call."""
+        import torch
+        t = self.tree
+        poses = t._tensor(poses, "poses", 22, torch.float64)
+        x_end = t._tensor(x_end, "x_end", None, torch.float64, (26,))
+        self._n_pose = self._count(n_pose, poses.shape[0], "n_pose")
+        _check(self._L.fl_scan_undistort_device(self.h, poses.data_ptr() if poses.shape[0] else None, self._n_pose.data_ptr(),
+                                                poses.shape[0], x_end.data_ptr(), t._stream()))
+
+    def voxel_downsample_device(self, leaf: float, out=None):
+        """fl_scan_voxel_downsample_device; returns out, an int32 tensor (1,) that receives feats_down_size on the current stream."""
+        import torch
+        t = self.tree
+        if out is None:
+            out = torch.empty(1, dtype=torch.int32, device=f"cuda:{t.device}")
+        out = t._tensor(out, "out", None, torch.int32, (1,))
+        _check(self._L.fl_scan_voxel_downsample_device(self.h, leaf, out.data_ptr(), t._stream()))
+        return out
+
+    def update_device(self, filt: "Esekf", x, P, R: float = 0.001, status=None):
+        """fl_filter_update_scan_device: x (26,) and P (23, 23) float64 tensors updated in place on success; returns status, an
+        int32 tensor (2,) = (FL_OK or FL_ERR_STATE, passes run), written on the current stream."""
+        import torch
+        t = self.tree
+        x = t._tensor(x, "x", None, torch.float64, (26,))
+        P = t._tensor(P, "P", None, torch.float64, (23, 23))
+        if status is None:
+            status = torch.empty(2, dtype=torch.int32, device=x.device)
+        status = t._tensor(status, "status", None, torch.int32, (2,))
+        _check(self._L.fl_filter_update_scan_device(filt.h, self.h, x.data_ptr(), P.data_ptr(), R, status.data_ptr(), t._stream()))
+        return status
 
 
 class LocalMap:

@@ -435,19 +435,23 @@ int fl_scan_destroy(fl_scan_t* s) {
     delete s;
     return FL_OK;
 }
-int fl_scan_upload(fl_scan_t* s, const float* xyzi, const float* offset_ms, int n) { SCAN_GUARD(s); return s->impl->upload(xyzi, offset_ms, n); }
+// the host forms first take over the cloud and counts of the device forms when those produced the current cloud
+#define SCAN_HOST_GUARD(s)                                                                   \
+    SCAN_GUARD(s);                                                                           \
+    { const int _rc = (s)->impl->settle(); if (_rc != FL_OK) return _rc; }
+int fl_scan_upload(fl_scan_t* s, const float* xyzi, const float* offset_ms, int n) { SCAN_HOST_GUARD(s); return s->impl->upload(xyzi, offset_ms, n); }
 int fl_scan_undistort(fl_scan_t* s, const double* imu_pose22, int n_pose, const double* x26_end) {
-    SCAN_GUARD(s);
+    SCAN_HOST_GUARD(s);
     return s->impl->undistort(imu_pose22, n_pose, x26_end);
 }
 int fl_scan_voxel_downsample(fl_scan_t* s, float leaf_size) {
-    SCAN_GUARD(s);
+    SCAN_HOST_GUARD(s);
     int n = 0;
     int rc = s->impl->voxel_downsample(leaf_size, &n);
     return rc == FL_OK ? n : rc;
 }
 int fl_scan_download(fl_scan_t* s, int which, float* out_xyzi, int cap) {
-    SCAN_GUARD(s);
+    SCAN_HOST_GUARD(s);
     int n = 0;
     int rc = s->impl->download(which, out_xyzi, cap, &n);
     return rc == FL_OK ? n : rc;
@@ -455,7 +459,33 @@ int fl_scan_download(fl_scan_t* s, int which, float* out_xyzi, int cap) {
 int fl_filter_update_scan(fl_filter_t* f, fl_scan_t* s, double* x26, double* P, double R, double* solve_time_s) {
     FILTER_HOST_GUARD(f);
     if (!s || !s->impl || s->map != f->map) { fl::set_last_error("fl_filter_update_scan: the scan must live on the filter's map"); return FL_ERR_ARG; }
+    { const int rc = s->impl->settle(); if (rc != FL_OK) return rc; }
     return f->impl->update_device(s->impl->down_device(), s->impl->down_count(), x26, P, R, solve_time_s);
+}
+// Device forms: the guard touch()es the map, so Map::query_begin orders them after everything enqueued on the handle's stream.
+int fl_scan_reserve(fl_scan_t* s, int n_max, int n_pose_max) { SCAN_GUARD(s); return s->impl->reserve_device(n_max, n_pose_max); }
+int fl_scan_upload_device(fl_scan_t* s, const float* xyzi_device, const float* offset_ms_device, const int* n_device, int n_max, void* stream) {
+    SCAN_GUARD(s);
+    return s->impl->upload_on_stream(xyzi_device, offset_ms_device, n_device, n_max, static_cast<cudaStream_t>(stream));
+}
+int fl_scan_undistort_device(fl_scan_t* s, const double* imu_pose22_device, const int* n_pose_device, int n_pose_max, const double* x26_end_device,
+                             void* stream) {
+    SCAN_GUARD(s);
+    return s->impl->undistort_on_stream(imu_pose22_device, n_pose_device, n_pose_max, x26_end_device, static_cast<cudaStream_t>(stream));
+}
+int fl_scan_voxel_downsample_device(fl_scan_t* s, float leaf_size, int* n_out_device, void* stream) {
+    SCAN_GUARD(s);
+    return s->impl->voxel_downsample_on_stream(leaf_size, n_out_device, static_cast<cudaStream_t>(stream));
+}
+int fl_filter_update_scan_device(fl_filter_t* f, fl_scan_t* s, double* x26_device, double* P_device, double R, int* status2_device, void* stream) {
+    FILTER_GUARD(f);
+    if (!s || !s->impl || s->map != f->map) { fl::set_last_error("fl_filter_update_scan_device: the scan must live on the filter's map"); return FL_ERR_ARG; }
+    if (!s->impl->dev_down_ready()) {
+        fl::set_last_error("fl_filter_update_scan_device: no fl_scan_voxel_downsample_device since the scan's last upload");
+        return FL_ERR_STATE;
+    }
+    return f->impl->update_scan_on_stream(s->impl->down_dev(), s->impl->down_count_dev(), s->impl->dev_n_max(), x26_device, P_device, R,
+                                          status2_device, static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------------------------ local-map cube

@@ -1071,13 +1071,18 @@ struct StateIn {
     int max_iter, extrinsic_est;
 };
 constexpr int STATE_THREADS = 256;
+// which call bound the filter's scan last, as stream work records it (Filter::d_bind_[1]): a host-form call (its size is the
+// host's), fl_filter_update_device (the filter's copy of the caller's scan), fl_filter_update_scan_device (the scan front end's cloud)
+constexpr int BIND_HOST = 0, BIND_COPY = 1, BIND_SCAN = 2;
 
 // Also clears k_update's publication block: its workers take a word as current when its tag equals pub_tag(nonce, pass), and
 // every replay of a captured graph passes the same nonce, so words left by the previous replay would otherwise look current.
 // And it clears `done` in the page-locked mirror, so download_state / get_pass_logs fetch this update's control block instead
 // of trusting a result an earlier host-form update mirrored there.
+// bind (fl_filter_update_device, null otherwise) receives the binding of this update: (nq, BIND_COPY), see Filter::read_binding.
 __global__ void __launch_bounds__(STATE_THREADS) k_state_in(FilterCtl* ctl, unsigned long long* pub, FilterCtl* mirror,
-                                                            const double* __restrict__ x26, const double* __restrict__ P, StateIn s) {
+                                                            const double* __restrict__ x26, const double* __restrict__ P, StateIn s,
+                                                            int* __restrict__ bind, int nq) {
     pdl_launch();           // k_update may begin launching: its pdl_wait() holds it until this grid is complete and flushed
     const int t = threadIdx.x;
     for (int i = t; i < NDOF * NDOF; i += STATE_THREADS) { const double v = P[i]; ctl->P[i] = v; ctl->P_prop[i] = v; }   // P_propagated = P_
@@ -1091,7 +1096,15 @@ __global__ void __launch_bounds__(STATE_THREADS) k_state_in(FilterCtl* ctl, unsi
         ctl->max_iter = s.max_iter; ctl->extrinsic_est = s.extrinsic_est; ctl->R = s.R;
         ctl->host_mirror = nullptr;
         mirror->done = 0;
+        if (bind) { bind[0] = nq; bind[1] = BIND_COPY; }
     }
+}
+
+// fl_filter_update_scan_device: the scan's count, clamped to [0, n_max], becomes the filter's own (bind[0]), with the binding
+// BIND_SCAN.  k_update_n reads bind[0] before its pdl_wait(): this kernel completes before k_state_in, its predecessor, starts.
+__global__ void k_count_in(const int* __restrict__ n, int n_max, int* __restrict__ bind) {
+    bind[0] = min(max(*n, 0), n_max);
+    bind[1] = BIND_SCAN;
 }
 
 // x26 / P receive the result only when the update succeeded; status2 = (FL_OK or the error download_state reports, passes run)
@@ -1104,6 +1117,12 @@ __global__ void __launch_bounds__(STATE_THREADS) k_state_out(const FilterCtl* __
         if (t < XLEN) x26[t] = ctl->x[t];
     }
     if (t == 0) { status2[0] = e == 0 ? FL_OK : (e == 2 ? FL_ERR_NCCL : FL_ERR_STATE); status2[1] = ctl->n_pass; }
+}
+
+// map_incremental over n_max rows with the count in device memory: rows [*n, n_max) are neither PointToAdd nor PointNoNeedDownsample
+__global__ void k_flags_clear(unsigned char* __restrict__ flag_add, unsigned char* __restrict__ flag_no, const int* __restrict__ n, int n_max) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q < n_max && q >= *n) { flag_add[q] = 0; flag_no[q] = 0; }
 }
 
 // ============================================================================= NCCL (lazy)
@@ -1157,6 +1176,7 @@ Filter::~Filter() {
     body_.release(); nearest_.release(); nearest_cnt_.release(); selected_.release(); normvec_.release(); plane_.release(); srange_.release();
     partials_.release(); red_.release(); ctl_.release(); ctl0_.release(); logs_.release(); pub_.release();
     mi_world_.release(); mi_flag_add_.release(); mi_flag_no_.release(); mi_list_add_.release(); mi_list_no_.release(); mi_tmp_.release(); mi_counts_.release();
+    d_bind_.release();
     if (h_ctl_) cudaFreeHost(h_ctl_);
     if (ev0_) cudaEventDestroy(ev0_);
     if (ev1_) cudaEventDestroy(ev1_);
@@ -1196,6 +1216,16 @@ int Filter::init() {
     upd_capacity_[0][1] = sms_ * occ;
     FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update<true, 2>, 2 * UPD_THREADS, 0));
     upd_capacity_[1][1] = sms_ * occ;
+    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_n<false, 1>, UPD_THREADS, 0));
+    upd_n_capacity_[0][0] = std::min(upd_capacity_[0][0], sms_ * std::max(1, occ));
+    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_n<true, 1>, UPD_THREADS, 0));
+    upd_n_capacity_[1][0] = std::min(upd_capacity_[1][0], sms_ * std::max(1, occ));
+    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_n<false, 2>, 2 * UPD_THREADS, 0));
+    upd_n_capacity_[0][1] = std::min(upd_capacity_[0][1], sms_ * occ);
+    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_n<true, 2>, 2 * UPD_THREADS, 0));
+    upd_n_capacity_[1][1] = std::min(upd_capacity_[1][1], sms_ * occ);
+    FL_CHECK(d_bind_.reserve(2 * sizeof(int)));
+    FL_CUDA(cudaMemsetAsync(d_bind_.ptr, 0, 2 * sizeof(int), stream()));
     FL_CHECK(partials_.reserve(sizeof(double) * PSTRIDE * (size_t)std::max(upd_capacity_[0][0], upd_capacity_[1][0])));
     max_resid_grid_ = sms_;
     FL_CHECK(partials_.reserve(sizeof(double) * PSTRIDE * (size_t)max_resid_grid_));
@@ -1239,12 +1269,19 @@ int Filter::set_params(int max_iter, const double* limit23, int extrinsic_est_en
 }
 
 int Filter::set_scan_device(const float4* d_body, int nq) {
+    FL_CHECK(bind_scan(d_body, nq));
+    // once a device form has bound the scan, stream work records the binding: from here on the host's (read_binding)
+    if (stream_bound_) FL_CUDA(cudaMemsetAsync(d_bind_.as<int>() + 1, 0, sizeof(int), stream()));
+    return FL_OK;
+}
+int Filter::bind_scan(const float4* d_body, int nq) {
     if (nq < 0) { set_last_error("scan: nq < 0"); return FL_ERR_ARG; }
     FL_CUDA(cudaSetDevice(map_->device()));
     FL_CHECK(reserve(std::max(1, nq)));
     scan_.body = d_body;
     scan_.Q = nq;
     if (!shard_set_) { scan_.q_begin = 0; scan_.q_end = nq; }
+    dev_count_ = false;
     // per-scan state of the reference's globals: point_selected_surf is rewritten for every point
     // on the first (always searching) pass, Nearest_Points likewise
     return FL_OK;
@@ -1376,9 +1413,7 @@ int Filter::run_passes() {
 }
 
 // the fused persistent kernel: blockIdx 0 solves, the others measure; every block must be co-resident (they wait for each other)
-int Filter::launch_update(int max_passes, int mode, int search_only, cudaStream_t st) {
-    FL_CUDA(cudaSetDevice(map_->device()));
-    const int nq = scan_.q_end - scan_.q_begin;
+UpdArgs Filter::upd_args(int max_passes, int mode, int search_only) {
     UpdArgs a;
     a.m = map_->view();
     if (search_mode_ == 0) a.m.dir.cap = 0;                  // A/B: every query through the BVH walk
@@ -1388,6 +1423,13 @@ int Filter::launch_update(int max_passes, int mode, int search_only, cudaStream_
     a.pub = pub_.as<unsigned long long>(); a.nonce = ++launch_nonce_;
     { const char* e = getenv("FASTLIO_B200_DBG"); a.dbg = e ? atoi(e) : 0; }
     a.pose_from_search = 0;
+    return a;
+}
+
+int Filter::launch_update(int max_passes, int mode, int search_only, cudaStream_t st) {
+    FL_CUDA(cudaSetDevice(map_->device()));
+    const int nq = scan_.q_end - scan_.q_begin;
+    const UpdArgs a = upd_args(max_passes, mode, search_only);
     const int cap = upd_capacity_[extrinsic_est_ ? 1 : 0][0];
     // every co-resident block works (a searching pass wants many warps in flight); small scans: at least 4 points per warp
     // one thread per point: full warps (the search is bound by a thread's own chain of loads, not by the number of SMs)
@@ -1551,14 +1593,15 @@ int Filter::update_on_stream(const float* d_body, int nq, double* d_x26, double*
         return FL_ERR_CAPACITY;
     }
     FL_CUDA(cudaSetDevice(dev));
-    FL_CHECK(set_scan_device(body_.as<float4>(), nq));       // within capacity: binds, allocates nothing
     bool joined = false;
     FL_CHECK(map_->query_begin(st, &joined));
+    FL_CHECK(bind_scan(body_.as<float4>(), nq));             // within capacity: binds, allocates nothing
+    stream_bound_ = true;
     if (nq > 0) FL_CUDA(cudaMemcpyAsync(body_.ptr, d_body, sizeof(float4) * (size_t)nq, cudaMemcpyDeviceToDevice, st));
     StateIn s;
     for (int i = 0; i < NDOF; i++) s.limit[i] = limit_[i];
     s.R = R; s.max_iter = max_iter_; s.extrinsic_est = extrinsic_est_;
-    k_state_in<<<1, STATE_THREADS, 0, st>>>(ctl_.as<FilterCtl>(), pub_.as<unsigned long long>(), h_ctl_, d_x26, d_P, s);
+    k_state_in<<<1, STATE_THREADS, 0, st>>>(ctl_.as<FilterCtl>(), pub_.as<unsigned long long>(), h_ctl_, d_x26, d_P, s, d_bind_.as<int>(), nq);
     FL_CUDA(cudaGetLastError());
     // run_passes's fused single-rank branch, on `st`
     neighbours_complete_ = false;
@@ -1566,6 +1609,76 @@ int Filter::update_on_stream(const float* d_body, int nq, double* d_x26, double*
     launches_ = 1;
     k_state_out<<<1, STATE_THREADS, 0, st>>>(ctl_.as<FilterCtl>(), d_x26, d_P, d_status2);
     return map_->query_end(st, joined);
+}
+
+int Filter::update_scan_on_stream(const float4* d_body, const int* d_n, int n_max, double* d_x26, double* d_P, double R, int* d_status2,
+                                  cudaStream_t st) {
+    const int dev = map_->device();
+    if (!device_ptr(d_x26, dev, 8) || !device_ptr(d_P, dev, 8) || !device_ptr(d_status2, dev, 4)) {
+        set_last_error("update_scan_device: a buffer is not device memory on device %d (x and P 8-byte, status 4-byte aligned)", dev);
+        return FL_ERR_ARG;
+    }
+    FL_CHECK(device_form_scope("update_scan_device", true));
+    if (n_max > capacity()) {
+        set_last_error("update_scan_device: the scan's n_max of %d exceeds the filter's capacity of %d (max_points, or the largest scan so far)",
+                       n_max, capacity());
+        return FL_ERR_CAPACITY;
+    }
+    FL_CUDA(cudaSetDevice(dev));
+    bool joined = false;
+    FL_CHECK(map_->query_begin(st, &joined));
+    FL_CHECK(bind_scan(d_body, n_max));                      // within capacity: binds, allocates nothing
+    dev_count_ = true;
+    q_max_ = n_max;
+    scan_body_ = d_body;
+    stream_bound_ = true;
+    // the count is the filter's own from here on (later host-form calls read it back)
+    k_count_in<<<1, 1, 0, st>>>(d_n, n_max, d_bind_.as<int>());
+    StateIn s;
+    for (int i = 0; i < NDOF; i++) s.limit[i] = limit_[i];
+    s.R = R; s.max_iter = max_iter_; s.extrinsic_est = extrinsic_est_;
+    k_state_in<<<1, STATE_THREADS, 0, st>>>(ctl_.as<FilterCtl>(), pub_.as<unsigned long long>(), h_ctl_, d_x26, d_P, s, nullptr, 0);
+    FL_CUDA(cudaGetLastError());
+    neighbours_complete_ = false;
+    // k_update_n over the row bound: the workers of the host form at n_max rows (tile t to block t, as at the count), one or
+    // two threads per point as the host form picks at n_max -- both forms give the same bytes
+    const int e = extrinsic_est_ ? 1 : 0;
+    const int tiles = (n_max + UPD_THREADS - 1) / UPD_THREADS;
+    const int pair = upd_pair(n_max) == 2 && tiles <= upd_n_capacity_[e][1] - 1 ? 2 : 1;
+    const int workers = std::max(0, std::min(upd_n_capacity_[e][0] - 1, tiles));
+    const UpdArgs a = upd_args(max_iter_ + 1, 0, 0);
+    const int* n = d_bind_.as<int>();
+    const int block = pair * UPD_THREADS;
+    cudaError_t rc;
+    if (e) rc = pair == 2 ? launch_pdl(k_update_n<true, 2>, workers + 1, block, st, pdl_, a, n) : launch_pdl(k_update_n<true, 1>, workers + 1, block, st, pdl_, a, n);
+    else rc = pair == 2 ? launch_pdl(k_update_n<false, 2>, workers + 1, block, st, pdl_, a, n) : launch_pdl(k_update_n<false, 1>, workers + 1, block, st, pdl_, a, n);
+    FL_CUDA(rc);
+    launches_ = 1;
+    k_state_out<<<1, STATE_THREADS, 0, st>>>(ctl_.as<FilterCtl>(), d_x26, d_P, d_status2);
+    return map_->query_end(st, joined);
+}
+
+// Host forms after a device form: the binding the stream work recorded last is read back (once per call), so a host form after a
+// graph replay runs over the replay's scan even when a host-form update was called between the capture and the replay.
+int Filter::read_binding() {
+    if (!stream_bound_) return FL_OK;
+    FL_CUDA(cudaSetDevice(map_->device()));
+    int b[2] = {0, BIND_HOST};
+    FL_CUDA(cudaStreamSynchronize(stream()));
+    FL_CUDA(cudaMemcpyAsync(b, d_bind_.ptr, sizeof(b), cudaMemcpyDeviceToHost, stream()));
+    FL_CUDA(cudaStreamSynchronize(stream()));
+    if (b[1] == BIND_HOST || shard_set_) return FL_OK;      // the host's binding stands (device forms refuse sharded filters)
+    if (b[1] == BIND_SCAN) {                                // the scan front end's cloud, the count on the device
+        scan_.body = scan_body_;
+        dev_count_ = true;
+        scan_.Q = scan_.q_end = std::max(0, std::min(b[0], q_max_));
+    } else {                                                // fl_filter_update_device's copy of the caller's scan
+        scan_.body = body_.as<float4>();
+        dev_count_ = false;
+        scan_.Q = scan_.q_end = b[0];
+    }
+    scan_.q_begin = 0;
+    return FL_OK;
 }
 
 int Filter::get_nearest_on_stream(float* d_pts, int* d_cnt, int nq, cudaStream_t st) {
@@ -1602,6 +1715,7 @@ int Filter::map_incremental(double fsm, int ekf_inited, int* n_to_add, int* n_no
     if (n_to_add) *n_to_add = 0;
     if (n_no_downsample) *n_no_downsample = 0;
     if (added) *added = 0;
+    FL_CHECK(read_binding());
     const int nq = scan_.Q;
     if (nq <= 0) return FL_OK;
     if (!(fsm > 0.0)) { set_last_error("map_incremental: filter_size_map_min must be > 0"); return FL_ERR_ARG; }
@@ -1645,7 +1759,7 @@ int Filter::map_incremental_on_stream(double fsm, int ekf_inited, int* d_out4, c
     if (!device_ptr(d_out4, dev, 4)) { set_last_error("map_incremental_device: out4 must be 4-byte aligned device memory on device %d", dev); return FL_ERR_ARG; }
     if (!(fsm > 0.0)) { set_last_error("map_incremental_device: filter_size_map_min must be > 0"); return FL_ERR_ARG; }
     FL_CHECK(device_form_scope("map_incremental_device", false));
-    const int nq = scan_.Q;
+    const int nq = dev_count_ ? q_max_ : scan_.Q;              // after update_scan_device: the row bound, the count on the device
     FL_CUDA(cudaSetDevice(dev));
     size_t tmp = 0;
     FL_CUDA(cub::DeviceSelect::Flagged(nullptr, tmp, (const float4*)nullptr, (const unsigned char*)nullptr, (float4*)nullptr, (int*)nullptr, nq, st));
@@ -1662,8 +1776,12 @@ int Filter::map_incremental_on_stream(double fsm, int ekf_inited, int* d_out4, c
     FL_CHECK(map_->async_prepare(nq, st, "map_incremental_device"));
     bool joined = false;
     FL_CHECK(map_->mutation_begin(st, &joined));
-    k_map_incremental<<<(nq + 255) / 256, 256, 0, st>>>(scan_, ctl_.as<FilterCtl>(), fsm, ekf_inited, mi_world_.as<float4>(),
+    ScanView sv = scan_;
+    sv.Q = nq;
+    k_map_incremental<<<(nq + 255) / 256, 256, 0, st>>>(sv, ctl_.as<FilterCtl>(), fsm, ekf_inited, mi_world_.as<float4>(),
                                                        mi_flag_add_.as<unsigned char>(), mi_flag_no_.as<unsigned char>());
+    // rows from the device count on enter neither list, so the compactions below give the count-n host form's lists
+    if (dev_count_) k_flags_clear<<<(nq + 255) / 256, 256, 0, st>>>(mi_flag_add_.as<unsigned char>(), mi_flag_no_.as<unsigned char>(), d_bind_.as<int>(), nq);
     FL_CUDA(cudaGetLastError());
     tmp = mi_tmp_.bytes;
     FL_CUDA(cub::DeviceSelect::Flagged(mi_tmp_.ptr, tmp, mi_world_.as<float4>(), mi_flag_add_.as<unsigned char>(), mi_list_add_.as<float4>(),
@@ -1677,6 +1795,7 @@ int Filter::map_incremental_on_stream(double fsm, int ekf_inited, int* d_out4, c
 }
 
 int Filter::get_nearest(float* out_pts, int* out_cnt, int nq) {
+    FL_CHECK(read_binding());
     if (nq > scan_.Q) { set_last_error("get_nearest: nq exceeds the bound scan"); return FL_ERR_ARG; }
     FL_CUDA(cudaSetDevice(map_->device()));
     FL_CHECK(complete_neighbours());
@@ -1686,6 +1805,7 @@ int Filter::get_nearest(float* out_pts, int* out_cnt, int nq) {
     return FL_OK;
 }
 int Filter::get_selected(unsigned char* out, int nq) {
+    FL_CHECK(read_binding());
     if (nq > scan_.Q) { set_last_error("get_selected: nq exceeds the bound scan"); return FL_ERR_ARG; }
     if (scan_.q_begin > 0 || scan_.q_end < nq) {
         set_last_error("get_selected: point_selected_surf of points outside this rank's shard [%d, %d) lives on the rank that owns them", scan_.q_begin, scan_.q_end);
@@ -1697,6 +1817,7 @@ int Filter::get_selected(unsigned char* out, int nq) {
     return FL_OK;
 }
 int Filter::get_pass_logs(PassLog* out, int cap, int* n) {
+    FL_CHECK(read_binding());
     FL_CUDA(cudaSetDevice(map_->device()));
     FL_CUDA(cudaStreamSynchronize(stream()));
     if (!(mirror_ && h_ctl_->done)) {                   // nothing ran since the upload (or the mirror is off): fetch the block

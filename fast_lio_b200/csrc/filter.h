@@ -99,6 +99,9 @@ public:
     // Nearest_Points / point_selected_surf of the last update into caller device buffers, on `st`
     int get_nearest_on_stream(float* d_pts, int* d_cnt, int nq, cudaStream_t st);
     int get_selected_on_stream(unsigned char* d_out, int nq, cudaStream_t st);
+    // update_on_stream on a scan bound in place (the scan front end's down-sampled cloud, fl_filter_update_scan_device) whose
+    // point count is read from device memory: d_n is copied into the filter's own count, grids follow n_max (k_update_n)
+    int update_scan_on_stream(const float4* d_body, const int* d_n, int n_max, double* d_x26, double* d_P, double R, int* d_status2, cudaStream_t st);
     // the largest scan the per-point buffers hold without growing (max_points at create, or the largest scan since)
     int capacity() const;
 
@@ -166,6 +169,21 @@ private:
     cudaError_t launch_upd(int workers, bool pdl, const UpdArgs& a, int pair, cudaStream_t st);
     // the device forms cover a single-rank filter (and the update a fused, solver-1 one); FL_ERR_STATE otherwise
     int device_form_scope(const char* what, bool update) const;
+    // the UpdArgs of a launch of k_update / k_update_n
+    UpdArgs upd_args(int max_passes, int mode, int search_only);
+    // binds the scan without recording the binding on the device (set_scan_device: the host forms' binding, recorded)
+    int bind_scan(const float4* d_body, int nq);
+    // device-count binding (update_scan_on_stream): the bound scan's count lives in d_bind_[0] and scan_.Q / q_end hold the row
+    // bound q_max_ until a host-form call reads the count back (read_binding); set_scan_device ends it
+    bool dev_count_ = false;
+    int q_max_ = 0;
+    const float4* scan_body_ = nullptr;      // the scan front end's cloud of the last update_scan_on_stream
+    // d_bind_ = (size, BIND_*): the binding the stream work recorded last, written by the device forms (in their graphs too) and,
+    // once a device form has run (stream_bound_), by the host forms' binds; read_binding restores it for the host forms
+    bool stream_bound_ = false;
+    DeviceBuffer d_bind_;
+    int upd_n_capacity_[2][2] = {{0, 0}, {0, 0}};   // co-resident k_update_n blocks, capped at k_update's (the same tiles per block)
+    int read_binding();
     int launches_ = 0;
     long long host_ns_[4] = {0, 0, 0, 0};
     bool shard_set_ = false;

@@ -16,6 +16,22 @@ void set_last_error(const char* fmt, ...);
 
 namespace {
 
+struct VgCtl {
+    float mn[3], mx[3];
+    int total;          // number of output points
+    int passthrough;    // PCL's "leaf size too small" exit: output = input
+};
+
+// The device forms' control block: their voxel grid, and what the host forms need to take the cloud over (ScanFrontEnd::settle).
+// Every device-form stage sets src, so the host forms see the result of whichever device-form stage ran last.
+struct ScanDevCtl {
+    VgCtl vg;           // vg.total: the device forms' feats_down_size
+    int n_raw;          // *n_device of their last upload, clamped to [0, n_max]
+    int src;            // 1: a device-form stage ran since the host forms last took the cloud over (settle clears it)
+    int stage;          // 1: their cloud was de-skewed (it is in the sorted buffers), 0: as uploaded
+    int down;           // 1: they down-sampled it since their upload
+};
+
 // ------------------------------------------------------------------------------------------------ de-skew
 struct EndState {
     D3 pos, offT;
@@ -65,9 +81,15 @@ __device__ __forceinline__ void compensate(float4& p, double t, const double* he
 // is: point i belongs to the LAST segment kp whose head is strictly older than the point; points older than
 // every head stay untouched.  One quirk is kept: the sweep `break`s on the first point and then re-tests
 // it against every earlier segment, so point 0 is compensated once per earlier segment that is older than it.
+// Device forms: n and n_pose are the row bounds, the counts are min(*n_dev, n) and *n_pose_dev clamped to [0, n_pose], and
+// the kernel marks the device forms' cloud as de-skewed and current (dc: null in the host form).
 __global__ void k_undistort(float4* __restrict__ pts, const float* __restrict__ t_ms, int n,
-                            const double* __restrict__ poses, int n_pose, const double* __restrict__ x_end) {
+                            const double* __restrict__ poses, int n_pose, const double* __restrict__ x_end,
+                            const int* __restrict__ n_dev, const int* __restrict__ n_pose_dev, ScanDevCtl* dc) {
     extern __shared__ double s_pose[];
+    if (n_dev) n = min(*n_dev, n);
+    if (n_pose_dev) n_pose = min(max(*n_pose_dev, 0), n_pose);
+    if (dc && blockIdx.x == 0 && threadIdx.x == 0) { dc->stage = 1; dc->src = 1; }
     for (int i = threadIdx.x; i < n_pose * POSE_DOUBLES; i += blockDim.x) s_pose[i] = poses[i];
     __syncthreads();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -93,19 +115,32 @@ __global__ void k_undistort(float4* __restrict__ pts, const float* __restrict__ 
 }
 
 // ------------------------------------------------------------------------------------------------ voxel grid
-struct VgCtl {
-    float mn[3], mx[3];
-    int total;          // number of output points
-    int passthrough;    // PCL's "leaf size too small" exit: output = input
-};
+// The `*_dev` counts of the kernels below: n is the row bound (n_max), the count min(*n_dev, n); null in the host forms.
+__device__ __forceinline__ int dev_count(const int* n_dev, int n) { return n_dev ? min(*n_dev, n) : n; }
 
-__global__ void k_vg_reset(VgCtl* c) {
+// dc (device forms, null in the host form): the down-sampled cloud is theirs and current
+__global__ void k_vg_reset(VgCtl* c, ScanDevCtl* dc) {
     if (threadIdx.x < 3) { c->mn[threadIdx.x] = FLT_MAX; c->mx[threadIdx.x] = -FLT_MAX; }
     if (threadIdx.x == 3) { c->total = 0; c->passthrough = 0; }
+    if (threadIdx.x == 4 && dc) { dc->down = 1; dc->src = 1; }
+}
+
+// fl_scan_upload_device: the first n = *n_dev (clamped to [0, n_max]) rows, and the offset time 0x7FFFFFFF (a NaN) in rows
+// [n, n_max).  cub's float twiddle maps that pattern to 0xFFFFFFFF, the largest key, and the sort is stable, so the padding rows
+// sort after the real ones and the first n rows of the n_max-row time sort are those of the n-row sort, NaN times included.
+__global__ void k_upload_n(const float4* __restrict__ xyzi, const float* __restrict__ t_ms, const int* __restrict__ n_dev, int n_max,
+                           float4* __restrict__ raw, float* __restrict__ time, ScanDevCtl* c) {
+    const int n = min(max(*n_dev, 0), n_max);
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i == 0) { c->n_raw = n; c->src = 1; c->stage = 0; c->down = 0; }
+    if (i >= n_max) return;
+    if (i < n) { raw[i] = xyzi[i]; time[i] = t_ms[i]; }
+    else time[i] = __int_as_float(0x7FFFFFFF);
 }
 
 // getMinMax3D (pcl/common/impl/common.hpp) over a dense cloud
-__global__ void k_vg_minmax(const float4* __restrict__ pts, int n, VgCtl* c) {
+__global__ void k_vg_minmax(const float4* __restrict__ pts, int n, VgCtl* c, const int* __restrict__ n_dev) {
+    n = dev_count(n_dev, n);
     float mn[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, mx[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const float4 p = pts[i];
@@ -161,11 +196,15 @@ __device__ __forceinline__ VgGrid vg_grid(const VgCtl* c, float leaf) {
     return g;
 }
 
-__global__ void k_vg_keys(const float4* __restrict__ pts, int n, float leaf, VgCtl* c, unsigned* __restrict__ keys, int* __restrict__ vals) {
+// Padding rows (device forms) get the key 0xFFFFFFFF.  Real keys are below 2^31 (the overflow test bounds the grid, passthrough
+// keys are row indices), and a real key equal to it would still precede the padding rows in the stable sort.
+__global__ void k_vg_keys(const float4* __restrict__ pts, int n, float leaf, VgCtl* c, unsigned* __restrict__ keys, int* __restrict__ vals,
+                          const int* __restrict__ n_dev) {
     const VgGrid g = vg_grid(c, leaf);
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i == 0) c->passthrough = g.overflow ? 1 : 0;
     if (i >= n) return;
+    if (i >= dev_count(n_dev, n)) { keys[i] = 0xFFFFFFFFu; vals[i] = i; return; }
     const float4 p = pts[i];
     const int i0 = int(__fsub_rn(floorf(__fmul_rn(p.x, g.inv)), float(g.min_b[0])));
     const int i1 = int(__fsub_rn(floorf(__fmul_rn(p.y, g.inv)), float(g.min_b[1])));
@@ -175,15 +214,18 @@ __global__ void k_vg_keys(const float4* __restrict__ pts, int n, float leaf, VgC
     vals[i] = i;
 }
 
-__global__ void k_vg_heads(const unsigned* __restrict__ keys, int n, int* __restrict__ heads) {
+// padding rows are no heads, so the exclusive scan over n_max rows gives the real rows the positions of the n-row scan
+__global__ void k_vg_heads(const unsigned* __restrict__ keys, int n, int* __restrict__ heads, const int* __restrict__ n_dev) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) heads[i] = (i == 0 || keys[i] != keys[i - 1]) ? 1 : 0;
+    if (i < n) heads[i] = (i < dev_count(n_dev, n) && (i == 0 || keys[i] != keys[i - 1])) ? 1 : 0;
 }
 
 // CentroidPoint per occupied cell: float sums in ascending input index (the radix sort is stable), then / count.
 // One thread per cell walks its run; raw scans put a handful of points into a cell.
 __global__ void k_vg_centroid(const float4* __restrict__ pts, const unsigned* __restrict__ keys, const int* __restrict__ vals,
-                              const int* __restrict__ heads, const int* __restrict__ pos, int n, float4* __restrict__ out, VgCtl* c) {
+                              const int* __restrict__ heads, const int* __restrict__ pos, int n, float4* __restrict__ out, VgCtl* c,
+                              const int* __restrict__ n_dev) {
+    n = dev_count(n_dev, n);
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     if (i == n - 1) c->total = pos[i] + heads[i];
@@ -205,9 +247,21 @@ __global__ void k_vg_centroid(const float4* __restrict__ pts, const unsigned* __
 // ================================================================================================ ScanFrontEnd
 ScanFrontEnd::~ScanFrontEnd() {
     cudaSetDevice(map_->device());
-    DeviceBuffer* all[] = {&raw_, &raw_alt_, &time_, &time_alt_, &down_, &keys_, &keys_alt_, &vals_, &vals_alt_, &heads_, &pos_, &cub_tmp_, &ctl_, &poses_};
+    DeviceBuffer* all[] = {&raw_, &raw_alt_, &time_, &time_alt_, &down_, &keys_, &keys_alt_, &vals_, &vals_alt_, &heads_, &pos_, &cub_tmp_, &ctl_, &poses_,
+                           &d_raw_, &d_time_, &d_sraw_, &d_stime_, &d_down_, &d_keys_, &d_keys_alt_, &d_vals_, &d_vals_alt_, &d_heads_, &d_pos_,
+                           &d_cub_, &d_ctl_};
     for (DeviceBuffer* b : all) b->release();
     if (h_count_) cudaFreeHost(h_count_);
+    if (h_dctl_) cudaFreeHost(h_dctl_);
+}
+
+// k_undistort's dynamic shared memory above the default 48 KB: the attribute only grows, so a launch the host form or
+// fl_scan_reserve allowed stays allowed (a captured graph keeps launching with the size of capture time)
+int ScanFrontEnd::undistort_smem(size_t smem) {
+    if (smem <= undistort_smem_) return FL_OK;
+    FL_CUDA(cudaFuncSetAttribute(k_undistort, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    undistort_smem_ = smem;
+    return FL_OK;
 }
 
 int ScanFrontEnd::init() {
@@ -229,11 +283,13 @@ int ScanFrontEnd::upload(const float* xyzi, const float* offset_ms, int n) {
     }
     n_raw_ = n;
     n_down_ = 0;
+    dev_uploaded_ = dev_undistorted_ = dev_down_ = false;      // the device forms' cloud is no longer the scan's
     return FL_OK;
 }
 
 int ScanFrontEnd::undistort(const double* poses, int n_pose, const double* x26_end) {
     if (n_pose < 0 || (n_pose > 0 && !poses) || !x26_end) { set_last_error("undistort: bad arguments"); return FL_ERR_ARG; }
+    dev_uploaded_ = dev_undistorted_ = dev_down_ = false;      // the host forms now hold the scan's cloud: device forms upload anew
     const int n = n_raw_;
     if (n == 0) return FL_OK;
     FL_CUDA(cudaSetDevice(map_->device()));
@@ -250,15 +306,15 @@ int ScanFrontEnd::undistort(const double* poses, int n_pose, const double* x26_e
     if (n_pose < 2) return FL_OK;                       // no segment: the backward sweep has nothing to walk
     const size_t np = (size_t)n_pose * POSE_DOUBLES;
     const size_t smem = sizeof(double) * np;
-    if (smem > 200 * 1024) { set_last_error("undistort: %d IMU poses do not fit shared memory", n_pose); return FL_ERR_CAPACITY; }
+    if (smem > UNDISTORT_SMEM_MAX) { set_last_error("undistort: %d IMU poses do not fit shared memory", n_pose); return FL_ERR_CAPACITY; }
     // a few KB from pageable host memory: the runtime stages them before returning, the caller's arrays are free at once
     FL_CHECK(poses_.reserve(sizeof(double) * (np + XLEN)));
     FL_CUDA(cudaMemcpyAsync(poses_.ptr, poses, sizeof(double) * np, cudaMemcpyHostToDevice, st));
     FL_CUDA(cudaMemcpyAsync(poses_.as<double>() + np, x26_end, sizeof(double) * XLEN, cudaMemcpyHostToDevice, st));
-    if (smem > 48 * 1024) FL_CUDA(cudaFuncSetAttribute(k_undistort, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    FL_CHECK(undistort_smem(smem));
     const int block = 128;
     k_undistort<<<(n + block - 1) / block, block, smem, st>>>(raw_.as<float4>(), time_.as<float>(), n, poses_.as<double>(), n_pose,
-                                                              poses_.as<double>() + (size_t)n_pose * POSE_DOUBLES);
+                                                              poses_.as<double>() + (size_t)n_pose * POSE_DOUBLES, nullptr, nullptr, nullptr);
     FL_CUDA(cudaGetLastError());
     return FL_OK;
 }
@@ -266,6 +322,7 @@ int ScanFrontEnd::undistort(const double* poses, int n_pose, const double* x26_e
 int ScanFrontEnd::voxel_downsample(float leaf, int* n_out) {
     if (n_out) *n_out = 0;
     if (!(leaf > 0.f)) { set_last_error("voxel_downsample: leaf size must be > 0"); return FL_ERR_ARG; }
+    dev_uploaded_ = dev_undistorted_ = dev_down_ = false;      // the host forms now hold the scan's cloud: device forms upload anew
     const int n = n_raw_;
     n_down_ = 0;
     if (n == 0) return FL_OK;
@@ -280,18 +337,18 @@ int ScanFrontEnd::voxel_downsample(float leaf, int* n_out) {
     FL_CHECK(pos_.reserve(sizeof(int) * (size_t)n));
     VgCtl* ctl = ctl_.as<VgCtl>();
     const int block = 256, grid = (n + block - 1) / block;
-    k_vg_reset<<<1, 32, 0, st>>>(ctl);
-    k_vg_minmax<<<std::min(grid, 132), block, 0, st>>>(raw_.as<float4>(), n, ctl);
-    k_vg_keys<<<grid, block, 0, st>>>(raw_.as<float4>(), n, leaf, ctl, keys_.as<unsigned>(), vals_.as<int>());
+    k_vg_reset<<<1, 32, 0, st>>>(ctl, nullptr);
+    k_vg_minmax<<<std::min(grid, 132), block, 0, st>>>(raw_.as<float4>(), n, ctl, nullptr);
+    k_vg_keys<<<grid, block, 0, st>>>(raw_.as<float4>(), n, leaf, ctl, keys_.as<unsigned>(), vals_.as<int>(), nullptr);
     size_t tmp_sort = 0, tmp_scan = 0;
     FL_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, keys_.as<unsigned>(), keys_alt_.as<unsigned>(), vals_.as<int>(), vals_alt_.as<int>(), n, 0, 32, st));
     FL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_scan, heads_.as<int>(), pos_.as<int>(), n, st));
     FL_CHECK(cub_tmp_.reserve(std::max(tmp_sort, tmp_scan)));
     FL_CUDA(cub::DeviceRadixSort::SortPairs(cub_tmp_.ptr, tmp_sort, keys_.as<unsigned>(), keys_alt_.as<unsigned>(), vals_.as<int>(), vals_alt_.as<int>(), n, 0, 32, st));
-    k_vg_heads<<<grid, block, 0, st>>>(keys_alt_.as<unsigned>(), n, heads_.as<int>());
+    k_vg_heads<<<grid, block, 0, st>>>(keys_alt_.as<unsigned>(), n, heads_.as<int>(), nullptr);
     FL_CUDA(cub::DeviceScan::ExclusiveSum(cub_tmp_.ptr, tmp_scan, heads_.as<int>(), pos_.as<int>(), n, st));
     k_vg_centroid<<<grid, block, 0, st>>>(raw_.as<float4>(), keys_alt_.as<unsigned>(), vals_alt_.as<int>(), heads_.as<int>(), pos_.as<int>(), n,
-                                          down_.as<float4>(), ctl);
+                                          down_.as<float4>(), ctl, nullptr);
     FL_CUDA(cudaGetLastError());
     FL_CUDA(cudaMemcpyAsync(h_count_, &ctl->total, sizeof(int), cudaMemcpyDeviceToHost, st));
     FL_CUDA(cudaStreamSynchronize(st));
@@ -311,6 +368,178 @@ int ScanFrontEnd::download(int which, float* out_xyzi, int cap, int* n) {
     const void* src = which == 0 ? raw_.ptr : down_.ptr;
     FL_CUDA(cudaMemcpyAsync(out_xyzi, src, sizeof(float4) * (size_t)take, cudaMemcpyDeviceToHost, map_->stream()));
     FL_CUDA(cudaStreamSynchronize(map_->stream()));
+    return FL_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ device forms
+// They own a fixed set of buffers, sized here and never by the calls themselves, and never swap them: a captured graph keeps
+// reading and writing the buffers of capture time, whatever host-form calls (which grow and swap their own buffers) ran since.
+int ScanFrontEnd::reserve_device(int n_max, int n_pose_max) {
+    if (n_max < 0 || n_pose_max < 0) { set_last_error("scan reserve: n_max and n_pose_max must be >= 0"); return FL_ERR_ARG; }
+    const size_t smem = sizeof(double) * POSE_DOUBLES * (size_t)n_pose_max;
+    if (smem > UNDISTORT_SMEM_MAX) { set_last_error("scan reserve: %d IMU poses do not fit shared memory", n_pose_max); return FL_ERR_CAPACITY; }
+    FL_CUDA(cudaSetDevice(map_->device()));
+    const size_t m = (size_t)std::max(1, n_max);
+    FL_CHECK(d_raw_.reserve(sizeof(float4) * m));
+    FL_CHECK(d_sraw_.reserve(sizeof(float4) * m));
+    FL_CHECK(d_down_.reserve(sizeof(float4) * m));
+    FL_CHECK(d_time_.reserve(sizeof(float) * m));
+    FL_CHECK(d_stime_.reserve(sizeof(float) * m));
+    FL_CHECK(d_keys_.reserve(sizeof(unsigned) * m));
+    FL_CHECK(d_keys_alt_.reserve(sizeof(unsigned) * m));
+    FL_CHECK(d_vals_.reserve(sizeof(int) * m));
+    FL_CHECK(d_vals_alt_.reserve(sizeof(int) * m));
+    FL_CHECK(d_heads_.reserve(sizeof(int) * m));
+    FL_CHECK(d_pos_.reserve(sizeof(int) * m));
+    size_t t_time = 0, t_vg = 0, t_scan = 0;
+    FL_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t_time, (const float*)nullptr, (float*)nullptr, (const float4*)nullptr, (float4*)nullptr, (int)m));
+    FL_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t_vg, (const unsigned*)nullptr, (unsigned*)nullptr, (const int*)nullptr, (int*)nullptr, (int)m));
+    FL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, t_scan, (const int*)nullptr, (int*)nullptr, (int)m));
+    FL_CHECK(d_cub_.reserve(std::max(t_time, std::max(t_vg, t_scan))));
+    if (!d_ctl_.ptr) {
+        FL_CHECK(d_ctl_.reserve(sizeof(ScanDevCtl)));
+        FL_CUDA(cudaMemsetAsync(d_ctl_.ptr, 0, sizeof(ScanDevCtl), map_->stream()));
+        FL_CUDA(cudaMallocHost(&h_dctl_, sizeof(ScanDevCtl)));
+    }
+    FL_CHECK(undistort_smem(smem));
+    FL_CUDA(cudaStreamSynchronize(map_->stream()));
+    res_n_max_ = std::max(res_n_max_, n_max);
+    res_pose_max_ = std::max(res_pose_max_, n_pose_max);
+    dev_used_ = true;
+    return FL_OK;
+}
+
+const float4* ScanFrontEnd::down_dev() const { return d_down_.as<float4>(); }
+const int* ScanFrontEnd::down_count_dev() const { return &d_ctl_.as<ScanDevCtl>()->vg.total; }
+
+// cub's temporary storage for `n` rows within what reserve_device sized
+int ScanFrontEnd::cub_fits(int n, const char* what) const {
+    size_t t_time = 0, t_vg = 0, t_scan = 0;
+    FL_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t_time, (const float*)nullptr, (float*)nullptr, (const float4*)nullptr, (float4*)nullptr, n));
+    FL_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t_vg, (const unsigned*)nullptr, (unsigned*)nullptr, (const int*)nullptr, (int*)nullptr, n));
+    FL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, t_scan, (const int*)nullptr, (int*)nullptr, n));
+    if (std::max(t_time, std::max(t_vg, t_scan)) > d_cub_.bytes) {
+        set_last_error("%s: %d rows exceed what fl_scan_reserve sized", what, n);
+        return FL_ERR_CAPACITY;
+    }
+    return FL_OK;
+}
+
+int ScanFrontEnd::upload_on_stream(const float* d_xyzi, const float* d_offset_ms, const int* d_n, int n_max, cudaStream_t st) {
+    const int dev = map_->device();
+    if (n_max < 0 || !device_ptr(d_n, dev, 4) || (n_max > 0 && (!device_ptr(d_xyzi, dev, 16) || !device_ptr(d_offset_ms, dev, 4)))) {
+        set_last_error("scan upload_device: n_max < 0, or a buffer is not device memory on device %d (points 16-byte, offset times and "
+                       "n 4-byte aligned)", dev);
+        return FL_ERR_ARG;
+    }
+    if (!d_ctl_.ptr || n_max > res_n_max_) {
+        set_last_error("scan upload_device: n_max = %d exceeds the %d rows fl_scan_reserve sized", n_max, d_ctl_.ptr ? res_n_max_ : 0);
+        return FL_ERR_CAPACITY;
+    }
+    FL_CUDA(cudaSetDevice(dev));
+    bool joined = false;
+    FL_CHECK(map_->query_begin(st, &joined));
+    const int block = 256;
+    k_upload_n<<<std::max(1, (n_max + block - 1) / block), block, 0, st>>>(reinterpret_cast<const float4*>(d_xyzi), d_offset_ms, d_n, n_max,
+                                                                            d_raw_.as<float4>(), d_time_.as<float>(), d_ctl_.as<ScanDevCtl>());
+    FL_CHECK(map_->query_end(st, joined));
+    dev_n_max_ = n_max;
+    dev_uploaded_ = true;
+    dev_undistorted_ = false;
+    dev_down_ = false;
+    return FL_OK;
+}
+
+int ScanFrontEnd::undistort_on_stream(const double* d_poses, const int* d_n_pose, int n_pose_max, const double* d_x26_end, cudaStream_t st) {
+    const int dev = map_->device();
+    if (n_pose_max < 0 || !device_ptr(d_n_pose, dev, 4) || !device_ptr(d_x26_end, dev, 8) || (n_pose_max > 0 && !device_ptr(d_poses, dev, 8))) {
+        set_last_error("scan undistort_device: n_pose_max < 0, or a buffer is not device memory on device %d (poses and x 8-byte, "
+                       "n_pose 4-byte aligned)", dev);
+        return FL_ERR_ARG;
+    }
+    if (!dev_uploaded_) { set_last_error("scan undistort_device: no fl_scan_upload_device since the last host-form upload"); return FL_ERR_STATE; }
+    const size_t smem = sizeof(double) * POSE_DOUBLES * (size_t)n_pose_max;
+    if (n_pose_max > res_pose_max_ || smem > UNDISTORT_SMEM_MAX) {
+        set_last_error("scan undistort_device: n_pose_max = %d exceeds the %d poses fl_scan_reserve sized", n_pose_max, res_pose_max_);
+        return FL_ERR_CAPACITY;
+    }
+    const int n = dev_n_max_;
+    FL_CHECK(cub_fits(n, "scan undistort_device"));
+    FL_CUDA(cudaSetDevice(dev));
+    bool joined = false;
+    FL_CHECK(map_->query_begin(st, &joined));
+    // the stable time sort of n_max rows (the padding rows last, see k_upload_n), then the backward pass over the first n
+    size_t tmp = d_cub_.bytes;
+    FL_CUDA(cub::DeviceRadixSort::SortPairs(d_cub_.ptr, tmp, d_time_.as<float>(), d_stime_.as<float>(), d_raw_.as<float4>(), d_sraw_.as<float4>(),
+                                            n, 0, 32, st));
+    const int block = 128;
+    ScanDevCtl* c = d_ctl_.as<ScanDevCtl>();
+    k_undistort<<<std::max(1, (n + block - 1) / block), block, smem, st>>>(d_sraw_.as<float4>(), d_stime_.as<float>(), n, d_poses, n_pose_max,
+                                                                           d_x26_end, &c->n_raw, d_n_pose, c);
+    FL_CHECK(map_->query_end(st, joined));
+    dev_undistorted_ = true;
+    return FL_OK;
+}
+
+int ScanFrontEnd::voxel_downsample_on_stream(float leaf, int* d_n_out, cudaStream_t st) {
+    const int dev = map_->device();
+    if (!(leaf > 0.f)) { set_last_error("voxel_downsample_device: leaf size must be > 0"); return FL_ERR_ARG; }
+    if (d_n_out && !device_ptr(d_n_out, dev, 4)) { set_last_error("voxel_downsample_device: n_out must be 4-byte aligned device memory on device %d", dev); return FL_ERR_ARG; }
+    if (!dev_uploaded_) { set_last_error("voxel_downsample_device: no fl_scan_upload_device since the last host-form upload"); return FL_ERR_STATE; }
+    const int n = dev_n_max_;
+    FL_CHECK(cub_fits(n, "voxel_downsample_device"));
+    FL_CUDA(cudaSetDevice(dev));
+    bool joined = false;
+    FL_CHECK(map_->query_begin(st, &joined));
+    ScanDevCtl* c = d_ctl_.as<ScanDevCtl>();
+    VgCtl* ctl = &c->vg;
+    const int* cnt = &c->n_raw;
+    const float4* src = dev_undistorted_ ? d_sraw_.as<float4>() : d_raw_.as<float4>();
+    unsigned *keys = d_keys_.as<unsigned>(), *keys_alt = d_keys_alt_.as<unsigned>();
+    int *vals = d_vals_.as<int>(), *vals_alt = d_vals_alt_.as<int>(), *heads = d_heads_.as<int>(), *pos = d_pos_.as<int>();
+    const int block = 256, grid = std::max(1, (n + block - 1) / block);
+    k_vg_reset<<<1, 32, 0, st>>>(ctl, c);
+    k_vg_minmax<<<std::min(grid, 132), block, 0, st>>>(src, n, ctl, cnt);
+    k_vg_keys<<<grid, block, 0, st>>>(src, n, leaf, ctl, keys, vals, cnt);
+    size_t tmp = d_cub_.bytes;
+    FL_CUDA(cub::DeviceRadixSort::SortPairs(d_cub_.ptr, tmp, keys, keys_alt, vals, vals_alt, n, 0, 32, st));
+    k_vg_heads<<<grid, block, 0, st>>>(keys_alt, n, heads, cnt);
+    tmp = d_cub_.bytes;
+    FL_CUDA(cub::DeviceScan::ExclusiveSum(d_cub_.ptr, tmp, heads, pos, n, st));
+    k_vg_centroid<<<grid, block, 0, st>>>(src, keys_alt, vals_alt, heads, pos, n, d_down_.as<float4>(), ctl, cnt);
+    FL_CUDA(cudaGetLastError());
+    if (d_n_out) FL_CUDA(cudaMemcpyAsync(d_n_out, &ctl->total, sizeof(int), cudaMemcpyDeviceToDevice, st));
+    FL_CHECK(map_->query_end(st, joined));
+    dev_down_ = true;
+    return FL_OK;
+}
+
+// Host forms after device forms: when the device forms produced the current cloud (their upload ran after the host forms' last
+// one, directly or in a graph replay), its counts are read back and its clouds copied into the host forms' buffers, so the host
+// forms continue from exactly the state the host-form chain would have left.  One read-back per host-form call once the device
+// forms are in use; none before.
+int ScanFrontEnd::settle() {
+    if (!dev_used_) return FL_OK;
+    FL_CUDA(cudaSetDevice(map_->device()));
+    cudaStream_t st = map_->stream();
+    FL_CUDA(cudaMemcpyAsync(h_dctl_, d_ctl_.ptr, sizeof(ScanDevCtl), cudaMemcpyDeviceToHost, st));
+    FL_CUDA(cudaStreamSynchronize(st));
+    const ScanDevCtl h = *static_cast<const ScanDevCtl*>(h_dctl_);
+    if (!h.src) return FL_OK;
+    const int n = h.n_raw;
+    FL_CHECK(raw_.reserve(sizeof(float4) * (size_t)std::max(1, n)));
+    FL_CHECK(time_.reserve(sizeof(float) * (size_t)std::max(1, n)));
+    if (n > 0) {
+        FL_CUDA(cudaMemcpyAsync(raw_.ptr, h.stage ? d_sraw_.ptr : d_raw_.ptr, sizeof(float4) * (size_t)n, cudaMemcpyDeviceToDevice, st));
+        FL_CUDA(cudaMemcpyAsync(time_.ptr, h.stage ? d_stime_.ptr : d_time_.ptr, sizeof(float) * (size_t)n, cudaMemcpyDeviceToDevice, st));
+    }
+    n_raw_ = n;
+    n_down_ = h.down ? h.vg.total : 0;
+    if (n_down_ > 0) {
+        FL_CHECK(down_.reserve(sizeof(float4) * (size_t)n_down_));
+        FL_CUDA(cudaMemcpyAsync(down_.ptr, d_down_.ptr, sizeof(float4) * (size_t)n_down_, cudaMemcpyDeviceToDevice, st));
+    }
+    FL_CUDA(cudaMemsetAsync(&d_ctl_.as<ScanDevCtl>()->src, 0, sizeof(int), st));
     return FL_OK;
 }
 

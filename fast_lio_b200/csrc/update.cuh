@@ -719,8 +719,10 @@ __device__ void sol_pass(SolverSm& S, FilterCtl* ctl, PassLog* logs, unsigned lo
 // search partner per point (knn_block_pair): 512 threads, one block per SM, the same 128-register cap.  Warps 8..15 only help
 // on the searching passes and otherwise just join the block barriers; the tiles, the partial rows and every sum are those of
 // PAIR = 1, so both forms give the same bytes.
+// The body is shared by k_update (the scan's points [q_begin, q_end)) and k_update_n (a point count in device memory): q1 is
+// the end of the points the workers measure.
 template <bool EXTR, int PAIR>
-__global__ void __launch_bounds__(UPD_THREADS * PAIR, 3 - PAIR) k_update(UpdArgs a) {
+__device__ __forceinline__ void update_body(const UpdArgs& a, const int q1) {
     static_assert(PAIR == 1 || PAIR == 2, "one or two threads per point");
     static_assert(sizeof(PairXch) <= sizeof(double) * WorkerSm<EXTR>::STAGE, "the partner's list fits the owner warp's stage slice");
     __shared__ __align__(16) unsigned char smem_raw[sizeof(SolverSm) > sizeof(WorkerSm<EXTR>) ? sizeof(SolverSm) : sizeof(WorkerSm<EXTR>)];
@@ -778,7 +780,7 @@ __global__ void __launch_bounds__(UPD_THREADS * PAIR, 3 - PAIR) k_update(UpdArgs
             double* stage = Wk.stage[warp & (UPD_WARPS - 1)];          // a partner warp hands its lists over in its owner's slice
             // tiles of UPD_THREADS consecutive points, dealt round-robin to the worker blocks -- the same tiles every pass (a point's
             // cached neighbours, plane and flag are only ever touched by its own thread)
-            const int q0 = a.sc.q_begin, q1 = a.sc.q_end;
+            const int q0 = a.sc.q_begin;
             for (int tile = q0 + wb * UPD_THREADS; tile < q1; tile += nwork * UPD_THREADS) {
                 const int q = tile + (tid & (UPD_THREADS - 1));
                 double h[12]; double z = 0.0; float ar = 0.f;
@@ -844,6 +846,21 @@ __global__ void __launch_bounds__(UPD_THREADS * PAIR, 3 - PAIR) k_update(UpdArgs
     if (tid == 0) { ctl->error = S.error | ctl->error; ctl->ticket = 0; }
     sol_sync();
     mirror_copy(ctl, UPD_THREADS);
+}
+
+template <bool EXTR, int PAIR>
+__global__ void __launch_bounds__(UPD_THREADS * PAIR, 3 - PAIR) k_update(UpdArgs a) {
+    update_body<EXTR, PAIR>(a, a.sc.q_end);
+}
+
+// fl_filter_update_scan_device: the points [q_begin, min(*n, q_end)), q_end the row bound the grid was sized for.  The tiles
+// below the count go to the blocks the host form gives them; blocks beyond write +0.0 partial rows, which leave sol_reduce's
+// fixed-order sums (they start from +0.0) unchanged, so the result is the host form's at count *n.  *n is written before the
+// kernel ahead of this one starts (fl_filter_update_scan_device copies it before k_state_in), so it may be read ahead of
+// pdl_wait().
+template <bool EXTR, int PAIR>
+__global__ void __launch_bounds__(UPD_THREADS * PAIR, 3 - PAIR) k_update_n(UpdArgs a, const int* __restrict__ n) {
+    update_body<EXTR, PAIR>(a, min(*n, a.sc.q_end));
 }
 
 }  // namespace fl

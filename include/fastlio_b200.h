@@ -310,6 +310,57 @@ int fl_scan_download(fl_scan_t* s, int which, float* out_xyzi, int cap);
 /* fl_filter_update on the down-sampled cloud of `s` without a host hop */
 int fl_filter_update_scan(fl_filter_t* f, fl_scan_t* s, double* x26, double* P, double R, double* solve_time_s);
 
+/* ---- device-buffer forms of the scan front end and of the update on it (the conventions of the map's *_device block above)
+ * Per scan, upload -> undistort -> voxel_downsample -> fl_filter_update_scan_device -> fl_filter_map_incremental_device run on
+ * the caller's stream with every point count in device memory, so one CUDA graph captured with an upper bound n_max replays a
+ * whole scan of any size up to it.  esekf::predict and lasermap_fov_segment stay on the host between replays.
+ * None of them synchronises the host, allocates, or sizes a launch from a device value: grids follow n_max (the n_max of the
+ * last fl_scan_upload_device) and the kernels stop at the device counts.  Host, wrong-device, null or misaligned pointers are
+ * FL_ERR_ARG; an n_max or n_pose_max above what fl_scan_reserve sized is FL_ERR_CAPACITY; nothing is enqueued on a refusal.
+ * Ordering: outside capture `stream` first waits for everything enqueued on the map's stream and the map's stream then waits
+ * for the call (Map::query_begin / query_end); inside capture nothing is joined.
+ * They use buffers of their own, which host-form calls never move, so a graph stays valid across host-form calls on the scan;
+ * capture again after fl_scan_reserve grows them.  Each call's outputs equal, byte for byte, those of its host form at the device
+ * count n; rows from n up to n_max of the device-form buffers are unspecified.
+ * Host forms after device forms: fl_scan_upload / undistort / voxel_downsample / download and fl_filter_update_scan first read
+ * the device counts back (once per call, and only once the device forms are in use).  Every device-form stage marks its result
+ * as the scan's current one on the device, so when a device-form stage ran after the host forms last took the cloud over
+ * (directly or in a graph replay: synchronise replays before host-form calls), the host forms continue from the state the
+ * host-form chain would have left.  A host-form undistort or voxel_downsample replaces the cloud: the device-form stages then
+ * need a new fl_scan_upload_device (FL_ERR_STATE before it).  Likewise fl_filter_get_nearest / get_selected / map_incremental /
+ * get_pass_logs read back which update bound the filter's scan last (a device form, also in a graph replay, or a host form)
+ * and run over that scan and its count. */
+/* Sizes every device-form buffer, cub's temporary storage for both sorts, and k_undistort's shared memory for up to n_max points
+ * and n_pose_max IMU poses (grow-only).  Synchronous.  FL_ERR_CAPACITY when n_pose_max poses exceed the shared memory
+ * fl_scan_undistort allows. */
+int fl_scan_reserve(fl_scan_t* s, int n_max, int n_pose_max);
+/* Measures.lidar (common_lib.h:47-58) from device memory: the first *n_device points (clamped to [0, n_max]) of xyzi_device
+ * (4 floats each) and offset_ms_device (PointType::curvature) are copied into the scan, so the caller may reuse its buffers once
+ * `stream` has passed the call. */
+int fl_scan_upload_device(fl_scan_t* s, const float* xyzi_device, const float* offset_ms_device, const int* n_device, int n_max,
+                          void* stream);
+/* ImuProcess::UndistortPcl, the sort (:234) and the backward pass (:312-346)         IMU_Processing.hpp:216-346
+ * The cloud of the last fl_scan_upload_device, sorted by offset time (stable, over n_max rows whose padding sorts last) and
+ * de-skewed with the first *n_pose_device (clamped to [0, n_pose_max]) poses of imu_pose22_device (n_pose_max x 22 doubles, the
+ * layout of fl_scan_undistort) and x26_end_device (26 doubles), which are read when `stream` reaches the call.  Fewer than two
+ * poses leave the points as sorted, as in fl_scan_undistort.  FL_ERR_STATE without a device-form upload since the last
+ * host-form upload, undistort or voxel_downsample. */
+int fl_scan_undistort_device(fl_scan_t* s, const double* imu_pose22_device, const int* n_pose_device, int n_pose_max,
+                             const double* x26_end_device, void* stream);
+/* downSizeFilterSurf.filter(*feats_down_body)                                        laserMapping.cpp:904-905
+ * fl_scan_voxel_downsample of the device forms' cloud (de-skewed or as uploaded).  feats_down_size stays in the scan for
+ * fl_filter_update_scan_device, and is also copied to n_out_device (may be NULL).  FL_ERR_STATE without a device-form upload since the
+ * last host-form upload, undistort or voxel_downsample. */
+int fl_scan_voxel_downsample_device(fl_scan_t* s, float leaf_size, int* n_out_device, void* stream);
+/* esekf::update_iterated_dyn_share_modified with feats_down_body bound      esekfom.hpp:1619-1931, laserMapping.cpp:638-754, :960
+ * fl_filter_update_scan on device buffers: the contract of fl_filter_update_device for x26_device, P_device and status2_device,
+ * on the device forms' down-sampled cloud of `s` (bound in place, like fl_filter_update_scan) with its count read on the device.
+ * Grids follow the scan's n_max; fl_filter_map_incremental_device afterwards also runs over the device count with n_max = the
+ * scan's n_max.  A sharded, solver-0 or fused-0 filter, or a scan without fl_scan_voxel_downsample_device since its last upload,
+ * is FL_ERR_STATE; a filter capacity below the scan's n_max FL_ERR_CAPACITY; a scan on another map FL_ERR_ARG. */
+int fl_filter_update_scan_device(fl_filter_t* f, fl_scan_t* s, double* x26_device, double* P_device, double R, int* status2_device,
+                                 void* stream);
+
 /* ------------------------------------------------------------------ local-map cube (SURVEY.md §8f row 2)
  * lasermap_fov_segment()                                            laserMapping.cpp:229-277
  * LocalMap_Points / Localmap_Initialized (:229-230) live in the handle; cube_len = cube_side_length (:774),
