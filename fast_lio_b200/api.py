@@ -52,7 +52,7 @@ SYMBOLS = [
     "fl_filter_update_device", "fl_filter_get_nearest_device", "fl_filter_get_selected_device",
     "fl_map_add_points_async", "fl_map_maintain", "fl_filter_map_incremental_device",
     "fl_scan_reserve", "fl_scan_upload_device", "fl_scan_undistort_device", "fl_scan_voxel_downsample_device",
-    "fl_filter_update_scan_device",
+    "fl_filter_update_scan_device", "fl_map_delete_boxes_async", "fl_localmap_segment_device",
 ]
 
 
@@ -102,6 +102,7 @@ def load():
     L.fl_map_add_points_device.argtypes = [_vp, _vp, C.c_int, C.c_int, _vp]
     L.fl_map_add_points_async.argtypes = [_vp, _vp, _vp, C.c_int, C.c_int, _vp, _vp]
     L.fl_map_maintain.argtypes = [_vp, C.POINTER(C.c_int)]
+    L.fl_map_delete_boxes_async.argtypes = [_vp, _vp, _vp, C.c_int, _vp, _vp]
     L.fl_filter_map_incremental_device.argtypes = [_vp, C.c_double, C.c_int, _vp, _vp]
     L.fl_filter_update_device.argtypes = [_vp, _vp, C.c_int, _vp, _vp, C.c_double, _vp, _vp]
     L.fl_filter_get_nearest_device.argtypes = [_vp, _vp, _vp, C.c_int, _vp]
@@ -142,6 +143,7 @@ def load():
     L.fl_localmap_destroy.argtypes = [C.c_void_p]
     L.fl_localmap_segment.argtypes = [C.c_void_p, C.c_void_p, _f64p, _f32p, C.POINTER(C.c_int)]
     L.fl_localmap_get.argtypes = [C.c_void_p, _f32p]
+    L.fl_localmap_segment_device.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp]
     L.fl_comm_unique_id.argtypes = [C.c_char_p]
     L.fl_filter_comm_init.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_char_p]
     L.fl_filter_set_shard.argtypes = [C.c_void_p, C.c_int, C.c_int]
@@ -401,6 +403,22 @@ class KdTree:
         status = self._tensor(status, "status", None, torch.int32, (2,))
         _check(self._L.fl_map_add_points_async(self.h, pts.data_ptr() if n_max > 0 else None, n.data_ptr(), n_max,
                                                int(downsample_on), status.data_ptr(), self._stream()))
+        return status
+
+    def delete_boxes_async(self, boxes, nb, nb_max: int, status=None):
+        """fl_map_delete_boxes_async: Delete_Point_Boxes of the first *nb rows of boxes ((>= nb_max, 6) float32), nb an int32 CUDA
+        tensor of one element read when the current stream reaches the call.  Returns status, an int32 tensor (2,) = (FL_OK, 1 =
+        maintenance due, or FL_ERR_CAPACITY = nothing changed; the number of points deleted), written on the current stream."""
+        import torch
+        boxes = self._tensor(boxes, "boxes", 6)
+        if boxes.shape[0] < nb_max:
+            raise ValueError(f"boxes: {boxes.shape[0]} rows, fewer than nb_max = {nb_max}")
+        nb = self._tensor(nb, "nb", None, torch.int32, (1,))
+        if status is None:
+            status = torch.empty(2, dtype=torch.int32, device=boxes.device)
+        status = self._tensor(status, "status", None, torch.int32, (2,))
+        _check(self._L.fl_map_delete_boxes_async(self.h, boxes.data_ptr() if nb_max > 0 else None, nb.data_ptr(), nb_max,
+                                                 status.data_ptr(), self._stream()))
         return status
 
     def maintain(self) -> bool:
@@ -745,6 +763,24 @@ class LocalMap:
         nb = _check(self._L.fl_localmap_segment(self.h, tree.h if tree is not None else None,
                                                 np.ascontiguousarray(pos_lid, dtype=np.float64), boxes, C.byref(nd)))
         return boxes[:nb].copy(), nd.value
+
+    def segment_device(self, tree: "KdTree", x, out3=None, boxes=None, n_scan=None):
+        """fl_localmap_segment_device on the current stream: pos_lid from x ((26,) float64 CUDA tensor), the cube slid on the map's
+        device and Delete_Point_Boxes of cub_needrm on `tree`, all-or-nothing.  Returns out3, an int32 tensor (3,) = (|cub_needrm|,
+        kdtree_delete_counter, status); boxes ((3, 6) float32, optional) receives cub_needrm; n_scan (int32 (1,), optional): a 0
+        there skips the call's work, as the reference skips an empty scan."""
+        import torch
+        x = tree._tensor(x, "x", None, torch.float64, (26,))
+        if out3 is None:
+            out3 = torch.empty(3, dtype=torch.int32, device=x.device)
+        out3 = tree._tensor(out3, "out3", None, torch.int32, (3,))
+        if boxes is not None:
+            boxes = tree._tensor(boxes, "boxes", None, torch.float32, (3, 6))
+        if n_scan is not None:
+            n_scan = tree._tensor(n_scan, "n_scan", None, torch.int32, (1,))
+        _check(self._L.fl_localmap_segment_device(self.h, tree.h, x.data_ptr(), n_scan.data_ptr() if n_scan is not None else None,
+                                                  boxes.data_ptr() if boxes is not None else None, out3.data_ptr(), tree._stream()))
+        return out3
 
     def box(self) -> np.ndarray:
         b = np.zeros(6, dtype=np.float32)

@@ -41,6 +41,7 @@ struct fl_scan {
 };
 struct fl_localmap {
     fl::LocalMapCube cube;
+    fl_map* map = nullptr;          // the map of the device form (retained), whose device holds the cube from then on
 };
 
 static_assert(sizeof(fl_pass_log_t) == sizeof(fl::PassLog), "pass-log layouts must match");
@@ -201,6 +202,12 @@ int fl_map_add_points_async(fl_map_t* m, const float* pts_xyzi_device, const int
     MAP_GUARD(m);
     return m->impl->add_points_async_checked(pts_xyzi_device, n_device, n_max, downsample_on != 0, status2_device,
                                              static_cast<cudaStream_t>(stream));
+}
+// Device form of Delete_Point_Boxes: never settles either
+int fl_map_delete_boxes_async(fl_map_t* m, const float* boxes6_device, const int* nb_device, int nb_max, int* status2_device,
+                              void* stream) {
+    MAP_GUARD(m);
+    return m->impl->delete_boxes_async_checked(boxes6_device, nb_device, nb_max, status2_device, static_cast<cudaStream_t>(stream));
 }
 int fl_map_maintain(fl_map_t* m, int* layout_changed) {
     MAP_GUARD(m);
@@ -498,12 +505,26 @@ int fl_localmap_create(fl_localmap_t** out, double cube_len, float det_range) {
     *out = l;
     return FL_OK;
 }
-int fl_localmap_destroy(fl_localmap_t* l) { delete l; return FL_OK; }
+int fl_localmap_destroy(fl_localmap_t* l) {
+    if (!l) return FL_OK;
+    fl_map* m = l->map;
+    delete l;
+    if (m) map_release(m);
+    return FL_OK;
+}
 int fl_localmap_segment(fl_localmap_t* l, fl_map_t* map, const double* pos_lid, float* boxes6_out, int* n_deleted) {
     if (n_deleted) *n_deleted = 0;
     if (!l || !pos_lid) { fl::set_last_error("fl_localmap_segment: null argument"); return FL_ERR_ARG; }
     float boxes[18];
-    const int nb = l->cube.slide(pos_lid, boxes);
+    int nb = 0;
+    if (l->map) {                                     // the device form's cube is the cube: read it, slide, write it back
+        std::lock_guard<std::mutex> lk(l->map->mu);
+        int rc = l->cube.pull();
+        if (rc == FL_OK) { nb = l->cube.slide(pos_lid, boxes); rc = l->cube.push(); }
+        if (rc != FL_OK) return rc;
+    } else {
+        nb = l->cube.slide(pos_lid, boxes);
+    }
     if (boxes6_out) for (int i = 0; i < nb * 6; i++) boxes6_out[i] = boxes[i];
     if (nb > 0 && map) {                              // if (cub_needrm.size() > 0) ikdtree.Delete_Point_Boxes(cub_needrm)  (:275)
         int deleted = fl_map_delete_boxes(map, boxes, nb);
@@ -514,9 +535,27 @@ int fl_localmap_segment(fl_localmap_t* l, fl_map_t* map, const double* pos_lid, 
 }
 int fl_localmap_get(fl_localmap_t* l, float* box6) {
     if (!l || !box6) return FL_ERR_ARG;
+    if (l->map) {
+        std::lock_guard<std::mutex> lk(l->map->mu);
+        const int rc = l->cube.pull();
+        if (rc != FL_OK) return rc;
+    }
     if (!l->cube.initialized()) { fl::set_last_error("fl_localmap_get: the cube is placed by the first fl_localmap_segment call"); return FL_ERR_STATE; }
     l->cube.get(box6);
     return FL_OK;
+}
+// Device form: the guard touch()es the map, so the call is ordered after everything enqueued on the map's stream
+int fl_localmap_segment_device(fl_localmap_t* l, fl_map_t* map, const double* x26_device, const int* n_scan_device,
+                               float* boxes18_device, int* out3_device, void* stream) {
+    if (!l) { fl::set_last_error("fl_localmap_segment_device: null cube handle"); return FL_ERR_ARG; }
+    if (l->map && l->map != map) { fl::set_last_error("fl_localmap_segment_device: the cube lives on another map"); return FL_ERR_ARG; }
+    MAP_GUARD(map);
+    const int rc = l->cube.segment_on_stream(map->impl, x26_device, n_scan_device, boxes18_device, out3_device,
+                                             static_cast<cudaStream_t>(stream));
+    // the cube moved to the map's device (even when a later step of the call failed): from now on it is the cube, and the map
+    // stays alive as long as the handle
+    if (!l->map && l->cube.device_map()) { l->map = map; map_retain(map); }
+    return rc;
 }
 
 // ------------------------------------------------------------------------------------ multi-GPU

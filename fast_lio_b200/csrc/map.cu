@@ -48,7 +48,9 @@ enum Counter { C_LEAF_USED = 0, C_DELETED, C_ADDED, C_GROUPS, C_NINSERT, C_TOMB,
                // sizes as read (RA, RB) and as applied (NA, NB: 0 when the plan refused), the plan's counts, its verdict, and
                // "maintenance due" (the host form would have re-packed or re-listed); C_REFUSED: a call was refused since the last
                // fl_map_maintain (sticky, unlike C_SKIP), C_NEED: the list-pool need the plan last computed
-               C_VALID, C_TOMBS, C_RA, C_RB, C_NA, C_NB, C_MISS, C_FIXES, C_SKIP, C_DUE, C_REFUSED, C_NEED, C_COUNT = 32 };
+               C_VALID, C_TOMBS, C_RA, C_RB, C_NA, C_NB, C_MISS, C_FIXES, C_SKIP, C_DUE, C_REFUSED, C_NEED,
+               // device form of Delete_Point_Boxes: the box count the plan let through (0 when it refused), and its verdict
+               C_DEL_NB, C_DEL_SKIP, C_COUNT = 32 };
 
 // ============================================================================= kernels
 // ----------------------------------------------------------------------------- k-d partition build
@@ -177,8 +179,10 @@ __global__ void k_fill_leaves(MapView m, const float4* __restrict__ src, const u
     m.payload[slot] = p.w;
 }
 
-// One warp per main leaf: AABB of the valid points of the leaf and of its overflow chain.
-__global__ void k_refit_leaves(MapView m) {
+// One warp per main leaf: AABB of the valid points of the leaf and of its overflow chain.  gate (may be null): the device form of
+// Delete_Point_Boxes refits only when its deleted count there is non-zero, as the host form does.
+__global__ void k_refit_leaves(MapView m, const int* __restrict__ gate) {
+    if (gate && *gate == 0) return;
     const int lane = threadIdx.x & 31;
     const int warps = (gridDim.x * blockDim.x) >> 5;
     for (int leaf = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; leaf < m.n_main; leaf += warps) {
@@ -206,7 +210,8 @@ __global__ void k_refit_leaves(MapView m) {
 }
 
 // One warp per entity of level k (k >= 1): union of its <= 32 children boxes.
-__global__ void k_refit_level(MapView m, int k) {
+__global__ void k_refit_level(MapView m, int k, const int* __restrict__ gate) {
+    if (gate && *gate == 0) return;
     const int lane = threadIdx.x & 31;
     const int warps = (gridDim.x * blockDim.x) >> 5;
     for (int e = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; e < m.count[k]; e += warps) {
@@ -491,9 +496,15 @@ __global__ void __launch_bounds__(256) k_knn_k(MapView m, const float4* __restri
 
 // Delete_Point_Boxes: every slot tests itself against the boxes (half-open, ikd_Tree.cpp:796).
 // A flat pass over the leaf array is bandwidth-trivial on HBM3e (16 B per slot) and needs
-// no tree descent, no lazy flags and no push-down.
+// no tree descent, no lazy flags and no push-down.  nb_dev / used_dev (may be null): the box count and the used-leaf count read
+// from device memory (the device form: the host's mirror of the used leaves misses those device-form inserts claimed since the
+// map last settled); the grid is then sized without them.
 __global__ void k_delete_boxes(MapView m, const float* __restrict__ boxes, int nb, int n_leaf_used, int* counters,
-                               float4* __restrict__ removed, int removed_cap) {
+                               float4* __restrict__ removed, int removed_cap, const int* __restrict__ nb_dev,
+                               const int* __restrict__ used_dev) {
+    if (nb_dev) nb = *nb_dev;
+    if (used_dev) n_leaf_used = *used_dev;
+    if (nb <= 0) return;
     const long long total = (long long)n_leaf_used * LEAF;
     const int lane = threadIdx.x & 31;
     int local = 0;
@@ -518,6 +529,31 @@ __global__ void k_delete_boxes(MapView m, const float* __restrict__ boxes, int n
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) local += __shfl_xor_sync(FULL, local, o);
     if (lane == 0 && local) atomicAdd(&counters[C_DELETED], local);
+}
+// Delete_Point_Boxes on the caller's stream.  The plan, before any slot is touched: the box count, and room in the removed-points
+// record for every valid point on top of what it holds (the host form grows the record to that before each delete).  Without
+// room nothing is deleted; the next full settle (fl_map_maintain) grows the record, as it does whenever the record is started.
+// A delete refusal leaves C_REFUSED alone: that flag makes the settle grow the map and its directory for the Add_Points forms.
+__global__ void k_delete_plan(int* counters, const int* __restrict__ nb_dev, int nb_max, bool record, int removed_cap) {
+    const int nb = min(max(*nb_dev, 0), nb_max);
+    const bool ok = nb == 0 || !record || (long long)counters[C_REMOVED] + counters[C_VALID] <= removed_cap;
+    counters[C_DEL_NB] = ok ? nb : 0;
+    counters[C_DEL_SKIP] = !ok;
+    counters[C_DELETED] = 0;
+}
+// after the delete: the host form's bookkeeping (delete_boxes) and its maybe_rebuild, which here only marks maintenance as due
+__global__ void k_delete_account(MapView m, int* counters, int chain_limit) {
+    const int d = counters[C_DELETED];
+    if (d == 0) return;
+    counters[C_VALID] -= d;
+    counters[C_TOMBS] += d;
+    const int tombs = counters[C_TOMBS];
+    if ((tombs > 1024 && tombs > counters[C_VALID]) || counters[C_LEAF_USED] - m.n_main > chain_limit) counters[C_DUE] = 1;
+}
+// status2 = (status, deleted)
+__global__ void k_delete_status(const int* __restrict__ counters, int* __restrict__ out) {
+    out[0] = counters[C_DEL_SKIP] ? FL_ERR_CAPACITY : (counters[C_DUE] ? 1 : FL_OK);
+    out[1] = counters[C_DELETED];
 }
 // Add_Point_Boxes (ikd_Tree.cpp:576-603 -> Add_by_range :854-934): points deleted by Delete_Point_Boxes that lie in the boxes
 // and have not been overwritten since come back (points removed by down-sampling do not, as in the reference)
@@ -1178,9 +1214,12 @@ int Map::ensure_capacity(int n_points) {
 
 int Map::refit() {
     FL_CUDA(cudaSetDevice(device_));
-    k_refit_leaves<<<blocks_for((long long)v_.n_main * 32, 256), 256, 0, stream_>>>(v_);
+    return refit_on(stream_, nullptr);
+}
+int Map::refit_on(cudaStream_t st, const int* gate) {
+    k_refit_leaves<<<blocks_for((long long)v_.n_main * 32, 256), 256, 0, st>>>(v_, gate);
     for (int k = 1; k < v_.n_levels; k++)
-        k_refit_level<<<blocks_for((long long)v_.count[k] * 32, 256), 256, 0, stream_>>>(v_, k);
+        k_refit_level<<<blocks_for((long long)v_.count[k] * 32, 256), 256, 0, st>>>(v_, k, gate);
     FL_CUDA(cudaGetLastError());
     return FL_OK;
 }
@@ -1374,20 +1413,10 @@ int Map::delete_boxes(const float* boxes6, int nb, int* deleted) {
     FL_CUDA(cudaMemcpyAsync(scratch_.ptr, boxes6, sizeof(float) * 6 * (size_t)nb, cudaMemcpyHostToDevice, stream_));
     FL_CUDA(cudaMemsetAsync(&counters_.as<int>()[C_DELETED], 0, sizeof(int), stream_));
     const int used = h_counters_[C_LEAF_USED];
-    if (record_removed_) {      // room for the worst case on top of what is already recorded
-        const size_t want = (size_t)n_removed_ + (size_t)n_valid_;
-        if (want * sizeof(float4) > removed_.bytes) {
-            DeviceBuffer bigger;
-            FL_CHECK(bigger.reserve(sizeof(float4) * (want + want / 2)));
-            if (n_removed_) FL_CUDA(cudaMemcpyAsync(bigger.ptr, removed_.ptr, sizeof(float4) * (size_t)n_removed_, cudaMemcpyDeviceToDevice, stream_));
-            FL_CUDA(cudaStreamSynchronize(stream_));
-            removed_.release();
-            removed_ = bigger;
-        }
-    }
+    if (record_removed_) FL_CHECK(removed_room());
     k_delete_boxes<<<blocks_for((long long)used * LEAF, 256), 256, 0, stream_>>>(v_, scratch_.as<float>(), nb, used, counters_.as<int>(),
                                                                                    record_removed_ ? removed_.as<float4>() : nullptr,
-                                                                                   (int)std::min<size_t>(removed_.bytes / sizeof(float4), 0x7fffffff));
+                                                                                   removed_cap(), nullptr, nullptr);
     FL_CUDA(cudaGetLastError());
     FL_CUDA(cudaMemcpyAsync(&h_counters_[C_DELETED], &counters_.as<int>()[C_DELETED], sizeof(int), cudaMemcpyDeviceToHost, stream_));
     FL_CUDA(cudaStreamSynchronize(stream_));
@@ -1403,6 +1432,79 @@ int Map::delete_boxes(const float* boxes6, int nb, int* deleted) {
     return FL_OK;
 }
 
+// Room in the removed-points record for the worst case of one more delete: every valid point on top of what it holds.  A record
+// that is allocated or moves leaves graphs captured before stale (they hold no record, or the old one).  Synchronous; the map
+// must be settled.
+int Map::removed_room() {
+    const size_t want = (size_t)n_removed_ + (size_t)n_valid_;
+    if (want * sizeof(float4) <= removed_.bytes && removed_.ptr) return FL_OK;
+    DeviceBuffer bigger;
+    FL_CHECK(bigger.reserve(sizeof(float4) * std::max<size_t>(want + want / 2, 1)));
+    if (n_removed_) FL_CUDA(cudaMemcpyAsync(bigger.ptr, removed_.ptr, sizeof(float4) * (size_t)n_removed_, cudaMemcpyDeviceToDevice, stream_));
+    FL_CUDA(cudaStreamSynchronize(stream_));
+    layout_dirty_ = true;
+    removed_.release();
+    removed_ = bigger;
+    return FL_OK;
+}
+int Map::removed_cap() const { return (int)std::min<size_t>(removed_.bytes / sizeof(float4), 0x7fffffff); }
+
+// Delete_Point_Boxes of up to nb_max boxes at `boxes`, count at *nb_dev, on `st`; status2 = (status, deleted).  The plan decides
+// first (k_delete_plan); the pass over the slots reads the used leaves from the device counters, and the refit runs only when a
+// point went away.  Every grid is fixed on the host: the same launches whether or not anything is deleted.
+int Map::enqueue_delete(const float* boxes, const int* nb_dev, int nb_max, int* status2, cudaStream_t st) {
+    int* d_cnt = counters_.as<int>();
+    const int chain_limit = std::max(64, (int)(rebuild_overflow_frac_ * v_.n_main));
+    k_delete_plan<<<1, 1, 0, st>>>(d_cnt, nb_dev, nb_max, record_removed_, removed_cap());
+    const int g = resident_blocks(k_delete_boxes, 256, (long long)v_.leaf_cap * LEAF, n_sm_);
+    k_delete_boxes<<<g, 256, 0, st>>>(v_, boxes, nb_max, 0, d_cnt, record_removed_ ? removed_.as<float4>() : nullptr, removed_cap(),
+                                      &d_cnt[C_DEL_NB], &d_cnt[C_LEAF_USED]);
+    k_delete_account<<<1, 1, 0, st>>>(v_, d_cnt, chain_limit);
+    FL_CHECK(refit_on(st, &d_cnt[C_DELETED]));          // tighten every AABB, when something was deleted
+    k_delete_status<<<1, 1, 0, st>>>(d_cnt, status2);
+    FL_CUDA(cudaGetLastError());
+    return FL_OK;
+}
+
+// Room in the removed-points record by the host's bound (deletes move points from the valid count to the record, device-form
+// inserts since the last settle add at most ub_n_ valid points).  Outside capture, when it might be short, the map settles and
+// the record grows (synchronously).  On a capturing stream such a call is FL_ERR_CAPACITY and captures nothing, as
+// async_prepare does: a graph captured with no record, or too small a one, would refuse every delete until captured again.
+// Replays that fill the record later are refused by the plan.
+int Map::delete_prepare(cudaStream_t st) {
+    if (!record_removed_) return FL_OK;
+    const size_t bound = (size_t)n_removed_ + (size_t)n_valid_ + (size_t)ub_n_;
+    if (bound * sizeof(float4) <= removed_.bytes && removed_.ptr) return FL_OK;
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    FL_CUDA(cudaStreamGetCaptureInfo(st, &cs));
+    if (cs != cudaStreamCaptureStatusNone) {
+        set_last_error("delete_boxes_async: the removed-points record might not hold this delete; call fl_map_maintain (or the call "
+                       "once outside capture) first");
+        return FL_ERR_CAPACITY;
+    }
+    FL_CHECK(settle(false));
+    return removed_room();
+}
+
+int Map::delete_boxes_async_checked(const float* d_boxes, const int* d_nb, int nb_max, int* d_status2, cudaStream_t st) {
+    if (nb_max < 0 || !device_ptr(d_nb, device_, 4) || !device_ptr(d_status2, device_, 4) || (nb_max > 0 && !device_ptr(d_boxes, device_, 4))) {
+        set_last_error("delete_boxes_async: nb_max < 0, or a buffer is not 4-byte aligned device memory on device %d", device_);
+        return FL_ERR_ARG;
+    }
+    FL_CUDA(cudaSetDevice(device_));
+    if (nb_max == 0) {                                  // nothing can be deleted: (FL_OK, 0)
+        bool joined = false;
+        FL_CHECK(query_begin(st, &joined));
+        FL_CUDA(cudaMemsetAsync(d_status2, 0, 2 * sizeof(int), st));
+        return query_end(st, joined);
+    }
+    FL_CHECK(delete_prepare(st));
+    bool joined = false;
+    FL_CHECK(mutation_begin(st, &joined));
+    FL_CHECK(enqueue_delete(d_boxes, d_nb, nb_max, d_status2, st));
+    return mutation_end(st, joined);
+}
+
 // KD_TREE::acquire_removed_points (ikd_Tree.cpp:661-676): the points Delete_Point_Boxes removed since the last call.  Recording
 // starts with the first call (the reference's caller asks before every box delete, laserMapping.cpp:273-275).
 int Map::acquire_removed(float* out_xyzi, int cap, int* n_out) {
@@ -1411,6 +1513,7 @@ int Map::acquire_removed(float* out_xyzi, int cap, int* n_out) {
     if (n_out) *n_out = n;
     if (!record_removed_) {
         record_removed_ = true;
+        layout_dirty_ = true;           // device-form deletes captured before record nothing: capture them again
         FL_CUDA(cudaMemsetAsync(&counters_.as<int>()[C_REMOVED], 0, sizeof(int), stream_));
         return FL_OK;
     }
@@ -1848,6 +1951,7 @@ int Map::settle(bool full, int* layout_changed) {
         FL_CUDA(cudaStreamSynchronize(stream_));
         n_valid_ = h_counters_[C_VALID];
         n_tomb_ = h_counters_[C_TOMBS];
+        if (record_removed_) n_removed_ = h_counters_[C_REMOVED];
         ub_n_ = 0;
         // what is owed survives read-only settles: only a full settle does it and clears it
         due_ = due_ || h_counters_[C_DUE] != 0;
@@ -1872,6 +1976,9 @@ int Map::settle(bool full, int* layout_changed) {
         FL_CHECK(publish_counts());          // C_DUE = 0
         FL_CUDA(cudaStreamSynchronize(stream_));
     }
+    // room in the started removed-points record for the next delete (a device-form delete refused for it, a record started by
+    // fl_map_acquire_removed and not sized yet), as the host form grows it before each delete
+    if (full && record_removed_) FL_CHECK(removed_room());
     if (layout_changed) { *layout_changed = layout_dirty_ ? 1 : 0; layout_dirty_ = false; }
     return FL_OK;
 }

@@ -79,6 +79,13 @@ public:
                          const int* list_counts, int* out, cudaStream_t st);
     // the public fl_map_add_points_async: argument checks, async_prepare, the join, add_points_async
     int add_points_async_checked(const float* d_pts, const int* d_n, int n_max, bool downsample_on, int* d_status2, cudaStream_t st);
+    // Device form of Delete_Point_Boxes (fl_map_delete_boxes_async), with the conventions of the Add_Points forms above.
+    //   delete_prepare: outside capture, room in the removed-points record by the host's bound (the one synchronous case)
+    //   enqueue_delete: up to nb_max boxes (min xyz, max xyz) at `boxes`, count *nb_dev (clamped to [0, nb_max]); a one-thread
+    //     plan checks the record's room first.  status2 = (status, deleted).  Between mutation_begin and mutation_end.
+    int delete_prepare(cudaStream_t st);
+    int enqueue_delete(const float* boxes, const int* nb_dev, int nb_max, int* status2, cudaStream_t st);
+    int delete_boxes_async_checked(const float* d_boxes, const int* d_nb, int nb_max, int* d_status2, cudaStream_t st);
     // Host-form calls settle first.  Read-only ones (full = false) refresh the host's mirror of the device counters (one read-back
     // when a device-form mutation may have run); the others (full = true) also run the re-pack / re-list the device forms deferred,
     // by the host form's rules.  *layout_changed: buffers or leaves moved since the last report (captured graphs are stale).
@@ -92,6 +99,8 @@ public:
     int dir_stats(int* out6) const;
     // recompute every AABB from the valid points (after deletions)
     int refit();
+    // the same launches on `st`; gate (may be null): every kernel returns at once when *gate is 0 on the device
+    int refit_on(cudaStream_t st, const int* gate);
 
     int size() const { return n_valid_ + n_tomb_; }       // KD_TREE::size()  (valid + lazily deleted; settle(false) first)
     int validnum() const { return n_valid_; }             // KD_TREE::validnum()
@@ -130,6 +139,9 @@ private:
     int add_points_host(const float4* d_pts, int n, bool downsample_on, int* added);
     // the host's n_valid_ / n_tomb_ into the device counters the device forms keep (after every host-form mutation)
     int publish_counts();
+    // the removed-points record: room for every valid point on top of what it holds (synchronous), and its capacity in points
+    int removed_room();
+    int removed_cap() const;
     // device forms: one Add_Points of the batch at pts, effective count at counters_[slot], after the plan kernel
     int enqueue_add(const float4* pts, int slot, bool downsample_on, int n_max, cudaStream_t st);
     int enqueue_insert(const float4* pts, const int* n_dev, int n_max, cudaStream_t st);

@@ -1,9 +1,10 @@
 // Scan front end: the steps between the raw LiDAR points and the measurement update, kept in HBM.
 //   sort by offset time + per-point de-skew     ImuProcess::UndistortPcl   src/IMU_Processing.hpp:232-234, 312-346
 //   voxel-grid down-sampling                    pcl::VoxelGrid::filter     src/laserMapping.cpp:904-905
-// and the sliding local-map cube that produces the delete boxes (host arithmetic only)
+// and the sliding local-map cube that produces the delete boxes (on the host, or on the device from the state there)
 //   LocalMapCube                                lasermap_fov_segment()     src/laserMapping.cpp:229-277
 #pragma once
+#include "lie.cuh"
 #include "map.h"
 
 namespace fl {
@@ -59,20 +60,83 @@ private:
     bool dev_used_ = false, dev_uploaded_ = false, dev_undistorted_ = false, dev_down_ = false;
 };
 
-// lasermap_fov_segment() without its globals: LocalMap_Points (:229) and Localmap_Initialized (:230) live here.
+// LocalMap_Points (:229) and Localmap_Initialized (:230)
+struct CubeBox {
+    float lo[3], hi[3];
+    int init;
+};
+// The cube arithmetic of lasermap_fov_segment() (:236-270), shared by the host form and the device form's one-thread kernel.
+// Slides `c` for the LiDAR position pos and returns the number of delete boxes written to boxes6 (<= 3, each min xyz / max xyz)
+// -- cub_needrm.  The arithmetic keeps the reference's types: cube corners are float (BoxPointType, ikd_Tree.h:42-45), the
+// position and cube_len are double, MOV_THRESHOLD (1.5f) and DET_RANGE are float (laserMapping.cpp:77-78).
+FL_HD int cube_slide(CubeBox& c, const double pos[3], double cube_len, float det_range, float* boxes6) {
+    const float margin = 1.5f * det_range;
+    if (!c.init) {                                     // :238-245: first call only centres the cube
+        for (int a = 0; a < 3; a++) {
+            c.lo[a] = float(pos[a] - cube_len / 2.0);
+            c.hi[a] = float(pos[a] + cube_len / 2.0);
+        }
+        c.init = 1;
+        return 0;
+    }
+    int dir[3];                                        // 0: stay, 1: towards the low face, 2: towards the high face
+    bool near_edge = false;
+    for (int a = 0; a < 3; a++) {
+        const float to_lo = float(fabs(pos[a] - double(c.lo[a])));
+        const float to_hi = float(fabs(pos[a] - double(c.hi[a])));
+        dir[a] = to_lo <= margin ? 1 : (to_hi <= margin ? 2 : 0);    // the low face wins (:259-264)
+        near_edge = near_edge || dir[a] != 0;
+    }
+    if (!near_edge) return 0;
+    const double shift = (cube_len - 2.0 * 1.5f * det_range) * 0.5 * 0.9, floor_ = double(det_range * (1.5f - 1));
+    const float step = float(shift < floor_ ? floor_ : shift);        // std::max (:256)
+    int nb = 0;
+    float new_lo[3], new_hi[3];
+    for (int a = 0; a < 3; a++) {
+        new_lo[a] = c.lo[a]; new_hi[a] = c.hi[a];
+        if (dir[a] == 0) continue;
+        float* b = boxes6 + nb * 6;                    // the slab the cube leaves behind, spanning the OLD cube on the other axes
+        for (int k = 0; k < 3; k++) { b[k] = c.lo[k]; b[3 + k] = c.hi[k]; }
+        if (dir[a] == 1) {
+            new_hi[a] = c.hi[a] - step; new_lo[a] = c.lo[a] - step;
+            b[a] = c.hi[a] - step;
+        } else {
+            new_hi[a] = c.hi[a] + step; new_lo[a] = c.lo[a] + step;
+            b[3 + a] = c.lo[a] + step;
+        }
+        nb++;
+    }
+    for (int a = 0; a < 3; a++) { c.lo[a] = new_lo[a]; c.hi[a] = new_hi[a]; }
+    return nb;
+}
+
+// lasermap_fov_segment() without its globals.  The host form slides the cube in host memory; the device form
+// (fl_localmap_segment_device) keeps it in a small buffer on the map's device, allocated by its first call, and from then on that
+// copy is the cube: host-form calls read it back and write it again (synchronously).
 class LocalMapCube {
 public:
     LocalMapCube(double cube_len, float det_range) : cube_len_(cube_len), det_range_(det_range) {}
-    // returns the number of delete boxes written to boxes6 (<= 3, each min xyz / max xyz) -- cub_needrm
-    int slide(const double pos_lid[3], float* boxes6);
-    bool initialized() const { return init_; }
+    ~LocalMapCube();
+    // returns the number of delete boxes written to boxes6 (<= 3) -- cub_needrm
+    int slide(const double pos_lid[3], float* boxes6) { return cube_slide(c_, pos_lid, cube_len_, det_range_, boxes6); }
+    bool initialized() const { return c_.init != 0; }
     void get(float* box6) const;
+
+    // Device form: pos_lid from the state x26 on the device, the cube slid there, then Map::enqueue_delete of its boxes,
+    // all-or-nothing; out3 = (|cub_needrm|, kdtree_delete_counter, status).  The first call (outside capture) allocates the
+    // buffer and uploads the host cube.  Call with the map's lock held.
+    int segment_on_stream(Map* map, const double* d_x26, const int* d_n_scan, float* d_boxes18, int* d_out3, cudaStream_t st);
+    Map* device_map() const { return dmap_; }
+    // the device cube into the host's copy / the host's copy into the device cube (synchronous, on the map's stream)
+    int pull();
+    int push();
 
 private:
     double cube_len_;
     float det_range_;
-    float lo_[3] = {0, 0, 0}, hi_[3] = {0, 0, 0};
-    bool init_ = false;
+    CubeBox c_ = {{0, 0, 0}, {0, 0, 0}, 0};
+    Map* dmap_ = nullptr;
+    DeviceBuffer dev_;              // SegState (scan.cu)
 };
 
 }  // namespace fl

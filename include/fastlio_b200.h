@@ -182,6 +182,24 @@ int fl_map_add_points_device(fl_map_t* m, const float* pts_xyzi_device, int n, i
  * re-list. */
 int fl_map_add_points_async(fl_map_t* m, const float* pts_xyzi_device, const int* n_device, int n_max, int downsample_on,
                             int* status2_device, void* stream);
+/* KD_TREE::Delete_Point_Boxes on the caller's stream                   ikd_Tree.cpp:632-658
+ * boxes6_device: nb_max x (min xyz, max xyz); nb read from *nb_device (clamped to [0, nb_max]) when `stream` reaches the call.
+ * status2_device = (status, deleted): FL_OK, 1 = maintenance due (the points were deleted, and the host form would have re-packed
+ * the leaves here: call fl_map_maintain), FL_ERR_CAPACITY = nothing changed; deleted = the return value of fl_map_delete_boxes (0
+ * on a refusal).  The contract of fl_map_add_points_async: the same joins, capture rules, argument refusals (boxes 4-byte
+ * aligned, may be NULL when nb_max = 0), no host synchronisation, allocation or launch sized from a device value.  The pass over
+ * the slots reads the map's used leaves on the device (inserts replayed since the last settle included), and the AABBs are refit
+ * only when a point was deleted: the launches are the same either way.  After a settle the map is exactly what
+ * fl_map_delete_boxes leaves.  Once fl_map_acquire_removed has started the removed-points record, a one-thread plan checks
+ * before any slot is touched that the record has room for every valid point on top of what it holds (the host form grows it to
+ * that before each delete); without room the call is refused, and fl_map_maintain (which sizes a started record for the next
+ * delete, and reports the layout changed when the record is allocated or moves) makes room.  The host's bound of the room is the
+ * record's count and the valid points at the last settle plus the points of device-form inserts since.  Outside capture, when
+ * that bound says the record might be short, the call first settles the map and grows the record (the one synchronous case);
+ * on a capturing stream it is FL_ERR_CAPACITY with nothing captured (call fl_map_maintain first).  Starting the record
+ * (fl_map_acquire_removed) reports a layout change at the next fl_map_maintain: deletes captured before it do not record. */
+int fl_map_delete_boxes_async(fl_map_t* m, const float* boxes6_device, const int* nb_device, int nb_max, int* status2_device,
+                              void* stream);
 /* Settles the host's view of the map and runs the re-pack / directory re-list that device-form mutations deferred (by the host
  * form's rules), and grows the map for a device-form call it refused (FL_ERR_CAPACITY).  *layout_changed (may be NULL) = 1 when
  * buffers or leaves moved since the last report: graphs captured before must be captured again.  Synchronous.  A status of 1 or a
@@ -311,9 +329,10 @@ int fl_scan_download(fl_scan_t* s, int which, float* out_xyzi, int cap);
 int fl_filter_update_scan(fl_filter_t* f, fl_scan_t* s, double* x26, double* P, double R, double* solve_time_s);
 
 /* ---- device-buffer forms of the scan front end and of the update on it (the conventions of the map's *_device block above)
- * Per scan, upload -> undistort -> voxel_downsample -> fl_filter_update_scan_device -> fl_filter_map_incremental_device run on
- * the caller's stream with every point count in device memory, so one CUDA graph captured with an upper bound n_max replays a
- * whole scan of any size up to it.  esekf::predict and lasermap_fov_segment stay on the host between replays.
+ * Per scan, fl_localmap_segment_device -> upload -> undistort -> voxel_downsample -> fl_filter_update_scan_device ->
+ * fl_filter_map_incremental_device run on the caller's stream with every point count in device memory, so one CUDA graph
+ * captured with an upper bound n_max replays a whole scan of any size up to it.  Only esekf::predict stays on the host between
+ * replays.
  * None of them synchronises the host, allocates, or sizes a launch from a device value: grids follow n_max (the n_max of the
  * last fl_scan_upload_device) and the kernels stop at the device counts.  Host, wrong-device, null or misaligned pointers are
  * FL_ERR_ARG; an n_max or n_pose_max above what fl_scan_reserve sized is FL_ERR_CAPACITY; nothing is enqueued on a refusal.
@@ -373,6 +392,21 @@ int fl_localmap_destroy(fl_localmap_t* l);
  * kdtree_delete_counter in *n_deleted (may be NULL). */
 int fl_localmap_segment(fl_localmap_t* l, fl_map_t* map, const double* pos_lid, float* boxes6_out, int* n_deleted);
 int fl_localmap_get(fl_localmap_t* l, float* box6);   /* LocalMap_Points as (min xyz, max xyz) */
+/* lasermap_fov_segment()                                             laserMapping.cpp:229-277
+ * pos_lid = pos + rot * offset_T_L_I (:890) from x26_device (26 doubles) when `stream` reaches the call; the cube lives on the
+ * map's device.  n_scan_device (may be NULL): when it holds 0 nothing happens (the loop skips an empty scan before the
+ * segment, :892-896).  boxes18_device (may be NULL) receives cub_needrm (3 boxes; those past |cub_needrm| are zero);
+ * out3_device = (|cub_needrm|, kdtree_delete_counter, status) with the statuses of fl_map_delete_boxes_async.  On
+ * FL_ERR_CAPACITY neither the map nor the cube changed (out3[0] and the boxes are what the call would have deleted), so the next
+ * call decides again from the unmoved cube.  The slide uses the arithmetic of fl_localmap_segment, and the delete is that of
+ * fl_map_delete_boxes_async with its conventions, ordering and capture rules; the launches are the same whether or not the cube
+ * moves.  The first call allocates the cube on the map's device and takes over the cube of the host form so far: it must be
+ * made outside capture (FL_ERR_STATE on a capturing stream, nothing captured).  A handle used with a second map is FL_ERR_ARG;
+ * host, wrong-device, null (x26, out3) or misaligned pointers (x26 8-byte, the others 4-byte) are FL_ERR_ARG; nothing is
+ * enqueued on a refusal.  From the first call on, fl_localmap_segment and fl_localmap_get read the device cube back (and the
+ * former writes it again), synchronously: synchronise graph replays before those host-form calls. */
+int fl_localmap_segment_device(fl_localmap_t* l, fl_map_t* map, const double* x26_device, const int* n_scan_device,
+                               float* boxes18_device, int* out3_device, void* stream);
 
 /* ------------------------------------------------------------------ multi-GPU (no reference counterpart)
  * scan points are sharded across ranks, the map is replicated, the 92 normal-equation doubles
