@@ -448,7 +448,8 @@ __device__ void apply_cols(double* mat, const double* J3, const double* J6, cons
 //                   (esekfom.hpp:1651-1699) and, for the reference-form solver, (P/R)^{-1};
 //   solve_finish  : gain, dx_, boxplus, convergence bookkeeping, final covariance
 //                   (esekfom.hpp:1715-1927), from the reduced normal equations in S.red.
-// Both are block-wide (blockDim >= 160).  The scalar manifold work is spread over the first lanes
+// Both are block-wide (blockDim a multiple of 32 and >= 160: solve_finish copies H^T H one
+// entry per thread; gj_eliminate takes any multiple of 32).  The scalar manifold work is spread over the first lanes
 // of different warps so that the FP64 chains (and their instruction fetches) overlap.
 #define STAMP(i) do { if (threadIdx.x == 0) ctl->prof[i] = clock64(); } while (0)
 

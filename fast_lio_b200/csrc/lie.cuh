@@ -162,7 +162,7 @@ FL_HD M33 A_matrix(const D3& v) {
 // ---- S2, S2_typ == 1 (S2.hpp:214-239)
 FL_HD void S2_Bx(const D3& v, double B[6]) {          // 3x2 row-major
     // S2.hpp:214-239 divides every entry by (L + v.x) and by L; here ONE reciprocal each (this runs in the single-warp solver,
-    // where an FP64 division is ~40 dependent instructions) -- the entries differ from the reference's by at most an ulp
+    // where an FP64 division is ~40 dependent instructions) -- the entries stay within 3 ulps of max|B| of the reference's
     const double L = S2_LEN;
     constexpr double invL = 1.0 / S2_LEN;
     if (v.x + L > MTK_TOL) {

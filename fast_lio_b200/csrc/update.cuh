@@ -493,42 +493,6 @@ __device__ void sol_exchange(SolverSm& S, P2PState* p2p) {
     sol_sync();
 }
 
-// Gauss-Jordan with partial pivoting on [A | B], ne rows, one COLUMN per lane, rows in registers.  The pivot row is scaled to a
-// unit pivot as it is chosen, so after the last step the solution row of unknown k is physical row `r` with row_k[r] == k.
-template <int N>
-__device__ __forceinline__ bool gj_cols(double (&c)[N], int* row_k, int lane) {
-    unsigned used = 0;
-    bool ok = true;
-#pragma unroll 1
-    for (int k = 0; k < N; k++) {
-        int p = 0; double best = -1.0;
-#pragma unroll
-        for (int r = 0; r < N; r++) {
-            const double v = fabs(c[r]);
-            const bool cand = !((used >> r) & 1u) && v > best;
-            best = cand ? v : best; p = cand ? r : p;
-        }
-        p = __shfl_sync(FULL, p, k);
-        best = __shfl_sync(FULL, best, k);
-        if (!(best > 0.0)) ok = false;
-        double apj = 0.0;
-#pragma unroll
-        for (int r = 0; r < N; r++) apj = (r == p) ? c[r] : apj;
-        const double inv = 1.0 / __shfl_sync(FULL, apj, k);
-        apj *= inv;                                        // the scaled pivot row, this lane's column
-#pragma unroll
-        for (int r = 0; r < N; r++) {
-            const double ck = __shfl_sync(FULL, c[r], k);
-            if (r == p) c[r] = apj;
-            else if (lane > k) c[r] -= ck * apj;
-        }
-        used |= 1u << p;
-        if (lane == 0) row_k[p] = k;
-    }
-    __syncwarp();
-    return ok;
-}
-
 // The H-dependent half of a pass (esekfom.hpp:1782-1834).  The critical path -- gain, dx_, convergence, [+] on the pose the
 // measurement model reads, publication -- runs in WARP 0 ALONE, with the system in registers and no block barrier; everything
 // else ([+] on velocity / biases / gravity, the log, the covariance bookkeeping and, on the pass that ends the update, the final

@@ -123,9 +123,18 @@ def true_state(lidar: str, step: int = 0) -> np.ndarray:
     return pack_state(pos, rot, off_r, off_t, vel, bg, ba, grav)
 
 
-def make_prior(x_true: np.ndarray, seed: int = 3, pos_sigma=0.05, rot_sigma_deg=0.5, coupling: float = 0.3):
+def make_prior(x_true: np.ndarray, seed: int = 3, pos_sigma=0.05, rot_sigma_deg=0.5, coupling: float = 0.3,
+               rot_err_deg=(0.0, 0.0, 0.0), grav_var: float = 0.0, grav_rot_corr: float = 0.0, grav_deg: float = 0.0,
+               offr_deg: float = 0.0):
     """Prior = truth [+] perturbation (SURVEY.md 8d) and the init_P pattern of
-    src/IMU_Processing.hpp:204-211."""
+    src/IMU_Processing.hpp:204-211.
+
+    Large corrections (all off by default; they draw no random numbers, so the default prior is unchanged):
+      rot_err_deg    adds a (roll, pitch, yaw) error and gives the rotation block a standard deviation of its angle;
+      grav_var       gives the gravity block that variance, grav_rot_corr of it coupled to the rotation block
+                     (gravity tangent = own part + k * rotation error), and grav_deg tilts the prior's gravity;
+      offr_deg       rotates offset_R_L_I by that angle about (1, 1, 1) / sqrt(3), with a matching standard deviation.
+    Each is a congruence P := T P T^T of the covariance above, so P stays symmetric positive definite."""
     rng = np.random.default_rng(seed)
     x = x_true.copy()
     x[0:3] += rng.normal(0.0, pos_sigma, 3)
@@ -148,6 +157,27 @@ def make_prior(x_true: np.ndarray, seed: int = 3, pos_sigma=0.05, rot_sigma_deg=
         Cm = Cm / d[:, None] / d[None, :]
         S = np.sqrt(np.diag(P))
         P = ((1.0 - coupling) * np.eye(23) + coupling * Cm) * S[:, None] * S[None, :]
+        P = 0.5 * (P + P.T)
+    T = np.eye(23)
+    sr = math.radians(float(np.linalg.norm(rot_err_deg)))
+    if sr:
+        x[3:7] = quat_mul(x[3:7], quat_exp(np.radians(np.asarray(rot_err_deg, dtype=np.float64))))
+        T[3:6, 3:6] *= sr / np.sqrt(np.diag(P)[3:6])
+    if offr_deg:
+        x[7:11] = quat_mul(x[7:11], quat_exp(np.full(3, math.radians(offr_deg) / math.sqrt(3.0))))
+        T[6:9, 6:9] *= math.radians(offr_deg) / np.sqrt(np.diag(P)[6:9])
+    if grav_var:
+        k = grav_rot_corr * math.sqrt(grav_var) / (sr or math.radians(rot_sigma_deg))
+        T[21:23, 21:23] *= math.sqrt(grav_var * (1.0 - grav_rot_corr ** 2)) / np.sqrt(np.diag(P)[21:23])
+        T[21, 3:6] = k * T[4, 3:6]               # tangent 0 follows pitch, tangent 1 follows roll
+        T[22, 3:6] = k * T[3, 3:6]
+    if grav_deg:
+        g = x[23:26] / np.linalg.norm(x[23:26])
+        axis = np.cross(g, [1.0, 0.0, 0.0])
+        axis /= np.linalg.norm(axis)
+        x[23:26] = quat_to_mat(quat_exp(axis * math.radians(grav_deg))) @ x[23:26]
+    if not np.array_equal(T, np.eye(23)):
+        P = T @ P @ T.T
         P = 0.5 * (P + P.T)
     return x, np.ascontiguousarray(P)
 

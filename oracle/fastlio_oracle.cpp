@@ -457,6 +457,17 @@ void oracle_state_boxplus(double* x26, const double* d23) { State s = load_state
 void oracle_state_boxminus(const double* a26, const double* b26, double* r23) { state_boxminus(load_state(a26), load_state(b26), r23); }
 int oracle_inverse(const double* A, double* Ainv, int n) { return inverse_lu(A, Ainv, n) ? 0 : -1; }
 void oracle_A_matrix(const double* v3in, double* out9) { M3 a = A_matrix(v3(v3in[0], v3in[1], v3in[2])); memcpy(out9, a.m, sizeof(a.m)); }
+// The MTK pieces one at a time (row-major outputs), for the manifold tests of the device code
+void oracle_so3_exp(const double* v3in, double* q4) { Quat q = so3_exp(v3(v3in[0], v3in[1], v3in[2])); q4[0] = q.x; q4[1] = q.y; q4[2] = q.z; q4[3] = q.w; }
+void oracle_so3_log(const double* q4, double* out3) { V3 l = so3_log(Quat{q4[0], q4[1], q4[2], q4[3]}); for (int i = 0; i < 3; i++) out3[i] = l[i]; }
+void oracle_S2_Bx(const double* v3in, double* out6) { double b[3][2]; S2_Bx(v3(v3in[0], v3in[1], v3in[2]), b); memcpy(out6, b, sizeof(b)); }
+void oracle_S2_boxminus(const double* self_other6, double* out2) {
+    S2_boxminus(v3(self_other6[0], self_other6[1], self_other6[2]), v3(self_other6[3], self_other6[4], self_other6[5]), out2);
+}
+void oracle_S2_Nx_yy(const double* v3in, double* out6) { double n[2][3]; S2_Nx_yy(v3(v3in[0], v3in[1], v3in[2]), n); memcpy(out6, n, sizeof(n)); }
+void oracle_S2_Mx(const double* v3_delta2, double* out6) {
+    double m[3][2]; S2_Mx(v3(v3_delta2[0], v3_delta2[1], v3_delta2[2]), v3_delta2 + 3, m); memcpy(out6, m, sizeof(m));
+}
 void oracle_transform_point(const double* x26, const float* pb, float* pw) {
     State s = load_state(x26);
     V3 p_body = v3(pb[0], pb[1], pb[2]);
