@@ -28,6 +28,23 @@ class PassLog(C.Structure):
                 ("x_after", C.c_double * 26)]
 
 
+def _log_dict(l: PassLog) -> dict:
+    return dict(searched=l.searched, valid=l.valid, effct=l.effct, converged=l.converged,
+                res_sum=l.res_sum, HtH=np.array(l.HtH).reshape(12, 12).copy(),
+                Hth=np.array(l.Hth).copy(), x_after=np.array(l.x_after).copy())
+
+
+def decode_pass_logs(raw, passes: int) -> list:
+    """The first `passes` entries of one hypothesis's log bytes from Esekf.update_batch_device (a (max_iter + 1,
+    sizeof(fl_pass_log_t)) uint8 array or tensor) as the dicts Esekf.pass_logs() returns."""
+    if hasattr(raw, "cpu"):
+        raw = raw.cpu().numpy()
+    buf = np.ascontiguousarray(raw, dtype=np.uint8).reshape(-1, C.sizeof(PassLog))
+    if not 0 <= passes <= len(buf):
+        raise ValueError(f"passes must be in [0, {len(buf)}], got {passes}")
+    return [_log_dict(PassLog.from_buffer_copy(buf[i].tobytes())) for i in range(passes)]
+
+
 class FastLioError(RuntimeError):
     pass
 
@@ -53,6 +70,7 @@ SYMBOLS = [
     "fl_map_add_points_async", "fl_map_maintain", "fl_filter_map_incremental_device",
     "fl_scan_reserve", "fl_scan_upload_device", "fl_scan_undistort_device", "fl_scan_voxel_downsample_device",
     "fl_filter_update_scan_device", "fl_map_delete_boxes_async", "fl_localmap_segment_device",
+    "fl_filter_reserve_batch", "fl_filter_batch_plan", "fl_filter_update_batch_device",
 ]
 
 
@@ -107,6 +125,9 @@ def load():
     L.fl_filter_update_device.argtypes = [_vp, _vp, C.c_int, _vp, _vp, C.c_double, _vp, _vp]
     L.fl_filter_get_nearest_device.argtypes = [_vp, _vp, _vp, C.c_int, _vp]
     L.fl_filter_get_selected_device.argtypes = [_vp, _vp, C.c_int, _vp]
+    L.fl_filter_reserve_batch.argtypes = [_vp, C.c_int]
+    L.fl_filter_batch_plan.argtypes = [_vp, C.c_int, C.c_int, _i32p]
+    L.fl_filter_update_batch_device.argtypes = [_vp, _vp, C.c_int, C.c_int, _vp, _vp, C.c_double, _vp, _vp, _vp]
     L.fl_filter_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int]
     L.fl_filter_destroy.argtypes = [C.c_void_p]
     L.fl_filter_set_params.argtypes = [C.c_void_p, C.c_int, _f64p, C.c_int]
@@ -506,13 +527,7 @@ class Esekf:
     def pass_logs(self):
         logs = (PassLog * 16)()
         n = _check(self._L.fl_filter_get_pass_logs(self.h, logs, 16))
-        out = []
-        for i in range(n):
-            l = logs[i]
-            out.append(dict(searched=l.searched, valid=l.valid, effct=l.effct, converged=l.converged,
-                            res_sum=l.res_sum, HtH=np.array(l.HtH).reshape(12, 12).copy(),
-                            Hth=np.array(l.Hth).copy(), x_after=np.array(l.x_after).copy()))
-        return out
+        return [_log_dict(logs[i]) for i in range(n)]
 
     # ---- device-buffer form: CUDA tensors on the map's device, enqueued on torch.cuda.current_stream()
     def update_device(self, scan, x, P, R: float = 0.001, status=None):
@@ -531,6 +546,38 @@ class Esekf:
         _check(self._L.fl_filter_update_device(self.h, scan.data_ptr() if nq else None, nq, x.data_ptr(), P.data_ptr(), R,
                                                status.data_ptr(), t._stream()))
         return status
+
+    # ---- batched form: one scan from many priors (fl_filter_update_batch_device)
+    def reserve_batch(self, nq_max: int):
+        """fl_filter_reserve_batch: size the batch's own buffers for scans of up to nq_max points (synchronous, grow-only)."""
+        _check(self._L.fl_filter_reserve_batch(self.h, int(nq_max)))
+
+    def batch_plan(self, nq: int, n_hyp: int):
+        """(workers per hypothesis, hypotheses per wave, waves) of a batch of n_hyp priors on an nq-point scan."""
+        out = np.zeros(3, dtype=np.int32)
+        _check(self._L.fl_filter_batch_plan(self.h, int(nq), int(n_hyp), out))
+        return int(out[0]), int(out[1]), int(out[2])
+
+    def update_batch_device(self, scan, x, P, R: float = 0.001, status=None, logs: bool = False):
+        """fl_filter_update_batch_device on the current stream: scan (nq, 4) float32, x (H, 26) and P (H, 23, 23) float64, updated
+        in place per hypothesis (only where it succeeds).  Returns status, an (H, 2) int32 tensor of (FL_OK or FL_ERR_STATE,
+        passes run); with logs=True also the pass logs as an (H, max_iter + 1, sizeof(fl_pass_log_t)) uint8 tensor (entries from
+        `passes` on stay zero; decode_pass_logs reads them).  Nothing synchronises, so the call can be captured into a CUDA graph."""
+        import torch
+        t = self.tree
+        scan = t._tensor(scan, "scan", 4)
+        x = t._tensor(x, "x", 26, torch.float64)
+        H = x.shape[0]
+        P = t._tensor(P, "P", None, torch.float64, (H, 23, 23))
+        if status is None:
+            status = torch.empty((H, 2), dtype=torch.int32, device=x.device)
+        status = t._tensor(status, "status", None, torch.int32, (H, 2))
+        lg = torch.zeros((H, self.max_iter + 1, C.sizeof(PassLog)), dtype=torch.uint8, device=x.device) if logs else None
+        nq = scan.shape[0]
+        _check(self._L.fl_filter_update_batch_device(self.h, scan.data_ptr() if nq else None, nq, H, x.data_ptr() if H else None,
+                                                     P.data_ptr() if H else None, R, status.data_ptr() if H else None,
+                                                     lg.data_ptr() if (logs and H) else None, t._stream()))
+        return (status, lg) if logs else status
 
     def map_incremental_device(self, filter_size_map_min: float = 0.5, flg_EKF_inited: bool = True, out4=None):
         """fl_filter_map_incremental_device on the current stream.  Returns out4, an int32 tensor (4,) = (|PointToAdd|,

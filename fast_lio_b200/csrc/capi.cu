@@ -304,6 +304,20 @@ int fl_filter_update_device(fl_filter_t* f, const float* body_xyzi_device, int n
     FILTER_GUARD(f);
     return f->impl->update_on_stream(body_xyzi_device, nq, x26_device, P_device, R, status2_device, static_cast<cudaStream_t>(stream));
 }
+static_assert(sizeof(fl_pass_log_t) == sizeof(fl::PassLog) && offsetof(fl_pass_log_t, x_after) == offsetof(fl::PassLog, x_after),
+              "fl_pass_log_t is fl::PassLog");
+int fl_filter_reserve_batch(fl_filter_t* f, int nq_max) { FILTER_GUARD(f); return f->impl->reserve_batch(nq_max); }
+int fl_filter_batch_plan(fl_filter_t* f, int nq, int n_hyp, int* out3) {
+    FILTER_GUARD(f);
+    if (!out3) { fl::set_last_error("fl_filter_batch_plan: null out3"); return FL_ERR_ARG; }
+    return f->impl->batch_plan(nq, n_hyp, &out3[0], &out3[1], &out3[2]);
+}
+int fl_filter_update_batch_device(fl_filter_t* f, const float* body_xyzi_device, int nq, int n_hyp, double* x26_device, double* P_device,
+                                  double R, int* status2_device, fl_pass_log_t* logs_device, void* stream) {
+    FILTER_GUARD(f);
+    return f->impl->update_batch_on_stream(body_xyzi_device, nq, n_hyp, x26_device, P_device, R, status2_device,
+                                           reinterpret_cast<fl::PassLog*>(logs_device), static_cast<cudaStream_t>(stream));
+}
 int fl_filter_get_nearest_device(fl_filter_t* f, float* out_pts_device, int* out_cnt_device, int nq, void* stream) {
     FILTER_GUARD(f);
     return f->impl->get_nearest_on_stream(out_pts_device, out_cnt_device, nq, static_cast<cudaStream_t>(stream));

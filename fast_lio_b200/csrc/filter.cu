@@ -1081,10 +1081,9 @@ constexpr int BIND_HOST = 0, BIND_COPY = 1, BIND_SCAN = 2;
 // And it clears `done` in the page-locked mirror, so download_state / get_pass_logs fetch this update's control block instead
 // of trusting a result an earlier host-form update mirrored there.
 // bind (fl_filter_update_device, null otherwise) receives the binding of this update: (nq, BIND_COPY), see Filter::read_binding.
-__global__ void __launch_bounds__(STATE_THREADS) k_state_in(FilterCtl* ctl, unsigned long long* pub, FilterCtl* mirror,
-                                                            const double* __restrict__ x26, const double* __restrict__ P, StateIn s,
-                                                            int* __restrict__ bind, int nq) {
-    pdl_launch();           // k_update may begin launching: its pdl_wait() holds it until this grid is complete and flushed
+// state_in: the control block and the publication block of one update, by the STATE_THREADS threads of one block.
+__device__ __forceinline__ void state_in(FilterCtl* ctl, unsigned long long* pub, const double* __restrict__ x26,
+                                         const double* __restrict__ P, const StateIn& s) {
     const int t = threadIdx.x;
     for (int i = t; i < NDOF * NDOF; i += STATE_THREADS) { const double v = P[i]; ctl->P[i] = v; ctl->P_prop[i] = v; }   // P_propagated = P_
     if (t < XLEN) { const double v = x26[t]; ctl->x[t] = v; ctl->x_prop[t] = v; ctl->x_search[t] = 0.0; }                 // x_propagated = x_
@@ -1096,9 +1095,25 @@ __global__ void __launch_bounds__(STATE_THREADS) k_state_in(FilterCtl* ctl, unsi
         ctl->iter = -1; ctl->t = 0; ctl->converge = 1; ctl->done = 0; ctl->n_pass = 0; ctl->error = 0; ctl->ticket = 0; ctl->gen = 0;
         ctl->max_iter = s.max_iter; ctl->extrinsic_est = s.extrinsic_est; ctl->R = s.R;
         ctl->host_mirror = nullptr;
+    }
+}
+__global__ void __launch_bounds__(STATE_THREADS) k_state_in(FilterCtl* ctl, unsigned long long* pub, FilterCtl* mirror,
+                                                            const double* __restrict__ x26, const double* __restrict__ P, StateIn s,
+                                                            int* __restrict__ bind, int nq) {
+    pdl_launch();           // k_update may begin launching: its pdl_wait() holds it until this grid is complete and flushed
+    state_in(ctl, pub, x26, P, s);
+    if (threadIdx.x == 0) {
         mirror->done = 0;
         if (bind) { bind[0] = nq; bind[1] = BIND_COPY; }
     }
+}
+// fl_filter_update_batch_device: block b sets up slot b of a wave from prior b of x26 / P (the wave's first prior) -- the
+// batch's own control and publication blocks; the filter's page-locked mirror and its binding are not touched.
+__global__ void __launch_bounds__(STATE_THREADS) k_batch_state_in(FilterCtl* ctl, unsigned long long* pub, const double* __restrict__ x26,
+                                                                  const double* __restrict__ P, StateIn s) {
+    pdl_launch();           // as k_state_in: k_update_batch waits in pdl_wait() for this grid
+    const int b = (int)blockIdx.x;
+    state_in(ctl + b, pub + (size_t)b * BATCH_PUB_WORDS, x26 + (size_t)b * XLEN, P + (size_t)b * NDOF * NDOF, s);
 }
 
 // fl_filter_update_scan_device: the scan's count, clamped to [0, n_max], becomes the filter's own (bind[0]), with the binding
@@ -1109,8 +1124,8 @@ __global__ void k_count_in(const int* __restrict__ n, int n_max, int* __restrict
 }
 
 // x26 / P receive the result only when the update succeeded; status2 = (FL_OK or the error download_state reports, passes run)
-__global__ void __launch_bounds__(STATE_THREADS) k_state_out(const FilterCtl* __restrict__ ctl, double* __restrict__ x26,
-                                                             double* __restrict__ P, int* __restrict__ status2) {
+__device__ __forceinline__ void state_out(const FilterCtl* __restrict__ ctl, double* __restrict__ x26, double* __restrict__ P,
+                                          int* __restrict__ status2) {
     const int t = threadIdx.x;
     const int e = ctl->error;
     if (e == 0) {
@@ -1118,6 +1133,16 @@ __global__ void __launch_bounds__(STATE_THREADS) k_state_out(const FilterCtl* __
         if (t < XLEN) x26[t] = ctl->x[t];
     }
     if (t == 0) { status2[0] = e == 0 ? FL_OK : (e == 2 ? FL_ERR_NCCL : FL_ERR_STATE); status2[1] = ctl->n_pass; }
+}
+__global__ void __launch_bounds__(STATE_THREADS) k_state_out(const FilterCtl* __restrict__ ctl, double* __restrict__ x26,
+                                                             double* __restrict__ P, int* __restrict__ status2) {
+    state_out(ctl, x26, P, status2);
+}
+// block b: slot b of a wave into prior b of x26 / P / status2 (the wave's first)
+__global__ void __launch_bounds__(STATE_THREADS) k_batch_state_out(const FilterCtl* __restrict__ ctl, double* __restrict__ x26,
+                                                                   double* __restrict__ P, int* __restrict__ status2) {
+    const int b = (int)blockIdx.x;
+    state_out(ctl + b, x26 + (size_t)b * XLEN, P + (size_t)b * NDOF * NDOF, status2 + 2 * b);
 }
 
 // map_incremental over n_max rows with the count in device memory: rows [*n, n_max) are neither PointToAdd nor PointNoNeedDownsample
@@ -1178,6 +1203,8 @@ Filter::~Filter() {
     partials_.release(); red_.release(); ctl_.release(); ctl0_.release(); logs_.release(); pub_.release();
     mi_world_.release(); mi_flag_add_.release(); mi_flag_no_.release(); mi_list_add_.release(); mi_list_no_.release(); mi_tmp_.release(); mi_counts_.release();
     d_bind_.release();
+    b_body_.release(); b_ctl_.release(); b_pub_.release(); b_partials_.release();
+    b_nearest_.release(); b_nearest_cnt_.release(); b_selected_.release(); b_plane_.release(); b_srange_.release();
     if (h_ctl_) cudaFreeHost(h_ctl_);
     if (ev0_) cudaEventDestroy(ev0_);
     if (ev1_) cudaEventDestroy(ev1_);
@@ -1225,6 +1252,10 @@ int Filter::init() {
     upd_n_capacity_[0][1] = std::min(upd_capacity_[0][1], sms_ * occ);
     FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_n<true, 2>, 2 * UPD_THREADS, 0));
     upd_n_capacity_[1][1] = std::min(upd_capacity_[1][1], sms_ * occ);
+    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_batch<false>, UPD_THREADS, 0));
+    batch_cap_[0] = sms_ * occ;
+    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_batch<true>, UPD_THREADS, 0));
+    batch_cap_[1] = sms_ * occ;
     FL_CHECK(d_bind_.reserve(2 * sizeof(int)));
     FL_CUDA(cudaMemsetAsync(d_bind_.ptr, 0, 2 * sizeof(int), stream()));
     FL_CHECK(partials_.reserve(sizeof(double) * PSTRIDE * (size_t)std::max(upd_capacity_[0][0], upd_capacity_[1][0])));
@@ -1333,10 +1364,10 @@ int Filter::restore_state() {
 }
 
 template <class... KArgs, class... Args>
-static cudaError_t launch_pdl(void (*kernel)(KArgs...), int grid, int block, cudaStream_t st, bool pdl, Args... args) {
+static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, int block, cudaStream_t st, bool pdl, Args... args) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3((unsigned)block); cfg.dynamicSmemBytes = 0; cfg.stream = st;
+    cfg.gridDim = grid; cfg.blockDim = dim3((unsigned)block); cfg.dynamicSmemBytes = 0; cfg.stream = st;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
@@ -1656,6 +1687,112 @@ int Filter::update_scan_on_stream(const float4* d_body, const int* d_n, int n_ma
     FL_CUDA(rc);
     launches_ = 1;
     k_state_out<<<1, STATE_THREADS, 0, st>>>(ctl_.as<FilterCtl>(), d_x26, d_P, d_status2);
+    return map_->query_end(st, joined);
+}
+
+// ----------------------------------------------------------------------------- batched update (fl_filter_update_batch_device)
+// Each hypothesis runs with the single form's workers (launch_update: min(cap - 1, tiles)), so its tiles, partial rows and sums
+// are those of fl_filter_update_device; a wave holds as many hypotheses as fit the co-resident k_update_batch grid.
+int Filter::batch_plan(int nq, int n_hyp, int* workers, int* slots, int* waves) const {
+    if (nq < 0 || n_hyp < 0) { set_last_error("batch_plan: nq and n_hyp must be >= 0"); return FL_ERR_ARG; }
+    const int e = extrinsic_est_ ? 1 : 0;
+    const int w = std::max(0, std::min(upd_capacity_[e][0] - 1, (nq + UPD_THREADS - 1) / UPD_THREADS));
+    if (w + 1 > batch_cap_[e]) {
+        set_last_error("batch_plan: a hypothesis takes %d blocks, %d k_update_batch blocks are co-resident", w + 1, batch_cap_[e]);
+        return FL_ERR_CAPACITY;
+    }
+    const int s = batch_cap_[e] / (w + 1);
+    *workers = w;
+    *slots = s;
+    *waves = (n_hyp + s - 1) / s;
+    return FL_OK;
+}
+
+int Filter::reserve_batch(int nq_max) {
+    if (nq_max < 0) { set_last_error("reserve_batch: nq_max must be >= 0"); return FL_ERR_ARG; }
+    if (nq_max > capacity()) {
+        set_last_error("reserve_batch: %d points exceed the filter's capacity of %d (max_points, or the largest scan so far)", nq_max, capacity());
+        return FL_ERR_CAPACITY;
+    }
+    FL_CUDA(cudaSetDevice(map_->device()));
+    // the largest wave of any nq <= nq_max, under either extrinsic_est_en: slots(workers) * the largest nq with those workers
+    // (a wave has at most cap slots, the zero-point scan's, and at most cap blocks, so at most cap partial rows)
+    size_t rows = 1;
+    int cap = 1;
+    for (int e = 0; e < 2; e++) {
+        const int wmax = std::max(0, std::min(upd_capacity_[e][0] - 1, (nq_max + UPD_THREADS - 1) / UPD_THREADS));
+        for (int w = 0; w <= wmax && w + 1 <= batch_cap_[e]; w++) {
+            const int nq_hi = w == wmax ? nq_max : std::min(nq_max, UPD_THREADS * w);
+            rows = std::max(rows, (size_t)(batch_cap_[e] / (w + 1)) * (size_t)nq_hi);
+        }
+        cap = std::max(cap, batch_cap_[e]);
+    }
+    FL_CHECK(b_body_.reserve(sizeof(float4) * (size_t)std::max(1, nq_max)));
+    FL_CHECK(b_ctl_.reserve(sizeof(FilterCtl) * (size_t)cap));
+    FL_CHECK(b_pub_.reserve(sizeof(unsigned long long) * BATCH_PUB_WORDS * (size_t)cap));
+    FL_CHECK(b_partials_.reserve(sizeof(double) * PSTRIDE * (size_t)cap));
+    FL_CHECK(b_nearest_.reserve(sizeof(float4) * KNN_K * rows));
+    FL_CHECK(b_nearest_cnt_.reserve(sizeof(int) * rows));
+    FL_CHECK(b_selected_.reserve(rows));
+    FL_CHECK(b_plane_.reserve(sizeof(float4) * rows));
+    FL_CHECK(b_srange_.reserve(sizeof(double) * rows));
+    FL_CUDA(cudaMemsetAsync(b_ctl_.ptr, 0, b_ctl_.bytes, stream()));
+    FL_CUDA(cudaMemsetAsync(b_pub_.ptr, 0, b_pub_.bytes, stream()));
+    FL_CUDA(cudaStreamSynchronize(stream()));
+    batch_nq_max_ = std::max(batch_nq_max_, nq_max);
+    return FL_OK;
+}
+
+int Filter::update_batch_on_stream(const float* d_body, int nq, int n_hyp, double* d_x26, double* d_P, double R, int* d_status2,
+                                   PassLog* d_logs, cudaStream_t st) {
+    const int dev = map_->device();
+    if (nq < 0 || n_hyp < 0 || (nq > 0 && !device_ptr(d_body, dev, 16)) ||
+        (n_hyp > 0 && (!device_ptr(d_x26, dev, 8) || !device_ptr(d_P, dev, 8) || !device_ptr(d_status2, dev, 4) ||
+                       (d_logs && !device_ptr(d_logs, dev, 8))))) {
+        set_last_error("update_batch_device: nq or n_hyp < 0, or a buffer is not device memory on device %d (scan 16-byte, x, P and "
+                       "logs 8-byte, status 4-byte aligned)", dev);
+        return FL_ERR_ARG;
+    }
+    FL_CHECK(device_form_scope("update_batch_device", true));
+    if (batch_nq_max_ < 0) { set_last_error("update_batch_device: call fl_filter_reserve_batch first"); return FL_ERR_STATE; }
+    if (nq > batch_nq_max_) {
+        set_last_error("update_batch_device: %d points exceed the %d fl_filter_reserve_batch sized", nq, batch_nq_max_);
+        return FL_ERR_CAPACITY;
+    }
+    int workers = 0, slots = 0, waves = 0;
+    FL_CHECK(batch_plan(nq, n_hyp, &workers, &slots, &waves));
+    if (n_hyp == 0) return FL_OK;
+    FL_CUDA(cudaSetDevice(dev));
+    bool joined = false;
+    FL_CHECK(map_->query_begin(st, &joined));
+    if (nq > 0) FL_CUDA(cudaMemcpyAsync(b_body_.ptr, d_body, sizeof(float4) * (size_t)nq, cudaMemcpyDeviceToDevice, st));
+    ScanView sc;
+    memset(&sc, 0, sizeof(sc));
+    sc.body = b_body_.as<float4>();
+    sc.nearest = b_nearest_.as<float4>(); sc.nearest_cnt = b_nearest_cnt_.as<int>(); sc.selected = b_selected_.as<unsigned char>();
+    sc.plane = b_plane_.as<float4>(); sc.srange = b_srange_.as<double>();
+    sc.q_begin = 0; sc.q_end = sc.Q = nq;
+    StateIn s;
+    for (int i = 0; i < NDOF; i++) s.limit[i] = limit_[i];
+    s.R = R; s.max_iter = max_iter_; s.extrinsic_est = extrinsic_est_;
+    const int log_stride = max_iter_ + 1;
+    FilterCtl* ctl = b_ctl_.as<FilterCtl>();
+    unsigned long long* pub = b_pub_.as<unsigned long long>();
+    for (int w = 0; w < waves; w++) {
+        const int h0 = w * slots, n = std::min(slots, n_hyp - h0);
+        double* x = d_x26 + (size_t)h0 * XLEN;
+        double* P = d_P + (size_t)h0 * NDOF * NDOF;
+        k_batch_state_in<<<n, STATE_THREADS, 0, st>>>(ctl, pub, x, P, s);
+        FL_CUDA(cudaGetLastError());
+        UpdArgs a = upd_args(max_iter_ + 1, 0, 0);    // the map view, the search A/B switch and a fresh nonce, as the single form
+        a.sc = sc; a.ctl = ctl; a.partials = b_partials_.as<double>(); a.pub = pub;
+        a.logs = d_logs ? d_logs + (size_t)h0 * log_stride : nullptr;
+        const dim3 grid((unsigned)(workers + 1), (unsigned)n);
+        FL_CUDA(extrinsic_est_ ? launch_pdl(k_update_batch<true>, grid, UPD_THREADS, st, pdl_, a, log_stride)
+                               : launch_pdl(k_update_batch<false>, grid, UPD_THREADS, st, pdl_, a, log_stride));
+        k_batch_state_out<<<n, STATE_THREADS, 0, st>>>(ctl, x, P, d_status2 + 2 * (size_t)h0);
+        FL_CUDA(cudaGetLastError());
+    }
     return map_->query_end(st, joined);
 }
 

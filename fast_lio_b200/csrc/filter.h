@@ -104,6 +104,16 @@ public:
     int update_scan_on_stream(const float4* d_body, const int* d_n, int n_max, double* d_x26, double* d_P, double R, int* d_status2, cudaStream_t st);
     // the largest scan the per-point buffers hold without growing (max_points at create, or the largest scan since)
     int capacity() const;
+    // One scan from n_hyp priors (fl_filter_update_batch_device), each exactly as update_on_stream would run it, in waves of
+    // `slots` hypotheses per k_update_batch launch.  The batch has buffers of its own (b_*): the scan's copy, per slot a control
+    // block, a publication block and partial rows, and caches of slots x nq rows, so the filter's own state, scan binding and
+    // results stay those of its last single update.  The map's walk counter (fl_map_dir_stats) does count the batch's walks.
+    // reserve_batch sizes them for every nq <= nq_max (grow-only, synchronous; a grow moves them); batch_plan gives the workers
+    // per hypothesis, the slots per wave and the waves for nq points and n_hyp hypotheses.
+    int reserve_batch(int nq_max);
+    int batch_plan(int nq, int n_hyp, int* workers, int* slots, int* waves) const;
+    int update_batch_on_stream(const float* d_body, int nq, int n_hyp, double* d_x26, double* d_P, double R, int* d_status2,
+                               PassLog* d_logs, cudaStream_t st);
 
     // map_incremental (laserMapping.cpp:427-474) on the device: classify every scan point with the final
     // state and its cached neighbours, then Add_Points(PointToAdd, true) + Add_Points(PointNoNeedDownsample, false)
@@ -184,6 +194,9 @@ private:
     DeviceBuffer d_bind_;
     int upd_n_capacity_[2][2] = {{0, 0}, {0, 0}};   // co-resident k_update_n blocks, capped at k_update's (the same tiles per block)
     int read_binding();
+    int batch_cap_[2] = {0, 0};        // co-resident k_update_batch<EXTR> blocks on this device
+    int batch_nq_max_ = -1;            // the nq_max reserve_batch sized the batch buffers for (-1: not yet)
+    DeviceBuffer b_body_, b_ctl_, b_pub_, b_partials_, b_nearest_, b_nearest_cnt_, b_selected_, b_plane_, b_srange_;
     int launches_ = 0;
     long long host_ns_[4] = {0, 0, 0, 0};
     bool shard_set_ = false;

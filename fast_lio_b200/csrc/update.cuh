@@ -827,4 +827,29 @@ __global__ void __launch_bounds__(UPD_THREADS * PAIR, 3 - PAIR) k_update_n(UpdAr
     update_body<EXTR, PAIR>(a, min(*n, a.sc.q_end));
 }
 
+// fl_filter_update_batch_device: one scan from gridDim.y priors in one launch.  Slot blockIdx.y is a whole k_update<EXTR, 1> grid
+// of its own -- blockIdx.x and gridDim.x mean what they mean there, so the slot has the solver block, the workers, the tiles and
+// the fixed-order sums of the single form -- with its own control block, publication block, partial rows, pass logs and
+// per-point caches; the map and the scan are shared.  The slot's caches are rows [s Q, (s + 1) Q) of flat arrays, its partial
+// rows start at s (gridDim.x - 1), its publication block is BATCH_PUB_WORDS words, its log entries start at s log_stride.
+// Footprint: the registers (128) and shared memory of k_update<EXTR, 1>, so the same co-resident grid; the slot's pointers are
+// values here rather than kernel parameters, so ptxas spills a little more (sm_90a, nvcc 12.9: stack 336 / 392 bytes against
+// 288 for EXTR false / true, spill stores + loads 508 / 716 bytes against 352 / 496).
+constexpr int BATCH_PUB_WORDS = 32;      // 256 bytes per slot
+template <bool EXTR>
+__global__ void __launch_bounds__(UPD_THREADS, 2) k_update_batch(UpdArgs a, int log_stride) {
+    const int s = (int)blockIdx.y;
+    const size_t rows = (size_t)s * (size_t)a.sc.Q;
+    a.ctl += s;
+    a.partials += (size_t)s * (gridDim.x - 1) * PSTRIDE;
+    a.pub += (size_t)s * BATCH_PUB_WORDS;
+    if (a.logs) a.logs += (size_t)s * log_stride;
+    a.sc.nearest += rows * KNN_K;
+    a.sc.nearest_cnt += rows;
+    a.sc.selected += rows;
+    a.sc.plane += rows;
+    a.sc.srange += rows;
+    update_body<EXTR, 1>(a, a.sc.q_end);
+}
+
 }  // namespace fl

@@ -306,6 +306,33 @@ int fl_filter_get_selected_device(fl_filter_t* f, unsigned char* out_device, int
  * filter is FL_ERR_STATE and a null, host or misaligned out4 FL_ERR_ARG, with nothing enqueued. */
 int fl_filter_map_incremental_device(fl_filter_t* f, double filter_size_map_min, int flg_EKF_inited, int* out4_device, void* stream);
 
+/* ---- batched form of the update: one scan from many priors (relocalisation, multi-hypothesis evaluation)
+ * esekf::update_iterated_dyn_share_modified run from n_hyp priors     esekfom.hpp:1619-1931, laserMapping.cpp:638-754
+ * Hypothesis h receives exactly the x, P, status pair and pass logs [0, passes) that fl_filter_update_device gives for the prior
+ * (x26_device[h], P_device[h]) on the same map, scan, R and parameters; log entries from `passes` on are not written, and, as in
+ * fl_filter_get_pass_logs, an entry of a pass without effective points leaves HtH and Hth as they were.  x26_device is
+ * [n_hyp][26], P_device [n_hyp][23 * 23], status2_device [n_hyp][2], logs_device (may be NULL) [n_hyp][max_iter + 1].
+ * The hypotheses run in waves: one launch holds `hypotheses per wave` of them, each with the workers of the single form, and a
+ * wave lasts as long as its slowest hypothesis.  fl_filter_batch_plan writes out3 = (workers per hypothesis, hypotheses per
+ * wave, waves) for nq points and n_hyp hypotheses (FL_ERR_CAPACITY if one hypothesis does not fit the co-resident grid).
+ * The batch uses buffers of its own: afterwards fl_filter_get_nearest / get_selected / get_pass_logs / download_state,
+ * map_incremental (both forms) and the *_device getters return what they returned before it.  fl_map_dir_stats does count its
+ * BVH walks.  There is no per-hypothesis Nearest_Points / point_selected_surf.
+ * fl_filter_reserve_batch sizes those buffers for every nq <= nq_max (a few MB); nq_max above the filter's capacity is
+ * FL_ERR_CAPACITY.  Synchronous and grow-only, like fl_scan_reserve; a grow moves the buffers, so capture graphs of the batch
+ * again after it.
+ * The conventions, ordering and capture rules of fl_filter_update_device: the scan is copied on `stream`, so the caller may free
+ * it once `stream` has passed the call; no host synchronisation, allocation or launch sized from a device value.  n_hyp = 0
+ * returns FL_OK and enqueues nothing.  FL_ERR_ARG: nq or n_hyp < 0; a host, wrong-device, null or misaligned pointer (scan 16
+ * bytes, x and P 8, status 4, logs 8; the scan may be null when nq = 0, the outputs when n_hyp = 0).  FL_ERR_STATE: no
+ * fl_filter_reserve_batch yet, or a sharded, solver-0 or fused-0 filter.  FL_ERR_CAPACITY: nq above the reserved nq_max.
+ * Nothing is enqueued on a refusal.  A filter runs one batch at a time: order batch calls on one filter on one stream (or
+ * join their streams). */
+int fl_filter_reserve_batch(fl_filter_t* f, int nq_max);
+int fl_filter_batch_plan(fl_filter_t* f, int nq, int n_hyp, int* out3);
+int fl_filter_update_batch_device(fl_filter_t* f, const float* body_xyzi_device, int nq, int n_hyp, double* x26_device,
+                                  double* P_device, double R, int* status2_device, fl_pass_log_t* logs_device, void* stream);
+
 /* ------------------------------------------------------------------ scan front end (SURVEY.md §8f rows 3-4)
  * The two steps that produce feats_down_body, kept in HBM on the map's device and stream so that a scan goes
  * raw -> de-skewed -> down-sampled -> update -> map_incremental with one upload. */
