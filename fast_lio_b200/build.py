@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libfastlio_b200.so")
 SOURCES = ["map.cu", "filter.cu", "scan.cu", "capi.cu"]
-HEADERS = ["common.cuh", "map.cuh", "map.h", "lie.cuh", "filter.h", "scan.h", "gj.cuh", "update.cuh", os.path.join("..", "..", "include", "fastlio_b200.h")]
+HEADERS = ["common.cuh", "map.cuh", "map.h", "lie.cuh", "filter.h", "scan.h", "gj.cuh", "measure.cuh", "update.cuh", os.path.join("..", "..", "include", "fastlio_b200.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -22,6 +22,7 @@
 
 #include "filter.h"
 #include "gj.cuh"
+#include "measure.cuh"
 
 namespace fl {
 
@@ -40,191 +41,6 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 __device__ __forceinline__ void pdl_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
 __device__ __forceinline__ int tri12(int a, int b) { return a * 12 - (a * (a - 1)) / 2 + (b - a); }   // a <= b
-
-// ============================================================================= esti_plane
-// float32 least squares A n = -1 on the 5 neighbours, column-pivoted Householder QR -- the
-// algorithm the reference gets from Eigen (common_lib.h:241, colPivHouseholderQr().solve) --
-// followed by the reference's normalisation and 0.1 m point-to-plane check (common_lib.h:243-256).
-__device__ __forceinline__ bool esti_plane_dev(float pabcd[4], const float (&pt)[KNN_K][3], float threshold) {
-    constexpr int rows = KNN_K, cols = 3, size = 3;
-    float qr[rows][cols];
-    float c[rows];
-#pragma unroll
-    for (int j = 0; j < rows; j++) { qr[j][0] = pt[j][0]; qr[j][1] = pt[j][1]; qr[j][2] = pt[j][2]; c[j] = -1.0f; }
-    float hc[size];
-    int transp[size];
-    float nu[cols], nd[cols];
-#pragma unroll
-    for (int k = 0; k < cols; k++) {
-        float s = 0.f;
-#pragma unroll
-        for (int i = 0; i < rows; i++) s += qr[i][k] * qr[i][k];
-        nd[k] = sqrtf(s); nu[k] = nd[k];
-    }
-    const float eps = 1.1920929e-07f;
-    const float maxn = fmaxf(nu[0], fmaxf(nu[1], nu[2]));
-    const float threshold_helper = (maxn * eps) * (maxn * eps) / float(rows);
-    const float norm_downdate_threshold = sqrtf(eps);
-    int nonzero_pivots = size;
-#pragma unroll
-    for (int k = 0; k < size; k++) {
-        int biggest = k; float bn = nu[k];
-#pragma unroll
-        for (int j = k + 1; j < cols; j++) if (nu[j] > bn) { bn = nu[j]; biggest = j; }
-        if (nonzero_pivots == size && bn * bn < threshold_helper * float(rows - k)) nonzero_pivots = k;
-        transp[k] = biggest;
-        if (k != biggest) {
-#pragma unroll
-            for (int j = k + 1; j < cols; j++) {
-                if (j == biggest) {
-#pragma unroll
-                    for (int i = 0; i < rows; i++) { float t = qr[i][k]; qr[i][k] = qr[i][j]; qr[i][j] = t; }
-                    float t = nu[k]; nu[k] = nu[j]; nu[j] = t;
-                    t = nd[k]; nd[k] = nd[j]; nd[j] = t;
-                }
-            }
-        }
-        float tailSq = 0.f;
-#pragma unroll
-        for (int i = k + 1; i < rows; i++) tailSq += qr[i][k] * qr[i][k];
-        const float c0 = qr[k][k];
-        float tau, beta;
-        if (tailSq <= 1.17549435e-38f) {
-            tau = 0.f; beta = c0;
-#pragma unroll
-            for (int i = k + 1; i < rows; i++) qr[i][k] = 0.f;
-        } else {
-            beta = sqrtf(c0 * c0 + tailSq);
-            if (c0 >= 0.f) beta = -beta;
-#pragma unroll
-            for (int i = k + 1; i < rows; i++) qr[i][k] = qr[i][k] / (c0 - beta);
-            tau = (beta - c0) / beta;
-        }
-        hc[k] = tau;
-        qr[k][k] = beta;
-        if (tau != 0.f) {
-#pragma unroll
-            for (int j = k + 1; j < cols; j++) {
-                float tmp = 0.f;
-#pragma unroll
-                for (int i = k + 1; i < rows; i++) tmp += qr[i][k] * qr[i][j];
-                tmp += qr[k][j];
-                qr[k][j] -= tau * tmp;
-#pragma unroll
-                for (int i = k + 1; i < rows; i++) qr[i][j] -= tau * qr[i][k] * tmp;
-            }
-        }
-#pragma unroll
-        for (int j = k + 1; j < cols; j++) {
-            if (nu[j] != 0.f) {
-                float temp = fabsf(qr[k][j]) / nu[j];
-                temp = (1.f + temp) * (1.f - temp);
-                temp = temp < 0.f ? 0.f : temp;
-                const float r = nu[j] / nd[j];
-                const float temp2 = temp * r * r;
-                if (temp2 <= norm_downdate_threshold) {
-                    float s = 0.f;
-#pragma unroll
-                    for (int i = k + 1; i < rows; i++) s += qr[i][j] * qr[i][j];
-                    nd[j] = sqrtf(s); nu[j] = nd[j];
-                } else {
-                    nu[j] *= sqrtf(temp);
-                }
-            }
-        }
-    }
-#pragma unroll
-    for (int k = 0; k < size; k++) {
-        if (k < nonzero_pivots) {
-            const float tau = hc[k];
-            if (tau != 0.f) {
-                float tmp = 0.f;
-#pragma unroll
-                for (int i = k + 1; i < rows; i++) tmp += qr[i][k] * c[i];
-                tmp += c[k];
-                c[k] -= tau * tmp;
-#pragma unroll
-                for (int i = k + 1; i < rows; i++) c[i] -= tau * qr[i][k] * tmp;
-            }
-        }
-    }
-#pragma unroll
-    for (int i = size - 1; i >= 0; i--) {
-        if (i < nonzero_pivots) {
-            float s = c[i];
-#pragma unroll
-            for (int j = i + 1; j < size; j++) if (j < nonzero_pivots) s -= qr[i][j] * c[j];
-            c[i] = s / qr[i][i];
-        }
-    }
-    int perm[3] = {0, 1, 2};
-#pragma unroll
-    for (int k = 0; k < size; k++) {
-        // swap(perm[k], perm[transp[k]]) with static indexing
-#pragma unroll
-        for (int j = 0; j < size; j++) if (j == transp[k] && j != k) { int t = perm[k]; perm[k] = perm[j]; perm[j] = t; }
-    }
-    float x[3] = {0.f, 0.f, 0.f};
-#pragma unroll
-    for (int i = 0; i < size; i++) {
-        if (i < nonzero_pivots) {
-#pragma unroll
-            for (int j = 0; j < 3; j++) if (perm[i] == j) x[j] = c[i];
-        }
-    }
-    const float n = sqrtf(x[0] * x[0] + x[1] * x[1] + x[2] * x[2]);
-    pabcd[0] = x[0] / n; pabcd[1] = x[1] / n; pabcd[2] = x[2] / n;
-    pabcd[3] = (float)(1.0 / (double)n);
-    bool ok = true;
-#pragma unroll
-    for (int j = 0; j < rows; j++)
-        if (fabsf(pabcd[0] * pt[j][0] + pabcd[1] * pt[j][1] + pabcd[2] * pt[j][2] + pabcd[3]) > threshold) ok = false;
-    return ok;
-}
-
-// ============================================================================= measurement model
-struct PoseS {            // the part of the state h_share_model reads
-    Q4 rot, offR; D3 pos, offT;
-};
-__device__ __forceinline__ PoseS load_pose(const double* x) {
-    PoseS p; p.rot = ldq(x + X_ROT); p.offR = ldq(x + X_OFFR); p.pos = ld3(x + X_POS); p.offT = ld3(x + X_OFFT);
-    return p;
-}
-// laserMapping.cpp:656-661
-__device__ __forceinline__ void body_to_world(const PoseS& s, const float4& pb, float& wx, float& wy, float& wz) {
-    D3 p_body = d3(pb.x, pb.y, pb.z);
-    D3 g = qrot(s.rot, qrot(s.offR, p_body) + s.offT) + s.pos;
-    wx = (float)g.x; wy = (float)g.y; wz = (float)g.z;
-}
-// laserMapping.cpp:723-751: one row of h_x (12 wide) and the entry of h
-template <bool EXTR>
-__device__ __forceinline__ void jacobian_row(const PoseS& s, const float4& pb, const float4& nv, double* h, double& z) {
-    D3 p_be = d3(pb.x, pb.y, pb.z);
-    D3 p_this = qrot(s.offR, p_be) + s.offT;
-    D3 n = d3(nv.x, nv.y, nv.z);
-    D3 C = qrot(qconj(s.rot), n);
-    D3 A = mul33v(hat3(p_this), C);
-    h[0] = n.x; h[1] = n.y; h[2] = n.z; h[3] = A.x; h[4] = A.y; h[5] = A.z;
-    if (EXTR) {
-        D3 B = mul33v(mul33(hat3(p_be), qmat(qconj(s.offR))), C);
-        h[6] = B.x; h[7] = B.y; h[8] = B.z; h[9] = C.x; h[10] = C.y; h[11] = C.z;
-    }
-    z = -(double)nv.w;
-}
-
-// the same with p_this = R_LI p_b + t_LI already at hand (body_to_world computes it on the way)
-template <bool EXTR>
-__device__ __forceinline__ void jacobian_row_at(const PoseS& s, const float4& pb, const D3& p_this, const float4& nv, double* h, double& z) {
-    D3 n = d3(nv.x, nv.y, nv.z);
-    D3 C = qrot(qconj(s.rot), n);
-    D3 A = mul33v(hat3(p_this), C);
-    h[0] = n.x; h[1] = n.y; h[2] = n.z; h[3] = A.x; h[4] = A.y; h[5] = A.z;
-    if (EXTR) {
-        D3 B = mul33v(mul33(hat3(d3(pb.x, pb.y, pb.z)), qmat(qconj(s.offR))), C);
-        h[6] = B.x; h[7] = B.y; h[8] = B.z; h[9] = C.x; h[10] = C.y; h[11] = C.z;
-    }
-    z = -(double)nv.w;
-}
 
 // Per-point part of h_share_model after the search (laserMapping.cpp:674-692).
 // Returns true when the point contributes a row.
@@ -249,10 +65,9 @@ __device__ __forceinline__ bool measure_point(const ScanView& sc, int q, const P
         const float4 pl = sc.plane[q];
         pabcd[0] = pl.x; pabcd[1] = pl.y; pabcd[2] = pl.z; pabcd[3] = pl.w;
     }
-    const float pd2 = pabcd[0] * wx + pabcd[1] * wy + pabcd[2] * wz + pabcd[3];          // :680
-    const D3 p_body = d3(pb.x, pb.y, pb.z);
-    const float score = (float)(1 - 0.9 * fabs((double)pd2) / sqrt(norm3(p_body)));     // :681 (T8)
-    if (!((double)score > 0.9)) return false;                            // :683
+    const float pd2 = plane_residual(pabcd, wx, wy, wz);                 // :680
+    float score;
+    if (!score_gate(pd2, sqrt(norm3(d3(pb.x, pb.y, pb.z))), score)) return false;    // :681-683
     sc.selected[q] = 1;
     const float4 nv = make_float4(pabcd[0], pabcd[1], pabcd[2], pd2);
     sc.normvec[q] = nv;
@@ -340,7 +155,7 @@ __device__ __forceinline__ void search_point(const MapView& m, const ScanView& s
     if (lane < KNN_K) sc.nearest[(size_t)q * KNN_K + lane] = p;
     if (lane == KNN_K - 1) {
         sc.nearest_cnt[q] = cnt;
-        sc.selected[q] = (cnt < KNN_K) ? 0 : (kb.d > 5.0f ? 0 : 1);          // laserMapping.cpp:671
+        sc.selected[q] = knn_gate(cnt, kb.d) ? 1 : 0;                         // laserMapping.cpp:671
     }
 }
 
@@ -828,7 +643,7 @@ __global__ void __maxnreg__(96) k_search_c(MapView m, ScanView sc, const FilterC
 #pragma unroll
     for (int j = 0; j < KNN_K; j++) sc.nearest[(size_t)q * KNN_K + j] = p[j];
     sc.nearest_cnt[q] = cnt;
-    sc.selected[q] = (cnt < KNN_K) ? 0 : (kb.d[KNN_K - 1] > 5.0f ? 0 : 1);          // laserMapping.cpp:671
+    sc.selected[q] = knn_gate(cnt, kb.d[KNN_K - 1]) ? 1 : 0;                         // laserMapping.cpp:671
 }
 
 // k_residual -- everything of h_share_model after the search (laserMapping.cpp:674-752), one

@@ -278,9 +278,7 @@ __device__ __forceinline__ bool measure_fused(const MapView& m, const ScanView& 
     D3 p_this = d3(0.0, 0.0, 0.0);
     if (active) {
         pb = __ldg(&sc.body[q]);
-        p_this = qrot(s.offR, d3(pb.x, pb.y, pb.z)) + s.offT;               // :656-661 (also the lever arm of the Jacobian, :733)
-        const D3 g = qrot(s.rot, p_this) + s.pos;
-        wx = (float)g.x; wy = (float)g.y; wz = (float)g.z;
+        p_this = body_to_world(s, pb, wx, wy, wz);                          // :656-661 (also the lever arm of the Jacobian, :733)
     }
     bool sel = false;
     float pabcd[4] = {0.f, 0.f, 0.f, 0.f};
@@ -298,7 +296,7 @@ __device__ __forceinline__ bool measure_fused(const MapView& m, const ScanView& 
 #pragma unroll
             for (int j = 0; j < KNN_K; j++) sc.nearest[(size_t)q * KNN_K + j] = p[j];
             sc.nearest_cnt[q] = cnt;
-            sel = cnt >= KNN_K && !(kb.d[KNN_K - 1] > 5.0f);                // :671
+            sel = knn_gate(cnt, kb.d[KNN_K - 1]);                           // :671
             if (search_only) { sc.selected[q] = sel ? 1 : 0; return false; }
             if (sel) {
                 float pn[KNN_K][3];
@@ -316,13 +314,13 @@ __device__ __forceinline__ bool measure_fused(const MapView& m, const ScanView& 
     }
     bool contrib = false;
     if (active && sel) {
-        const float pd2 = pabcd[0] * wx + pabcd[1] * wy + pabcd[2] * wz + pabcd[3];             // :680
+        const float pd2 = plane_residual(pabcd, wx, wy, wz);                                    // :680
         // sqrt(p_body.norm()) depends on the point alone: computed on the searching passes, cached for the others
         double srange;
         if (searched) { srange = sqrt(norm3(d3(pb.x, pb.y, pb.z))); sc.srange[q] = srange; }
         else srange = sc.srange[q];
-        const float score = (float)(1 - 0.9 * fabs((double)pd2) / srange);                     // :681 (T8)
-        if ((double)score > 0.9) {                                                              // :683
+        float score;
+        if (score_gate(pd2, srange, score)) {                                                   // :681-683
             contrib = true;
             absres = fabsf(pd2);                                                                // res_last
             jacobian_row_at<EXTR>(s, pb, p_this, make_float4(pabcd[0], pabcd[1], pabcd[2], pd2), h, z);    // :723-751

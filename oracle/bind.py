@@ -59,6 +59,10 @@ def lib():
         assert L.oracle_pass_log_size() == C.sizeof(PassLog)
         L.oracle_esti_plane.argtypes = [_f32p, C.c_float, _f32p]
         L.oracle_esti_plane.restype = C.c_int
+        L.oracle_esti_plane_trace.argtypes = [_f32p, C.c_float, _f32p, _i32p]
+        L.oracle_esti_plane_trace.restype = C.c_int
+        L.oracle_measure_point.argtypes = [_f64p, _f32p, _f32p, C.c_int, C.c_float, C.c_int, _f64p]
+        L.oracle_measure_point.restype = None
         L.oracle_state_boxplus.argtypes = [_f64p, _f64p]
         L.oracle_state_boxminus.argtypes = [_f64p, _f64p, _f64p]
         L.oracle_inverse.argtypes = [_f64p, _f64p, C.c_int]
@@ -218,6 +222,25 @@ def esti_plane(pts5x3, threshold=0.1):
     out = np.zeros(4, dtype=np.float32)
     ok = lib().oracle_esti_plane(np.ascontiguousarray(pts5x3, dtype=np.float32).reshape(-1), threshold, out)
     return bool(ok), out
+
+
+def esti_plane_trace(pts5x3, threshold=0.1):
+    """esti_plane plus the branches it took: (ok, pabcd, trace) with trace = dict(nonzero_pivots, transp (3),
+    tiny_tail (3), norm (3x3): 0 not visited, 1 downdated, 2 recomputed, 3 skipped as a zero column)."""
+    out = np.zeros(4, dtype=np.float32)
+    tr = np.zeros(16, dtype=np.int32)
+    ok = lib().oracle_esti_plane_trace(np.ascontiguousarray(pts5x3, dtype=np.float32).reshape(-1), threshold, out, tr)
+    return bool(ok), out, dict(nonzero_pivots=int(tr[0]), transp=tr[1:4].copy(), tiny_tail=tr[4:7].copy(), norm=tr[7:16].reshape(3, 3).copy())
+
+
+def measure_point(x26, pb3, near5x3, cnt, d2_last, extrinsic_est_en):
+    """One point of h_share_model with every stage evaluated: 25 doubles = world point (3), kNN gate, plane ok,
+    score gate, pabcd (4), pd2, score, row (12), h."""
+    out = np.zeros(25)
+    lib().oracle_measure_point(np.ascontiguousarray(x26, dtype=np.float64), np.ascontiguousarray(pb3, dtype=np.float32).reshape(-1),
+                               np.ascontiguousarray(near5x3, dtype=np.float32).reshape(-1), int(cnt), float(d2_last),
+                               int(extrinsic_est_en), out)
+    return out
 
 
 class LocalMap:

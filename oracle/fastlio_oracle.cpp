@@ -314,7 +314,12 @@ static bool inverse_lu(const double* A, double* Ainv, int n) {
 // float 5x3 least squares A x = -1 via Eigen 3.3 ColPivHouseholderQR
 // (Eigen/src/QR/ColPivHouseholderQR.h computeInPlace + _solve_impl,
 //  Eigen/src/Householder/Householder.h makeHouseholder / applyHouseholderOnTheLeft).
-static bool esti_plane_f(float pca_result[4], const float pts[NUM_MATCH_POINTS][3], float threshold) {
+// Branches taken, for the tests: transp, nonzero_pivots, tiny_tail[k] (makeHouseholder's tailSq <= min branch) and
+// norm[k][j] for j > k: 0 not visited (j <= k), 1 downdated, 2 recomputed, 3 skipped (normsUpdated[j] == 0).
+struct PlaneTrace { int nonzero_pivots; int transp[3]; int tiny_tail[3]; int norm[3][3]; };
+
+static bool esti_plane_f(float pca_result[4], const float pts[NUM_MATCH_POINTS][3], float threshold, PlaneTrace* trace = nullptr) {
+    if (trace) memset(trace, 0, sizeof(*trace));
     const int rows = NUM_MATCH_POINTS, cols = 3, size = 3;
     float qr[5][3];
     float c[5];
@@ -348,6 +353,7 @@ static bool esti_plane_f(float pca_result[4], const float pts[NUM_MATCH_POINTS][
         float c0 = qr[k][k];
         float tau, beta;
         const float tol = (std::numeric_limits<float>::min)();
+        if (trace) trace->tiny_tail[k] = tailSq <= tol;
         if (tailSq <= tol) {
             tau = 0.f; beta = c0;
             for (int i = k+1; i < rows; i++) qr[i][k] = 0.f;
@@ -372,12 +378,14 @@ static bool esti_plane_f(float pca_result[4], const float pts[NUM_MATCH_POINTS][
         }
         // column-norm downdate (LAPACK working note 176 style, as in Eigen 3.3)
         for (int j = k+1; j < cols; j++) {
+            if (trace) trace->norm[k][j] = 3;
             if (normsUpdated[j] != 0.f) {
                 float temp = std::fabs(qr[k][j]) / normsUpdated[j];
                 temp = (1.f + temp) * (1.f - temp);
                 temp = temp < 0.f ? 0.f : temp;
                 float r = normsUpdated[j] / normsDirect[j];
                 float temp2 = temp * r * r;
+                if (trace) trace->norm[k][j] = temp2 <= norm_downdate_threshold ? 2 : 1;
                 if (temp2 <= norm_downdate_threshold) {
                     float s = 0.f; for (int i = k+1; i < rows; i++) s += qr[i][j] * qr[i][j];
                     normsDirect[j] = std::sqrt(s);
@@ -388,6 +396,7 @@ static bool esti_plane_f(float pca_result[4], const float pts[NUM_MATCH_POINTS][
             }
         }
     }
+    if (trace) { trace->nonzero_pivots = nonzero_pivots; for (int k = 0; k < 3; k++) trace->transp[k] = transp[k]; }
     // _solve_impl: c = Q^T b (first nonzero_pivots reflectors), back-substitute, un-permute
     for (int k = 0; k < nonzero_pivots; k++) {
         float tau = hCoeffs[k];
@@ -423,6 +432,44 @@ static bool esti_plane_f(float pca_result[4], const float pts[NUM_MATCH_POINTS][
     return true;
 }
 
+// laserMapping.cpp:656-661
+inline V3 body_to_world(const State& s, const float* pb, float pw[3]) {
+    V3 p_global = add(qrot(s.rot, add(qrot(s.offR, v3(pb[0], pb[1], pb[2])), s.offT)), s.pos);
+    pw[0] = float(p_global[0]); pw[1] = float(p_global[1]); pw[2] = float(p_global[2]);
+    return p_global;
+}
+
+// laserMapping.cpp:671
+inline bool knn_gate(int cnt, float d2_last) { return cnt < NUM_MATCH_POINTS ? false : (d2_last > 5 ? false : true); }
+
+// laserMapping.cpp:680-681: returns the score; pd2 out
+inline float plane_score(const float pabcd[4], const float pw[3], const float* pb, float& pd2) {
+    V3 p_body = v3(pb[0], pb[1], pb[2]);
+    pd2 = pabcd[0] * pw[0] + pabcd[1] * pw[1] + pabcd[2] * pw[2] + pabcd[3];          // :680
+    return float(1 - 0.9 * std::fabs(pd2) / std::sqrt(norm(p_body)));                // :681 (T8)
+}
+
+// laserMapping.cpp:723-751: one row of h_x and its entry of h, from normvec = (n, pd2)
+inline void jacobian_row(const State& s, const float* pb, const float* nv, int extrinsic_est_en, double* row, double& h) {
+    V3 point_this_be = v3(pb[0], pb[1], pb[2]);
+    M3 point_be_crossmat = hat(point_this_be);
+    V3 point_this = add(qrot(s.offR, point_this_be), s.offT);
+    M3 point_crossmat = hat(point_this);
+    V3 norm_vec = v3(nv[0], nv[1], nv[2]);
+    V3 C = qrot(qconj(s.rot), norm_vec);
+    V3 A = mul(point_crossmat, C);
+    row[0] = norm_vec[0]; row[1] = norm_vec[1]; row[2] = norm_vec[2];
+    row[3] = A[0]; row[4] = A[1]; row[5] = A[2];
+    if (extrinsic_est_en) {
+        // point_be_crossmat * s.offset_R_L_I.conjugate() * C : Eigen evaluates
+        // (Matrix3 * Quaternion) by converting the quaternion to a rotation matrix.
+        V3 B = mul(mul(point_be_crossmat, qmat(qconj(s.offR))), C);
+        row[6] = B[0]; row[7] = B[1]; row[8] = B[2];
+        row[9] = C[0]; row[10] = C[1]; row[11] = C[2];
+    }
+    h = -double(nv[3]);                                                              // :751
+}
+
 }  // namespace
 
 // ============================================================================
@@ -453,6 +500,44 @@ int oracle_esti_plane(const float* pts15, float threshold, float* out4) {
     return esti_plane_f(out4, p, threshold) ? 1 : 0;
 }
 
+// oracle_esti_plane plus the branches it took: trace16 = nonzero_pivots, transp[3], tiny_tail[3], norm[3][3] (PlaneTrace)
+int oracle_esti_plane_trace(const float* pts15, float threshold, float* out4, int* trace16) {
+    static_assert(sizeof(PlaneTrace) == 16 * sizeof(int), "PlaneTrace layout");
+    float p[5][3];
+    for (int i = 0; i < 5; i++) for (int j = 0; j < 3; j++) p[i][j] = pts15[i*3+j];
+    PlaneTrace tr;
+    const int ok = esti_plane_f(out4, p, threshold, &tr) ? 1 : 0;
+    memcpy(trace16, &tr, sizeof(tr));
+    return ok;
+}
+
+// One point of h_share_model (laserMapping.cpp:656-692, :723-751) with every stage evaluated whatever the gates before it
+// decided: pw[3]; flags[3] = kNN gate (:671), plane fit accepted (:678), score gate (:683); pabcd[4]; pd2; score; row[12]
+// (zero beyond 6 without extrinsic estimation); h.  out25 = pw, flags, pabcd, pd2, score, row, h as doubles.
+void oracle_measure_point(const double* x26, const float* pb3, const float* near15, int cnt, float d2_last, int extrinsic_est_en,
+                          double* out25) {
+    const State s = load_state(x26);
+    float pw[3];
+    body_to_world(s, pb3, pw);
+    const bool gate = knn_gate(cnt, d2_last);
+    float pn[5][3];
+    for (int i = 0; i < 5; i++) for (int j = 0; j < 3; j++) pn[i][j] = near15[i*3+j];
+    float pabcd[4];
+    const bool ok = esti_plane_f(pabcd, pn, 0.1f);
+    float pd2;
+    const float sc = plane_score(pabcd, pw, pb3, pd2);
+    const float nv[4] = {pabcd[0], pabcd[1], pabcd[2], pd2};
+    double row[12] = {0}, h;
+    jacobian_row(s, pb3, nv, extrinsic_est_en, row, h);
+    double* o = out25;
+    for (int i = 0; i < 3; i++) *o++ = pw[i];
+    *o++ = gate; *o++ = ok; *o++ = sc > 0.9;
+    for (int i = 0; i < 4; i++) *o++ = pabcd[i];
+    *o++ = pd2; *o++ = sc;
+    for (int i = 0; i < 12; i++) *o++ = row[i];
+    *o++ = h;
+}
+
 void oracle_state_boxplus(double* x26, const double* d23) { State s = load_state(x26); state_boxplus(s, d23); store_state(s, x26); }
 void oracle_state_boxminus(const double* a26, const double* b26, double* r23) { state_boxminus(load_state(a26), load_state(b26), r23); }
 int oracle_inverse(const double* A, double* Ainv, int n) { return inverse_lu(A, Ainv, n) ? 0 : -1; }
@@ -469,10 +554,7 @@ void oracle_S2_Mx(const double* v3_delta2, double* out6) {
     double m[3][2]; S2_Mx(v3(v3_delta2[0], v3_delta2[1], v3_delta2[2]), v3_delta2 + 3, m); memcpy(out6, m, sizeof(m));
 }
 void oracle_transform_point(const double* x26, const float* pb, float* pw) {
-    State s = load_state(x26);
-    V3 p_body = v3(pb[0], pb[1], pb[2]);
-    V3 p_global = add(qrot(s.rot, add(qrot(s.offR, p_body), s.offT)), s.pos);
-    pw[0] = float(p_global[0]); pw[1] = float(p_global[1]); pw[2] = float(p_global[2]);
+    body_to_world(load_state(x26), pb, pw);
 }
 
 // ----------------------------------------------------------------------------
@@ -535,9 +617,8 @@ int oracle_update_iterated(const float* body_pts, int Q, double* x26, double* P,
 #pragma omp parallel for schedule(static)
         for (int i = 0; i < Q; i++) {                                   // :650
             const float* pb = &body_pts[size_t(i) * 4];
-            V3 p_body = v3(pb[0], pb[1], pb[2]);
-            V3 p_global = add(qrot(s.rot, add(qrot(s.offR, p_body), s.offT)), s.pos);   // :657
-            float pw[3] = {float(p_global[0]), float(p_global[1]), float(p_global[2])};
+            float pw[3];
+            body_to_world(s, pb, pw);                                     // :657
             world[size_t(i)*3+0] = pw[0]; world[size_t(i)*3+1] = pw[1]; world[size_t(i)*3+2] = pw[2];
             float* near = &Nearest[size_t(i) * 20];
             if (do_search) {                                              // :667-672
@@ -546,7 +627,7 @@ int oracle_update_iterated(const float* body_pts, int Q, double* x26, double* P,
                 int cnt = knn(knn_ctx, pw, NUM_MATCH_POINTS, tmp, d2);
                 NearestCnt[i] = cnt;
                 for (int j = 0; j < cnt * 4; j++) near[j] = tmp[j];
-                point_selected_surf[i] = cnt < NUM_MATCH_POINTS ? 0 : (d2[NUM_MATCH_POINTS - 1] > 5 ? 0 : 1);
+                point_selected_surf[i] = knn_gate(cnt, d2[NUM_MATCH_POINTS - 1]) ? 1 : 0;
             }
             if (!point_selected_surf[i]) continue;                        // :674
             point_selected_surf[i] = 0;                                   // :677
@@ -554,8 +635,8 @@ int oracle_update_iterated(const float* body_pts, int Q, double* x26, double* P,
             float pn[NUM_MATCH_POINTS][3];
             for (int j = 0; j < NUM_MATCH_POINTS; j++) { pn[j][0] = near[j*4]; pn[j][1] = near[j*4+1]; pn[j][2] = near[j*4+2]; }
             if (esti_plane_f(pabcd, pn, 0.1f)) {                          // :678
-                float pd2 = pabcd[0] * pw[0] + pabcd[1] * pw[1] + pabcd[2] * pw[2] + pabcd[3];   // :680
-                float sc = float(1 - 0.9 * std::fabs(pd2) / std::sqrt(norm(p_body)));            // :681 (T8)
+                float pd2;
+                const float sc = plane_score(pabcd, pw, pb, pd2);         // :680-681
                 if (sc > 0.9) {                                           // :683
                     point_selected_surf[i] = 1;
                     normvec[size_t(i)*4+0] = pabcd[0]; normvec[size_t(i)*4+1] = pabcd[1];
@@ -576,25 +657,7 @@ int oracle_update_iterated(const float* body_pts, int Q, double* x26, double* P,
             h.assign(effct_feat_num, 0.0);
             for (int r = 0; r < effct_feat_num; r++) {                    // :723-752
                 const int i = eff[r];
-                const float* pb = &body_pts[size_t(i) * 4];
-                V3 point_this_be = v3(pb[0], pb[1], pb[2]);
-                M3 point_be_crossmat = hat(point_this_be);
-                V3 point_this = add(qrot(s.offR, point_this_be), s.offT);
-                M3 point_crossmat = hat(point_this);
-                V3 norm_vec = v3(normvec[size_t(i)*4+0], normvec[size_t(i)*4+1], normvec[size_t(i)*4+2]);
-                V3 C = qrot(qconj(s.rot), norm_vec);
-                V3 A = mul(point_crossmat, C);
-                double* row = &h_x[size_t(r) * 12];
-                row[0] = norm_vec[0]; row[1] = norm_vec[1]; row[2] = norm_vec[2];
-                row[3] = A[0]; row[4] = A[1]; row[5] = A[2];
-                if (extrinsic_est_en) {
-                    // point_be_crossmat * s.offset_R_L_I.conjugate() * C : Eigen evaluates
-                    // (Matrix3 * Quaternion) by converting the quaternion to a rotation matrix.
-                    V3 B = mul(mul(point_be_crossmat, qmat(qconj(s.offR))), C);
-                    row[6] = B[0]; row[7] = B[1]; row[8] = B[2];
-                    row[9] = C[0]; row[10] = C[1]; row[11] = C[2];
-                }
-                h[r] = -double(normvec[size_t(i)*4+3]);                   // :751
+                jacobian_row(s, &body_pts[size_t(i) * 4], &normvec[size_t(i) * 4], extrinsic_est_en, &h_x[size_t(r) * 12], h[r]);
             }
         }
         if (log) log->valid = valid ? 1 : 0;

@@ -1,10 +1,12 @@
-// Test harness for the FP64 manifold arithmetic (lie.cuh) and the Gauss-Jordan solvers (gj.cuh).
+// Test harness for the FP64 manifold arithmetic (lie.cuh), the per-point measurement model (measure.cuh) and the
+// Gauss-Jordan solvers (gj.cuh).
 //
-// mh_eval runs one lie.cuh function over a batch of inputs, either in a kernel (one thread per input) or on the host,
+// mh_eval runs one lie.cuh or measure.cuh function over a batch of inputs, either in a kernel (one thread per input) or on the host,
 // from the same FL_HD code; mh_gj runs one Gauss-Jordan routine per block over a batch of systems.  Built with the
 // library's nvcc flags (tests/manifold_harness.py), so it measures the arithmetic the library ships.
 #include "../../fast_lio_b200/csrc/gj.cuh"
 #include "../../fast_lio_b200/csrc/lie.cuh"
+#include "../../fast_lio_b200/csrc/measure.cuh"
 
 namespace fl {
 void set_last_error(const char*, ...) {}
@@ -13,11 +15,49 @@ using namespace fl;
 
 enum Fn {
     F_COS_SINC_SQRT, F_SO3_EXP, F_SO3_LOG, F_A_MATRIX, F_S2_BX, F_S2_BOXPLUS, F_S2_BOXMINUS, F_S2_NX_YY, F_S2_MX,
-    F_S2_CONGRUENCE, F_STATE_BOXPLUS, F_STATE_BOXMINUS, F_COUNT
+    F_S2_CONGRUENCE, F_STATE_BOXPLUS, F_STATE_BOXMINUS, F_ESTI_PLANE, F_MEASURE, F_COUNT
 };
 // inputs / outputs per evaluation, in doubles
 static const int kWidth[F_COUNT][2] = {{1, 2}, {3, 4}, {4, 3}, {3, 9}, {3, 6}, {5, 3}, {6, 2}, {3, 6}, {5, 6},
-                                       {8, 4}, {49, 26}, {52, 23}};
+                                       {8, 4}, {49, 26}, {52, 23}, {16, 5}, {47, 38}};
+
+// Floats travel exactly in the double arrays.
+FL_HD void esti_plane_eval(const double* in, double* out) {      // in: 5 x 3 points, threshold; out: ok, pabcd
+    float pt[KNN_K][3], pabcd[4];
+    for (int j = 0; j < KNN_K; j++) for (int c = 0; c < 3; c++) pt[j][c] = (float)in[3 * j + c];
+    out[0] = esti_plane_dev(pabcd, pt, (float)in[15]) ? 1.0 : 0.0;
+    for (int c = 0; c < 4; c++) out[1 + c] = pabcd[c];
+}
+
+// One scan point through the measurement model in the order of measure_fused (update.cuh), every stage evaluated whatever
+// the gates before it decided.  in: x26, body point (3), 5 x 3 neighbours, neighbour count, 5th squared distance, extr.
+// out: world point (3), kNN gate, plane ok, score gate, pabcd (4), pd2, score, row (12, jacobian_row_at), z, and the row
+// and z of jacobian_row (the split kernels' form).
+template <bool EXTR>
+FL_HD void measure_eval(const double* in, double* out) {
+    const PoseS s = load_pose(in);
+    const float4 pb = make_float4((float)in[26], (float)in[27], (float)in[28], 0.f);
+    float pn[KNN_K][3];
+    for (int j = 0; j < KNN_K; j++) for (int c = 0; c < 3; c++) pn[j][c] = (float)in[29 + 3 * j + c];
+    float wx, wy, wz;
+    const D3 p_this = body_to_world(s, pb, wx, wy, wz);
+    const bool gate = knn_gate((int)in[44], (float)in[45]);
+    float pabcd[4];
+    const bool ok = esti_plane_dev(pabcd, pn, 0.1f);
+    const float pd2 = plane_residual(pabcd, wx, wy, wz);
+    float score;
+    const bool scored = score_gate(pd2, sqrt(norm3(d3(pb.x, pb.y, pb.z))), score);
+    const float4 nv = make_float4(pabcd[0], pabcd[1], pabcd[2], pd2);
+    double h[12] = {0.0}, h2[12] = {0.0}, z, z2;
+    jacobian_row_at<EXTR>(s, pb, p_this, nv, h, z);
+    jacobian_row<EXTR>(s, pb, nv, h2, z2);
+    out[0] = wx; out[1] = wy; out[2] = wz;
+    out[3] = gate; out[4] = ok; out[5] = scored;
+    for (int c = 0; c < 4; c++) out[6 + c] = pabcd[c];
+    out[10] = pd2; out[11] = score;
+    for (int c = 0; c < 12; c++) { out[12 + c] = h[c]; out[25 + c] = h2[c]; }
+    out[24] = z; out[37] = z2;
+}
 
 FL_HD void eval(int fn, const double* in, double* out) {
     switch (fn) {
@@ -33,6 +73,8 @@ FL_HD void eval(int fn, const double* in, double* out) {
     case F_S2_CONGRUENCE: S2_congruence(ld3(in), ld3(in + 3), in[6], in[7], out); break;
     case F_STATE_BOXPLUS: for (int i = 0; i < XLEN; i++) out[i] = in[i]; state_boxplus(out, in + XLEN); break;
     case F_STATE_BOXMINUS: state_boxminus(in, in + XLEN, out); break;
+    case F_ESTI_PLANE: esti_plane_eval(in, out); break;
+    case F_MEASURE: if (in[46] != 0.0) measure_eval<true>(in, out); else measure_eval<false>(in, out); break;
     }
 }
 

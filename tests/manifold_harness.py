@@ -1,4 +1,4 @@
-"""ctypes front of tests/kernels/manifold_harness.cu, compiled with the library's nvcc flags into a temporary directory."""
+"""ctypes front of tests/kernels/manifold_harness.cu (lie.cuh, measure.cuh and gj.cuh over batches of inputs), compiled with the library's nvcc flags into a temporary directory."""
 from __future__ import annotations
 
 import ctypes as C
@@ -12,7 +12,7 @@ from fast_lio_b200 import build
 SRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "kernels", "manifold_harness.cu")
 
 FNS = ["cos_sinc_sqrt", "so3_exp", "so3_log", "A_matrix", "S2_Bx", "S2_boxplus", "S2_boxminus", "S2_Nx_yy", "S2_Mx",
-       "S2_congruence", "state_boxplus", "state_boxminus"]
+       "S2_congruence", "state_boxplus", "state_boxminus", "esti_plane", "measure"]
 GJ = ["gj_eliminate", "gj_warp", "gj_warp_reg6", "gj_warp_reg12", "gj_cols6", "gj_cols12"]
 
 _f64p = np.ctypeslib.ndpointer(dtype=np.float64, flags="C_CONTIGUOUS")
