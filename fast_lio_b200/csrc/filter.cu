@@ -1015,7 +1015,7 @@ Filter::~Filter() {
     for (int r = 0; r < P2P_MAX_RANKS; r++) if (peer_ptr_[r]) cudaIpcCloseMemHandle(peer_ptr_[r]);
     mailbox_.release(); p2p_.release();
     body_.release(); nearest_.release(); nearest_cnt_.release(); selected_.release(); normvec_.release(); plane_.release(); srange_.release();
-    partials_.release(); red_.release(); ctl_.release(); ctl0_.release(); logs_.release(); pub_.release();
+    partials_.release(); red_.release(); ctl_.release(); ctl0_.release(); logs_.release(); pub_.release(); rows_.release();
     mi_world_.release(); mi_flag_add_.release(); mi_flag_no_.release(); mi_list_add_.release(); mi_list_no_.release(); mi_tmp_.release(); mi_counts_.release();
     d_bind_.release();
     b_body_.release(); b_ctl_.release(); b_pub_.release(); b_partials_.release();
@@ -1071,6 +1071,24 @@ int Filter::init() {
     batch_cap_[0] = sms_ * occ;
     FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_batch<true>, UPD_THREADS, 0));
     batch_cap_[1] = sms_ * occ;
+    // k_update_wave: k_update<EXTR, 2>'s block with its tile's points in dynamic shared memory
+    FL_CUDA(cudaFuncSetAttribute(k_update_wave<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WavePoint)));
+    FL_CUDA(cudaFuncSetAttribute(k_update_wave<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WavePoint)));
+    FL_CUDA(cudaFuncSetAttribute(k_update_n_wave<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WavePoint)));
+    FL_CUDA(cudaFuncSetAttribute(k_update_n_wave<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WavePoint)));
+    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_wave<false>, 2 * UPD_THREADS, sizeof(WavePoint)));
+    wave_capacity_[0] = sms_ * occ;
+    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_wave<true>, 2 * UPD_THREADS, sizeof(WavePoint)));
+    wave_capacity_[1] = sms_ * occ;
+    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_n_wave<false>, 2 * UPD_THREADS, sizeof(WavePoint)));
+    wave_n_capacity_[0] = std::min(wave_capacity_[0], sms_ * occ);
+    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_n_wave<true>, 2 * UPD_THREADS, sizeof(WavePoint)));
+    wave_n_capacity_[1] = std::min(wave_capacity_[1], sms_ * occ);
+    {
+        const size_t bytes = sizeof(unsigned long long) * 2 * PSTRIDE * (size_t)std::max(1, std::max(wave_capacity_[0], wave_capacity_[1]));
+        FL_CHECK(rows_.reserve(bytes));
+        FL_CUDA(cudaMemsetAsync(rows_.ptr, 0, bytes, stream()));     // tag 0: never current (row_tag)
+    }
     FL_CHECK(d_bind_.reserve(2 * sizeof(int)));
     FL_CUDA(cudaMemsetAsync(d_bind_.ptr, 0, 2 * sizeof(int), stream()));
     FL_CHECK(partials_.reserve(sizeof(double) * PSTRIDE * (size_t)std::max(upd_capacity_[0][0], upd_capacity_[1][0])));
@@ -1179,15 +1197,19 @@ int Filter::restore_state() {
 }
 
 template <class... KArgs, class... Args>
-static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, int block, cudaStream_t st, bool pdl, Args... args) {
+static cudaError_t launch_pdl_smem(void (*kernel)(KArgs...), dim3 grid, int block, size_t smem, cudaStream_t st, bool pdl, Args... args) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = grid; cfg.blockDim = dim3((unsigned)block); cfg.dynamicSmemBytes = 0; cfg.stream = st;
+    cfg.gridDim = grid; cfg.blockDim = dim3((unsigned)block); cfg.dynamicSmemBytes = smem; cfg.stream = st;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
     cfg.attrs = attr; cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
+}
+template <class... KArgs, class... Args>
+static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, int block, cudaStream_t st, bool pdl, Args... args) {
+    return launch_pdl_smem(kernel, grid, block, 0, st, pdl, args...);
 }
 
 // Nearest_Points of the points other ranks own: the same search, with the state the last searching pass used, on this rank's
@@ -1282,7 +1304,14 @@ int Filter::launch_update(int max_passes, int mode, int search_only, cudaStream_
     // one thread per point: full warps (the search is bound by a thread's own chain of loads, not by the number of SMs)
     int workers = mode == 3 ? 0 : std::min(cap - 1, (nq + UPD_THREADS - 1) / UPD_THREADS);
     if (workers < 0) workers = 0;
-    FL_CUDA(launch_upd(workers, pdl_, a, upd_pair(nq), st));
+    const int pair = upd_pair(nq);
+    if (use_wave(workers, pair, mode)) {      // pair 2: the tiles fit the 512-thread grid, so workers == tiles (one each)
+        unsigned long long* rows = rows_.as<unsigned long long>();
+        FL_CUDA(extrinsic_est_ ? launch_pdl_smem(k_update_wave<true>, workers + 1, 2 * UPD_THREADS, sizeof(WavePoint), st, pdl_, a, rows)
+                               : launch_pdl_smem(k_update_wave<false>, workers + 1, 2 * UPD_THREADS, sizeof(WavePoint), st, pdl_, a, rows));
+        return FL_OK;
+    }
+    FL_CUDA(launch_upd(workers, pdl_, a, pair, st));
     return FL_OK;
 }
 
@@ -1497,7 +1526,11 @@ int Filter::update_scan_on_stream(const float4* d_body, const int* d_n, int n_ma
     const int* n = d_bind_.as<int>();
     const int block = pair * UPD_THREADS;
     cudaError_t rc;
-    if (e) rc = pair == 2 ? launch_pdl(k_update_n<true, 2>, workers + 1, block, st, pdl_, a, n) : launch_pdl(k_update_n<true, 1>, workers + 1, block, st, pdl_, a, n);
+    if (pair == 2 && workers + 1 <= wave_n_capacity_[e]) {
+        unsigned long long* rows = rows_.as<unsigned long long>();
+        rc = e ? launch_pdl_smem(k_update_n_wave<true>, workers + 1, block, sizeof(WavePoint), st, pdl_, a, n, rows)
+               : launch_pdl_smem(k_update_n_wave<false>, workers + 1, block, sizeof(WavePoint), st, pdl_, a, n, rows);
+    } else if (e) rc = pair == 2 ? launch_pdl(k_update_n<true, 2>, workers + 1, block, st, pdl_, a, n) : launch_pdl(k_update_n<true, 1>, workers + 1, block, st, pdl_, a, n);
     else rc = pair == 2 ? launch_pdl(k_update_n<false, 2>, workers + 1, block, st, pdl_, a, n) : launch_pdl(k_update_n<false, 1>, workers + 1, block, st, pdl_, a, n);
     FL_CUDA(rc);
     launches_ = 1;

@@ -193,6 +193,10 @@ private:
     bool stream_bound_ = false;
     DeviceBuffer d_bind_;
     int upd_n_capacity_[2][2] = {{0, 0}, {0, 0}};   // co-resident k_update_n blocks, capped at k_update's (the same tiles per block)
+    // k_update_wave / k_update_n_wave: co-resident blocks [EXTR] and the tagged partial rows (one per worker block)
+    int wave_capacity_[2] = {0, 0}, wave_n_capacity_[2] = {0, 0};
+    DeviceBuffer rows_;
+    bool use_wave(int workers, int pair, int mode) const { return mode == 0 && pair == 2 && workers + 1 <= wave_capacity_[extrinsic_est_ ? 1 : 0]; }
     int read_binding();
     int batch_cap_[2] = {0, 0};        // co-resident k_update_batch<EXTR> blocks on this device
     int batch_nq_max_ = -1;            // the nq_max reserve_batch sized the batch buffers for (-1: not yet)

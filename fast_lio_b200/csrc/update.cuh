@@ -850,4 +850,303 @@ __global__ void __launch_bounds__(UPD_THREADS, 2) k_update_batch(UpdArgs a, int 
     update_body<EXTR, 1>(a, a.sc.q_end);
 }
 
+// ============================================================================= one tile per worker block: k_update_wave
+// The single-GPU update (mode 0) when every tile of the scan has a worker block of its own, which is exactly when Filter::upd_pair
+// picks two threads per point: the 512-thread block, the paired search and the tiles of k_update<EXTR, 2>, so the same bytes.
+// Thread t < 256 owns point tile + t for the whole launch, which removes three things from every pass's chain:
+//   * the point's state stays in shared memory (WavePoint): the body point, sqrt(|p_body|), the plane and the selected flag; a
+//     pass that does not search no longer reloads selected -> plane -> srange from L2 (the memory copies are still written);
+//   * the pickup of the solver's publication: lanes 0..28 of warp 0 spin on their own tagged word, then one barrier;
+//   * the partial rows go out as tagged words (row_tag: 32 bits of payload, 32 of tag, as pub_store), with no ticket; each
+//     solver warp spins on and sums its own rows as they arrive, in sol_reduce's order.
+// A graph replay keeps the launch nonce it was captured with, so the rows are tagged with an epoch kept in device memory
+// (word WAVE_EPOCH of the publication block, outside the control block that restore_state rewinds): each launch tags with
+// the stored epoch + 1 and the solver stores it when the update ends, so no row of an earlier launch is ever current.
+// Stamps in ctl->prof besides k_update's clock64 ones, in %globaltimer ns so they compare across SMs, for the pass that ends
+// the update: [11] the solver has summed every partial row, [2] its publication is visible on the solver's SM (an otherwise
+// idle thread of block 0 polls for it), [3] the last worker block has picked it up.  Each is read by a thread nothing waits
+// for: a %globaltimer read costs several hundred cycles on H100.
+struct WavePoint {                 // dynamic shared memory of a worker block: its tile's points
+    float4 body[UPD_THREADS];
+    float4 plane[UPD_THREADS];
+    double srange[UPD_THREADS];
+    unsigned char sel[UPD_THREADS];
+};
+constexpr int WAVE_EPOCH = 32;     // word of the publication block (a 128-byte line of its own)
+__device__ __forceinline__ unsigned row_tag(unsigned epoch, int pass) { return pub_tag(epoch, pass + 1); }     // never 0
+__device__ __forceinline__ unsigned long long globaltimer() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+__device__ __forceinline__ ulonglong2 row_load(const unsigned long long* p) {
+    ulonglong2 v;
+    asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(v.x), "=l"(v.y) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ bool row_current(ulonglong2 v, unsigned tag) { return (unsigned)(v.x >> 32) == tag && (unsigned)(v.y >> 32) == tag; }
+__device__ __forceinline__ double row_value(ulonglong2 v) { return __longlong_as_double((long long)((v.y << 32) | (v.x & 0xffffffffull))); }
+
+// measure_fused<EXTR, 2> with the point's state in `pt` (slot threadIdx.x % 256); the same outputs in memory
+template <bool EXTR>
+__device__ __forceinline__ bool measure_wave(const MapView& m, const ScanView& sc, int q, bool active, const PoseS& s, bool searched,
+                                             bool search_only, WalkPool& walks, int& phase, double* stage, WavePoint& pt, double* h,
+                                             double& z, float& absres) {
+    const int i = threadIdx.x & (UPD_THREADS - 1);
+    float4 pb = make_float4(0.f, 0.f, 0.f, 0.f);
+    float wx = 0.f, wy = 0.f, wz = 0.f;
+    D3 p_this = d3(0.0, 0.0, 0.0);
+    if (active) {
+        pb = pt.body[i];
+        p_this = body_to_world(s, pb, wx, wy, wz);
+    }
+    bool sel = false;
+    float pabcd[4] = {0.f, 0.f, 0.f, 0.f};
+    if (searched) {
+        TBest kb;
+        knn_block_pair(m, active, wx, wy, wz, kb, walks, phase, stage);
+        if (threadIdx.x >= UPD_THREADS) return false;
+        if (active) {
+            float4 p[KNN_K];
+            const int cnt = knn_fetch(m, kb, p);
+#pragma unroll
+            for (int j = 0; j < KNN_K; j++) sc.nearest[(size_t)q * KNN_K + j] = p[j];
+            sc.nearest_cnt[q] = cnt;
+            sel = knn_gate(cnt, kb.d[KNN_K - 1]);
+            if (search_only) { sc.selected[q] = sel ? 1 : 0; return false; }
+            if (sel) {
+                float pn[KNN_K][3];
+#pragma unroll
+                for (int j = 0; j < KNN_K; j++) { pn[j][0] = p[j].x; pn[j][1] = p[j].y; pn[j][2] = p[j].z; }
+                sel = esti_plane_dev(pabcd, pn, 0.1f);
+                if (sel) { const float4 pl = make_float4(pabcd[0], pabcd[1], pabcd[2], pabcd[3]); sc.plane[q] = pl; pt.plane[i] = pl; }
+            }
+        }
+    } else if (active) {
+        sel = pt.sel[i] != 0;
+        if (sel) { const float4 pl = pt.plane[i]; pabcd[0] = pl.x; pabcd[1] = pl.y; pabcd[2] = pl.z; pabcd[3] = pl.w; }
+    }
+    bool contrib = false;
+    if (active && sel) {
+        const float pd2 = plane_residual(pabcd, wx, wy, wz);
+        const double srange = pt.srange[i];
+        if (searched) sc.srange[q] = srange;
+        float score;
+        if (score_gate(pd2, srange, score)) {
+            contrib = true;
+            absres = fabsf(pd2);
+            jacobian_row_at<EXTR>(s, pb, p_this, make_float4(pabcd[0], pabcd[1], pabcd[2], pd2), h, z);
+        }
+    }
+    if (active) { sc.selected[q] = contrib ? 1 : 0; pt.sel[i] = contrib ? 1 : 0; }
+    return contrib;
+}
+
+// sol_reduce over tagged rows: warp w takes the rows w, w + 8, ... of pass `tag` GATHER_ROWS at a time, spins until each of them
+// is current (every poll reloads all the stale words of the batch at once: one round trip) and sums them in ascending order from
+// +0.0 (sol_reduce's order; the +0.0 rows it adds past nwork change no sum)
+constexpr int GATHER_ROWS = 8;
+__device__ void sol_gather(SolverSm& S, FilterCtl* ctl, const unsigned long long* __restrict__ rows, int nwork, unsigned tag) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    double a0 = 0.0, a1 = 0.0, a2 = 0.0;
+    bool late = false;
+    const long long t0 = clock64();
+    for (int b = warp; b < nwork; b += GATHER_ROWS * UPD_WARPS) {
+        const unsigned long long* base = rows + (size_t)b * PSTRIDE * 2 + 2 * lane;
+        ulonglong2 v[GATHER_ROWS][3];
+#pragma unroll
+        for (int k = 0; k < GATHER_ROWS; k++) {
+#pragma unroll
+            for (int j = 0; j < 3; j++) v[k][j] = make_ulonglong2(0ull, 0ull);
+            if (b + k * UPD_WARPS < nwork) {
+#pragma unroll
+                for (int j = 0; j < 3; j++) v[k][j] = row_load(base + (size_t)k * UPD_WARPS * PSTRIDE * 2 + 64 * j);
+            }
+        }
+        while (true) {
+            bool stale = false;
+#pragma unroll
+            for (int k = 0; k < GATHER_ROWS; k++) {
+#pragma unroll
+                for (int j = 0; j < 3; j++) stale |= b + k * UPD_WARPS < nwork && !row_current(v[k][j], tag);
+            }
+            if (!stale) break;
+            if (clock64() - t0 > SPIN_LIMIT) { late = true; break; }
+#pragma unroll
+            for (int k = 0; k < GATHER_ROWS; k++) {
+#pragma unroll
+                for (int j = 0; j < 3; j++) {
+                    if (b + k * UPD_WARPS < nwork && !row_current(v[k][j], tag)) v[k][j] = row_load(base + (size_t)k * UPD_WARPS * PSTRIDE * 2 + 64 * j);
+                }
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < GATHER_ROWS; k++) {
+            if (b + k * UPD_WARPS < nwork) { a0 += row_value(v[k][0]); a1 += row_value(v[k][1]); a2 += row_value(v[k][2]); }
+        }
+        if (late) break;
+    }
+    S.wred[warp][lane] = a0; S.wred[warp][lane + 32] = a1; S.wred[warp][lane + 64] = a2;
+    if (late) S.late = 2;
+    sol_sync();
+    if (tid == 0) ctl->prof[9] = clock64();
+    if (tid < PSTRIDE) {
+        double v = 0.0;
+#pragma unroll
+        for (int w = 0; w < UPD_WARPS; w++) v += S.wred[w][tid];
+        S.red[tid] = v;
+        if (tid < 78) {
+            int a = 0, rem = tid;
+            while (rem >= 12 - a) { rem -= 12 - a; a++; }
+            const int b = a + rem;
+            S.HTH[a * 12 + b] = v; S.HTH[b * 12 + a] = v;
+        }
+    }
+    sol_sync();
+    if (tid == 128) ctl->prof[11] = (long long)globaltimer();         // a warp the gain does not wait for
+}
+
+// update_body<EXTR, 2> for mode 0 with one tile per worker block (gridDim.x - 1 >= the tiles of [q_begin, q1)); rows: the
+// partial rows as tagged words, [worker block][PSTRIDE][2]
+template <bool EXTR>
+__device__ __forceinline__ void update_wave_body(const UpdArgs& a, unsigned long long* __restrict__ rows, const int q1) {
+    static_assert(sizeof(PairXch) <= sizeof(double) * WorkerSm<EXTR>::STAGE, "the partner's list fits the owner warp's stage slice");
+    __shared__ __align__(16) unsigned char smem_raw[sizeof(SolverSm) > sizeof(WorkerSm<EXTR>) ? sizeof(SolverSm) : sizeof(WorkerSm<EXTR>)];
+    extern __shared__ __align__(16) unsigned char wave_dyn[];
+    __shared__ volatile int solver_ended;
+    FilterCtl* ctl = a.ctl;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int nwork = (int)gridDim.x - 1;
+    pdl_wait();
+    pdl_launch();
+    const unsigned epoch = (unsigned)__ldcg(a.pub + WAVE_EPOCH) + 1u;
+    if (blockIdx.x > 0) {
+        // ------------------------------------------------------------------ worker block
+        WorkerSm<EXTR>& Wk = *reinterpret_cast<WorkerSm<EXTR>*>(smem_raw);
+        WavePoint& pt = *reinterpret_cast<WavePoint*>(wave_dyn);
+        const int wb = (int)blockIdx.x - 1;
+        const int i = tid & (UPD_THREADS - 1), q = a.sc.q_begin + wb * UPD_THREADS + i;
+        const bool active = q < q1, owner = tid < UPD_THREADS;
+        if (tid == 0) { Wk.abort = 0; Wk.walks.n[0] = Wk.walks.n[1] = 0; }
+        int walk_phase = 0;
+        double* stage = Wk.stage[warp & (UPD_WARPS - 1)];
+        for (int p = 0; p < a.max_passes; p++) {
+            PoseS s;
+            bool searched;
+            if (p == 0) {
+                // the state this launch starts from, and the tile's points, loaded together
+                const bool done = __ldcg(&ctl->done) != 0;
+                searched = __ldcg(&ctl->converge) != 0 || a.search_only;
+                s = load_pose(a.pose_from_search ? ctl->x_search : ctl->x);
+                if (owner && active) {
+                    const float4 pb = __ldg(&a.sc.body[q]);
+                    pt.body[i] = pb;
+                    pt.srange[i] = sqrt(norm3(d3(pb.x, pb.y, pb.z)));       // sqrt(p_body.norm()) of the score, for every pass
+                    if (!searched) {                                        // the fit and the flag of an earlier launch
+                        pt.sel[i] = a.sc.selected[q];
+                        if (pt.sel[i]) { pt.plane[i] = a.sc.plane[q]; pt.srange[i] = a.sc.srange[q]; }
+                    }
+                }
+                __syncthreads();
+                if (done && !a.search_only) return;
+            } else {
+                const unsigned tag = pub_tag(a.nonce, p);
+                if (warp == 0 && lane < PUB_WORDS) {
+                    unsigned long long w = pub_load(a.pub + lane);
+                    const long long t0 = clock64();
+                    while ((unsigned)(w >> 32) != tag) {
+                        if (clock64() - t0 > SPIN_LIMIT) { Wk.abort = 1; atomicExch(&ctl->error, 3); break; }
+                        w = pub_load(a.pub + lane);
+                    }
+                    if (lane < 28) Wk.pose_bits[lane] = (unsigned)w; else Wk.flags = (unsigned)w;
+                }
+                __syncthreads();
+                if (Wk.abort) return;
+                if (Wk.flags & 2u) {
+                    // reading %globaltimer takes hundreds of cycles: stamped only where nothing waits for it
+                    if (tid == 0) atomicMax(reinterpret_cast<unsigned long long*>(&ctl->prof[3]), globaltimer());
+                    return;
+                }
+                searched = (Wk.flags & 1u) != 0;
+                double x14[14];
+#pragma unroll
+                for (int k = 0; k < 14; k++) x14[k] = __longlong_as_double((long long)(((unsigned long long)Wk.pose_bits[2 * k + 1] << 32) | Wk.pose_bits[2 * k]));
+                s.pos = d3(x14[X_POS], x14[X_POS + 1], x14[X_POS + 2]);
+                s.rot.x = x14[X_ROT]; s.rot.y = x14[X_ROT + 1]; s.rot.z = x14[X_ROT + 2]; s.rot.w = x14[X_ROT + 3];
+                s.offR.x = x14[X_OFFR]; s.offR.y = x14[X_OFFR + 1]; s.offR.z = x14[X_OFFR + 2]; s.offR.w = x14[X_OFFR + 3];
+                s.offT = d3(x14[X_OFFT], x14[X_OFFT + 1], x14[X_OFFT + 2]);
+            }
+            double acc[3] = {0.0, 0.0, 0.0};
+            double h[12]; double z = 0.0; float ar = 0.f;
+            bool contrib = false;
+            if (owner || searched)
+                contrib = measure_wave<EXTR>(a.m, a.sc, q, active, s, searched, a.search_only != 0, Wk.walks, walk_phase, stage, pt, h, z, ar);
+            if (owner && !a.search_only) warp_accumulate<EXTR>(contrib, h, z, ar, acc, lane, stage);
+            if (a.search_only) return;
+            if (owner) {
+#pragma unroll
+                for (int j = 0; j < 3; j++) Wk.wred[warp][lane + 32 * j] = acc[j];
+            }
+            __syncthreads();
+            if (tid < PSTRIDE) {
+                double v = 0.0;
+#pragma unroll
+                for (int w = 0; w < UPD_WARPS; w++) v += Wk.wred[w][tid];
+                const unsigned long long bits = (unsigned long long)__double_as_longlong(v);
+                unsigned long long* dst = rows + ((size_t)wb * PSTRIDE + tid) * 2;
+                const unsigned tag = row_tag(epoch, p);
+                pub_store(dst, tag, (unsigned)bits);
+                pub_store(dst + 1, tag, (unsigned)(bits >> 32));
+            }
+        }
+        return;
+    }
+    // ------------------------------------------------------------------ solver block
+    if (a.search_only) return;
+    if (tid == 0) solver_ended = 0;
+    __syncthreads();
+    if (tid >= UPD_THREADS) {
+        // one thread stamps the publications as they become visible on this SM
+        if (tid == UPD_THREADS) {
+            for (int p = 1; p <= a.max_passes; p++) {
+                const unsigned tag = pub_tag(a.nonce, p);
+                unsigned long long w;
+                while ((unsigned)((w = pub_load(a.pub + 28)) >> 32) != tag) if (solver_ended) return;
+                ctl->prof[2] = (long long)globaltimer();
+                if (w & 2u) return;
+            }
+        }
+        return;
+    }
+    SolverSm& S = *reinterpret_cast<SolverSm*>(smem_raw);
+    sol_load(S, ctl);
+    for (int p = 0; p < a.max_passes && !S.done; p++) {
+        if (tid == 0) ctl->prof[0] = clock64();
+        if (S.converge && tid < XLEN) ctl->x_search[tid] = S.x[tid];
+        sol_prepare(S);
+        if (tid == 0) ctl->prof[8] = clock64();
+        sol_gather(S, ctl, rows, nwork, row_tag(epoch, p));
+        if (tid == 0) ctl->prof[1] = clock64();
+        sol_pass<EXTR>(S, ctl, a.logs, a.pub, pub_tag(a.nonce, p + 1));
+        if (tid == 0) ctl->prof[7] = clock64();
+    }
+    if (tid == 0) {
+        ctl->error = S.error | ctl->error; ctl->ticket = 0;
+        a.pub[WAVE_EPOCH] = epoch;
+        solver_ended = 1;
+    }
+    sol_sync();
+    mirror_copy(ctl, UPD_THREADS);
+}
+
+template <bool EXTR>
+__global__ void __launch_bounds__(2 * UPD_THREADS, 1) k_update_wave(UpdArgs a, unsigned long long* rows) {
+    update_wave_body<EXTR>(a, rows, a.sc.q_end);
+}
+// k_update_n's form: the point count in device memory (read before pdl_wait, see k_update_n)
+template <bool EXTR>
+__global__ void __launch_bounds__(2 * UPD_THREADS, 1) k_update_n_wave(UpdArgs a, const int* __restrict__ n, unsigned long long* rows) {
+    update_wave_body<EXTR>(a, rows, min(*n, a.sc.q_end));
+}
+
 }  // namespace fl

@@ -29,6 +29,10 @@ p = np.array(list(prof), dtype=np.int64)
 if f.fused():
     print("last-pass cycles (k_update solver block): prepare", p[8] - p[0], "wait for tickets", p[9] - p[8], "reduce(+exchange)", p[1] - p[9],
           "gain", p[4] - p[1], "dx+converge", p[6] - p[4], "pose boxplus", p[10] - p[6], "publish", p[5] - p[10], "after publication (log, covariance)", p[7] - p[5], "total", p[7] - p[0])
+    if p[11] and p[2] and p[3]:
+        # k_update_wave only (%globaltimer ns, comparable across SMs): the pass that ends the update
+        print("last pass ns (k_update_wave): every partial row in -> publication visible", p[2] - p[11],
+              "publication -> last worker block has it", p[3] - p[2])
 else:
     print("last-pass cycles: prepare", p[8] - p[0], "wait", p[9] - p[8], "reduce", p[1] - p[9], "gain", p[4] - p[1],
           "dxu", p[5] - p[4], "boxplus", p[6] - p[5], "tail", p[7] - p[6], "total", p[7] - p[0])
