@@ -1051,47 +1051,34 @@ int Filter::init() {
     else FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_search<4>, SEARCH_THREADS, 0));
     search_grid_max_ = sms_ * std::max(1, occ);
     if (const char* e = getenv("FASTLIO_B200_LEGACY")) fused_ = !(e[0] == '1');      // A/B: the split kernels of round 1
-    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update<false, 1>, UPD_THREADS, 0));
-    upd_capacity_[0][0] = sms_ * std::max(1, occ);
-    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update<true, 1>, UPD_THREADS, 0));
-    upd_capacity_[1][0] = sms_ * std::max(1, occ);
-    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update<false, 2>, 2 * UPD_THREADS, 0));
-    upd_capacity_[0][1] = sms_ * occ;
-    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update<true, 2>, 2 * UPD_THREADS, 0));
-    upd_capacity_[1][1] = sms_ * occ;
-    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_n<false, 1>, UPD_THREADS, 0));
-    upd_n_capacity_[0][0] = std::min(upd_capacity_[0][0], sms_ * std::max(1, occ));
-    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_n<true, 1>, UPD_THREADS, 0));
-    upd_n_capacity_[1][0] = std::min(upd_capacity_[1][0], sms_ * std::max(1, occ));
-    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_n<false, 2>, 2 * UPD_THREADS, 0));
-    upd_n_capacity_[0][1] = std::min(upd_capacity_[0][1], sms_ * occ);
-    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_n<true, 2>, 2 * UPD_THREADS, 0));
-    upd_n_capacity_[1][1] = std::min(upd_capacity_[1][1], sms_ * occ);
-    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_batch<false>, UPD_THREADS, 0));
-    batch_cap_[0] = sms_ * occ;
-    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_batch<true>, UPD_THREADS, 0));
-    batch_cap_[1] = sms_ * occ;
-    // k_update_wave: k_update<EXTR, 2>'s block with its tile's points in dynamic shared memory
-    FL_CUDA(cudaFuncSetAttribute(k_update_wave<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WavePoint)));
-    FL_CUDA(cudaFuncSetAttribute(k_update_wave<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WavePoint)));
-    FL_CUDA(cudaFuncSetAttribute(k_update_n_wave<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WavePoint)));
-    FL_CUDA(cudaFuncSetAttribute(k_update_n_wave<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WavePoint)));
-    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_wave<false>, 2 * UPD_THREADS, sizeof(WavePoint)));
-    wave_capacity_[0] = sms_ * occ;
-    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_wave<true>, 2 * UPD_THREADS, sizeof(WavePoint)));
-    wave_capacity_[1] = sms_ * occ;
-    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_n_wave<false>, 2 * UPD_THREADS, sizeof(WavePoint)));
-    wave_n_capacity_[0] = std::min(wave_capacity_[0], sms_ * occ);
-    FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_update_n_wave<true>, 2 * UPD_THREADS, sizeof(WavePoint)));
-    wave_n_capacity_[1] = std::min(wave_capacity_[1], sms_ * occ);
+    // co-resident blocks of every update kernel (the solver block and its workers wait for each other).  The one-thread k_update
+    // forms count at least one block per SM; a k_update_n form runs its host form's tiles, so it is capped at that form's grid.
+    const void* const upd_fn[UK_COUNT][2] = {      // [UpdKernel][EXTR]
+        {(const void*)k_update<false, 1>, (const void*)k_update<true, 1>}, {(const void*)k_update<false, 2>, (const void*)k_update<true, 2>},
+        {(const void*)k_update_n<false, 1>, (const void*)k_update_n<true, 1>}, {(const void*)k_update_n<false, 2>, (const void*)k_update_n<true, 2>},
+        {(const void*)k_update_wave<false>, (const void*)k_update_wave<true>}, {(const void*)k_update_n_wave<false>, (const void*)k_update_n_wave<true>},
+        {(const void*)k_update_batch<false>, (const void*)k_update_batch<true>}};
+    upd_caps_.threads = UPD_THREADS;
+    upd_caps_.wave_smem = (int)sizeof(WavePoint);      // a wave block's tile of points in dynamic shared memory
+    for (int k = 0; k < UK_COUNT; k++)
+        for (int e = 0; e < 2; e++) {
+            const int smem = k == UK_WAVE || k == UK_N_WAVE ? upd_caps_.wave_smem : 0;
+            if (smem) FL_CUDA(cudaFuncSetAttribute(upd_fn[k][e], cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+            FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, upd_fn[k][e], upd_kernel_pair(k) * UPD_THREADS, smem));
+            int& cap = upd_caps_.blocks[k][e];
+            cap = sms_ * (k == UK_UPDATE1 || k == UK_N1 ? std::max(1, occ) : occ);
+            const int host = k == UK_N1 ? UK_UPDATE1 : k == UK_N2 ? UK_UPDATE2 : k == UK_N_WAVE ? UK_WAVE : -1;
+            if (host >= 0) cap = std::min(cap, upd_caps_.blocks[host][e]);
+        }
     {
-        const size_t bytes = sizeof(unsigned long long) * 2 * PSTRIDE * (size_t)std::max(1, std::max(wave_capacity_[0], wave_capacity_[1]));
+        const int* wave = upd_caps_.blocks[UK_WAVE];
+        const size_t bytes = sizeof(unsigned long long) * 2 * PSTRIDE * (size_t)std::max(1, std::max(wave[0], wave[1]));
         FL_CHECK(rows_.reserve(bytes));
         FL_CUDA(cudaMemsetAsync(rows_.ptr, 0, bytes, stream()));     // tag 0: never current (row_tag)
     }
     FL_CHECK(d_bind_.reserve(2 * sizeof(int)));
     FL_CUDA(cudaMemsetAsync(d_bind_.ptr, 0, 2 * sizeof(int), stream()));
-    FL_CHECK(partials_.reserve(sizeof(double) * PSTRIDE * (size_t)std::max(upd_capacity_[0][0], upd_capacity_[1][0])));
+    FL_CHECK(partials_.reserve(sizeof(double) * PSTRIDE * (size_t)std::max(upd_caps_.blocks[UK_UPDATE1][0], upd_caps_.blocks[UK_UPDATE1][1])));
     max_resid_grid_ = sms_;
     FL_CHECK(partials_.reserve(sizeof(double) * PSTRIDE * (size_t)max_resid_grid_));
     FL_CHECK(reserve(std::max(1, max_points_)));
@@ -1222,17 +1209,9 @@ int Filter::complete_neighbours() {
     for (int r = 0; r < 2; r++) {
         if (ranges[r][1] <= ranges[r][0]) continue;
         scan_.q_begin = ranges[r][0]; scan_.q_end = ranges[r][1];
-        UpdArgs a;
-        a.m = map_->view();
-        if (search_mode_ == 0) a.m.dir.cap = 0;
-        a.sc = scan_; a.ctl = ctl_.as<FilterCtl>(); a.partials = partials_.as<double>(); a.red_g = red_.as<double>();
-        a.logs = logs_.as<PassLog>(); a.p2p = p2p_.as<P2PState>();
-        a.mode = 0; a.max_passes = 1; a.search_only = 1; a.dbg = 0; a.pose_from_search = 1;
-        a.pub = pub_.as<unsigned long long>(); a.nonce = ++launch_nonce_;
-        const int cap = upd_capacity_[extrinsic_est_ ? 1 : 0][0];
-        const int nq = scan_.q_end - scan_.q_begin;
-        const int workers = std::max(1, std::min(cap - 1, (nq + UPD_THREADS - 1) / UPD_THREADS));
-        cudaError_t e = launch_upd(workers, false, a, upd_pair(nq));
+        UpdArgs a = upd_args(1, 0, 1);
+        a.dbg = 0; a.pose_from_search = 1;
+        cudaError_t e = launch_plan(plan(UR_NEIGHBOURS, scan_.q_end - scan_.q_begin), a, stream());
         if (e != cudaSuccess) { scan_.q_begin = keep_b; scan_.q_end = keep_e; set_last_error("complete_neighbours: %s", cudaGetErrorString(e)); return FL_ERR_CUDA; }
     }
     scan_.q_begin = keep_b; scan_.q_end = keep_e;
@@ -1297,38 +1276,31 @@ UpdArgs Filter::upd_args(int max_passes, int mode, int search_only) {
 
 int Filter::launch_update(int max_passes, int mode, int search_only, cudaStream_t st) {
     FL_CUDA(cudaSetDevice(map_->device()));
-    const int nq = scan_.q_end - scan_.q_begin;
-    const UpdArgs a = upd_args(max_passes, mode, search_only);
-    const int cap = upd_capacity_[extrinsic_est_ ? 1 : 0][0];
-    // every co-resident block works (a searching pass wants many warps in flight); small scans: at least 4 points per warp
-    // one thread per point: full warps (the search is bound by a thread's own chain of loads, not by the number of SMs)
-    int workers = mode == 3 ? 0 : std::min(cap - 1, (nq + UPD_THREADS - 1) / UPD_THREADS);
-    if (workers < 0) workers = 0;
-    const int pair = upd_pair(nq);
-    if (use_wave(workers, pair, mode)) {      // pair 2: the tiles fit the 512-thread grid, so workers == tiles (one each)
-        unsigned long long* rows = rows_.as<unsigned long long>();
-        FL_CUDA(extrinsic_est_ ? launch_pdl_smem(k_update_wave<true>, workers + 1, 2 * UPD_THREADS, sizeof(WavePoint), st, pdl_, a, rows)
-                               : launch_pdl_smem(k_update_wave<false>, workers + 1, 2 * UPD_THREADS, sizeof(WavePoint), st, pdl_, a, rows));
-        return FL_OK;
-    }
-    FL_CUDA(launch_upd(workers, pdl_, a, pair, st));
+    FL_CUDA(launch_plan(plan((UpdRoute)mode, scan_.q_end - scan_.q_begin), upd_args(max_passes, mode, search_only), st));
     return FL_OK;
 }
 
-// Two threads per point (k_update<EXTR, 2>) when the shard's tiles all fit the co-resident 512-thread grid, so the tiles, the
-// workers and their partial rows are exactly those of the one-thread form; a larger scan keeps one thread per point rather
-// than idle half its warps on the passes that do not search.  FASTLIO_B200_PAIR=1 forces one thread per point (A/B).
-int Filter::upd_pair(int nq) const {
-    if (const char* e = getenv("FASTLIO_B200_PAIR")) if (e[0] == '1') return 1;
-    const int tiles = (nq + UPD_THREADS - 1) / UPD_THREADS;
-    return tiles >= 1 && tiles <= upd_capacity_[extrinsic_est_ ? 1 : 0][1] - 1 ? 2 : 1;
+UpdPlan Filter::plan(UpdRoute r, int rows, int n_hyp) const {
+    const char* e = getenv("FASTLIO_B200_PAIR");
+    return plan_update(upd_caps_, r, rows, extrinsic_est_, e && e[0] == '1', n_hyp);
 }
-cudaError_t Filter::launch_upd(int workers, bool pdl, const UpdArgs& a, int pair, cudaStream_t st) {
-    const int block = pair * UPD_THREADS;
-    if (extrinsic_est_) return pair == 2 ? launch_pdl(k_update<true, 2>, workers + 1, block, st, pdl, a)
-                                         : launch_pdl(k_update<true, 1>, workers + 1, block, st, pdl, a);
-    return pair == 2 ? launch_pdl(k_update<false, 2>, workers + 1, block, st, pdl, a)
-                     : launch_pdl(k_update<false, 1>, workers + 1, block, st, pdl, a);
+
+template <bool E>
+static cudaError_t launch_upd_kernel(const UpdPlan& p, bool pdl, cudaStream_t st, const UpdArgs& a, const int* n, unsigned long long* rows, int log_stride) {
+    const dim3 grid((unsigned)p.grid_x, (unsigned)p.slots);
+    switch (p.kernel) {
+    case UK_UPDATE1: return launch_pdl(k_update<E, 1>, grid, p.block, st, pdl, a);
+    case UK_UPDATE2: return launch_pdl(k_update<E, 2>, grid, p.block, st, pdl, a);
+    case UK_N1: return launch_pdl(k_update_n<E, 1>, grid, p.block, st, pdl, a, n);
+    case UK_N2: return launch_pdl(k_update_n<E, 2>, grid, p.block, st, pdl, a, n);
+    case UK_WAVE: return launch_pdl_smem(k_update_wave<E>, grid, p.block, p.smem, st, pdl, a, rows);
+    case UK_N_WAVE: return launch_pdl_smem(k_update_n_wave<E>, grid, p.block, p.smem, st, pdl, a, n, rows);
+    case UK_BATCH: return launch_pdl(k_update_batch<E>, grid, p.block, st, pdl, a, log_stride);
+    default: return cudaErrorInvalidValue;
+    }
+}
+cudaError_t Filter::launch_plan(const UpdPlan& p, const UpdArgs& a, cudaStream_t st, const int* n, int log_stride) {
+    return (extrinsic_est_ ? launch_upd_kernel<true> : launch_upd_kernel<false>)(p, pdl_ && p.pdl, st, a, n, rows_.as<unsigned long long>(), log_stride);
 }
 
 int Filter::launch_search_only() {
@@ -1455,6 +1427,13 @@ int Filter::device_form_scope(const char* what, bool update) const {
     return FL_OK;
 }
 
+StateIn Filter::state_in_args(double R) const {
+    StateIn s;
+    for (int i = 0; i < NDOF; i++) s.limit[i] = limit_[i];
+    s.R = R; s.max_iter = max_iter_; s.extrinsic_est = extrinsic_est_;
+    return s;
+}
+
 int Filter::update_on_stream(const float* d_body, int nq, double* d_x26, double* d_P, double R, int* d_status2, cudaStream_t st) {
     const int dev = map_->device();
     if (nq < 0 || (nq > 0 && !device_ptr(d_body, dev, 16)) || !device_ptr(d_x26, dev, 8) || !device_ptr(d_P, dev, 8) ||
@@ -1474,10 +1453,8 @@ int Filter::update_on_stream(const float* d_body, int nq, double* d_x26, double*
     FL_CHECK(bind_scan(body_.as<float4>(), nq));             // within capacity: binds, allocates nothing
     stream_bound_ = true;
     if (nq > 0) FL_CUDA(cudaMemcpyAsync(body_.ptr, d_body, sizeof(float4) * (size_t)nq, cudaMemcpyDeviceToDevice, st));
-    StateIn s;
-    for (int i = 0; i < NDOF; i++) s.limit[i] = limit_[i];
-    s.R = R; s.max_iter = max_iter_; s.extrinsic_est = extrinsic_est_;
-    k_state_in<<<1, STATE_THREADS, 0, st>>>(ctl_.as<FilterCtl>(), pub_.as<unsigned long long>(), h_ctl_, d_x26, d_P, s, d_bind_.as<int>(), nq);
+    k_state_in<<<1, STATE_THREADS, 0, st>>>(ctl_.as<FilterCtl>(), pub_.as<unsigned long long>(), h_ctl_, d_x26, d_P, state_in_args(R),
+                                            d_bind_.as<int>(), nq);
     FL_CUDA(cudaGetLastError());
     // run_passes's fused single-rank branch, on `st`
     neighbours_complete_ = false;
@@ -1510,49 +1487,31 @@ int Filter::update_scan_on_stream(const float4* d_body, const int* d_n, int n_ma
     stream_bound_ = true;
     // the count is the filter's own from here on (later host-form calls read it back)
     k_count_in<<<1, 1, 0, st>>>(d_n, n_max, d_bind_.as<int>());
-    StateIn s;
-    for (int i = 0; i < NDOF; i++) s.limit[i] = limit_[i];
-    s.R = R; s.max_iter = max_iter_; s.extrinsic_est = extrinsic_est_;
-    k_state_in<<<1, STATE_THREADS, 0, st>>>(ctl_.as<FilterCtl>(), pub_.as<unsigned long long>(), h_ctl_, d_x26, d_P, s, nullptr, 0);
+    k_state_in<<<1, STATE_THREADS, 0, st>>>(ctl_.as<FilterCtl>(), pub_.as<unsigned long long>(), h_ctl_, d_x26, d_P, state_in_args(R), nullptr, 0);
     FL_CUDA(cudaGetLastError());
     neighbours_complete_ = false;
     // k_update_n over the row bound: the workers of the host form at n_max rows (tile t to block t, as at the count), one or
     // two threads per point as the host form picks at n_max -- both forms give the same bytes
-    const int e = extrinsic_est_ ? 1 : 0;
-    const int tiles = (n_max + UPD_THREADS - 1) / UPD_THREADS;
-    const int pair = upd_pair(n_max) == 2 && tiles <= upd_n_capacity_[e][1] - 1 ? 2 : 1;
-    const int workers = std::max(0, std::min(upd_n_capacity_[e][0] - 1, tiles));
-    const UpdArgs a = upd_args(max_iter_ + 1, 0, 0);
-    const int* n = d_bind_.as<int>();
-    const int block = pair * UPD_THREADS;
-    cudaError_t rc;
-    if (pair == 2 && workers + 1 <= wave_n_capacity_[e]) {
-        unsigned long long* rows = rows_.as<unsigned long long>();
-        rc = e ? launch_pdl_smem(k_update_n_wave<true>, workers + 1, block, sizeof(WavePoint), st, pdl_, a, n, rows)
-               : launch_pdl_smem(k_update_n_wave<false>, workers + 1, block, sizeof(WavePoint), st, pdl_, a, n, rows);
-    } else if (e) rc = pair == 2 ? launch_pdl(k_update_n<true, 2>, workers + 1, block, st, pdl_, a, n) : launch_pdl(k_update_n<true, 1>, workers + 1, block, st, pdl_, a, n);
-    else rc = pair == 2 ? launch_pdl(k_update_n<false, 2>, workers + 1, block, st, pdl_, a, n) : launch_pdl(k_update_n<false, 1>, workers + 1, block, st, pdl_, a, n);
-    FL_CUDA(rc);
+    FL_CUDA(launch_plan(plan(UR_DEVICE_COUNT, n_max), upd_args(max_iter_ + 1, 0, 0), st, d_bind_.as<int>()));
     launches_ = 1;
     k_state_out<<<1, STATE_THREADS, 0, st>>>(ctl_.as<FilterCtl>(), d_x26, d_P, d_status2);
     return map_->query_end(st, joined);
 }
 
 // ----------------------------------------------------------------------------- batched update (fl_filter_update_batch_device)
-// Each hypothesis runs with the single form's workers (launch_update: min(cap - 1, tiles)), so its tiles, partial rows and sums
-// are those of fl_filter_update_device; a wave holds as many hypotheses as fit the co-resident k_update_batch grid.
+// Each hypothesis runs with the single form's workers, so its tiles, partial rows and sums are those of fl_filter_update_device;
+// a wave holds as many hypotheses as fit the co-resident k_update_batch grid (plan_update, UR_BATCH).
 int Filter::batch_plan(int nq, int n_hyp, int* workers, int* slots, int* waves) const {
     if (nq < 0 || n_hyp < 0) { set_last_error("batch_plan: nq and n_hyp must be >= 0"); return FL_ERR_ARG; }
-    const int e = extrinsic_est_ ? 1 : 0;
-    const int w = std::max(0, std::min(upd_capacity_[e][0] - 1, (nq + UPD_THREADS - 1) / UPD_THREADS));
-    if (w + 1 > batch_cap_[e]) {
-        set_last_error("batch_plan: a hypothesis takes %d blocks, %d k_update_batch blocks are co-resident", w + 1, batch_cap_[e]);
+    const UpdPlan p = plan(UR_BATCH, nq, n_hyp);
+    if (!p.slots) {
+        set_last_error("batch_plan: a hypothesis takes %d blocks, %d k_update_batch blocks are co-resident", p.grid_x,
+                       upd_caps_.blocks[UK_BATCH][extrinsic_est_ ? 1 : 0]);
         return FL_ERR_CAPACITY;
     }
-    const int s = batch_cap_[e] / (w + 1);
-    *workers = w;
-    *slots = s;
-    *waves = (n_hyp + s - 1) / s;
+    *workers = p.workers;
+    *slots = p.slots;
+    *waves = p.waves;
     return FL_OK;
 }
 
@@ -1568,12 +1527,14 @@ int Filter::reserve_batch(int nq_max) {
     size_t rows = 1;
     int cap = 1;
     for (int e = 0; e < 2; e++) {
-        const int wmax = std::max(0, std::min(upd_capacity_[e][0] - 1, (nq_max + UPD_THREADS - 1) / UPD_THREADS));
-        for (int w = 0; w <= wmax && w + 1 <= batch_cap_[e]; w++) {
+        const int wmax = plan_update(upd_caps_, UR_BATCH, nq_max, e, false).workers;
+        for (int w = 0; w <= wmax; w++) {
             const int nq_hi = w == wmax ? nq_max : std::min(nq_max, UPD_THREADS * w);
-            rows = std::max(rows, (size_t)(batch_cap_[e] / (w + 1)) * (size_t)nq_hi);
+            const UpdPlan p = plan_update(upd_caps_, UR_BATCH, nq_hi, e, false);     // w workers
+            if (!p.slots) break;
+            rows = std::max(rows, (size_t)p.slots * (size_t)nq_hi);
         }
-        cap = std::max(cap, batch_cap_[e]);
+        cap = std::max(cap, upd_caps_.blocks[UK_BATCH][e]);
     }
     FL_CHECK(b_body_.reserve(sizeof(float4) * (size_t)std::max(1, nq_max)));
     FL_CHECK(b_ctl_.reserve(sizeof(FilterCtl) * (size_t)cap));
@@ -1608,8 +1569,9 @@ int Filter::update_batch_on_stream(const float* d_body, int nq, int n_hyp, doubl
         return FL_ERR_CAPACITY;
     }
     int workers = 0, slots = 0, waves = 0;
-    FL_CHECK(batch_plan(nq, n_hyp, &workers, &slots, &waves));
+    FL_CHECK(batch_plan(nq, n_hyp, &workers, &slots, &waves));      // FL_ERR_CAPACITY where one hypothesis does not fit
     if (n_hyp == 0) return FL_OK;
+    UpdPlan p = plan(UR_BATCH, nq, n_hyp);
     FL_CUDA(cudaSetDevice(dev));
     bool joined = false;
     FL_CHECK(map_->query_begin(st, &joined));
@@ -1620,9 +1582,7 @@ int Filter::update_batch_on_stream(const float* d_body, int nq, int n_hyp, doubl
     sc.nearest = b_nearest_.as<float4>(); sc.nearest_cnt = b_nearest_cnt_.as<int>(); sc.selected = b_selected_.as<unsigned char>();
     sc.plane = b_plane_.as<float4>(); sc.srange = b_srange_.as<double>();
     sc.q_begin = 0; sc.q_end = sc.Q = nq;
-    StateIn s;
-    for (int i = 0; i < NDOF; i++) s.limit[i] = limit_[i];
-    s.R = R; s.max_iter = max_iter_; s.extrinsic_est = extrinsic_est_;
+    const StateIn s = state_in_args(R);
     const int log_stride = max_iter_ + 1;
     FilterCtl* ctl = b_ctl_.as<FilterCtl>();
     unsigned long long* pub = b_pub_.as<unsigned long long>();
@@ -1635,9 +1595,8 @@ int Filter::update_batch_on_stream(const float* d_body, int nq, int n_hyp, doubl
         UpdArgs a = upd_args(max_iter_ + 1, 0, 0);    // the map view, the search A/B switch and a fresh nonce, as the single form
         a.sc = sc; a.ctl = ctl; a.partials = b_partials_.as<double>(); a.pub = pub;
         a.logs = d_logs ? d_logs + (size_t)h0 * log_stride : nullptr;
-        const dim3 grid((unsigned)(workers + 1), (unsigned)n);
-        FL_CUDA(extrinsic_est_ ? launch_pdl(k_update_batch<true>, grid, UPD_THREADS, st, pdl_, a, log_stride)
-                               : launch_pdl(k_update_batch<false>, grid, UPD_THREADS, st, pdl_, a, log_stride));
+        p.slots = n;                                  // grid.y: the hypotheses of this wave (the last may be partial)
+        FL_CUDA(launch_plan(p, a, st, nullptr, log_stride));
         k_batch_state_out<<<n, STATE_THREADS, 0, st>>>(ctl, x, P, d_status2 + 2 * (size_t)h0);
         FL_CUDA(cudaGetLastError());
     }

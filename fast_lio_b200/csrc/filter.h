@@ -5,6 +5,7 @@
 #pragma once
 #include "lie.cuh"
 #include "map.h"
+#include "upd_plan.h"
 
 namespace fl {
 
@@ -55,6 +56,7 @@ struct ScanView {
 
 struct NcclApi;
 struct UpdArgs;
+struct StateIn;
 
 // Peer-memory exchange of the per-pass sums (fused into k_residual's solver block): every rank owns a
 // mailbox [2 epoch parities][nranks][96] values, each two epoch-tagged 8-byte words; peers store into it over NVLink.
@@ -171,12 +173,13 @@ private:
     bool fused_ = true;
     DeviceBuffer pub_;                 // k_update's publication block
     unsigned launch_nonce_ = 0;
-    int upd_capacity_[2][2] = {{0, 0}, {0, 0}};   // co-resident k_update<EXTR, PAIR> blocks on this device, [EXTR][PAIR - 1]
+    UpdCaps upd_caps_ = {};                      // co-resident blocks of every update kernel on this device (init)
     int launch_update(int max_passes, int mode, int search_only) { return launch_update(max_passes, mode, search_only, stream()); }
     int launch_update(int max_passes, int mode, int search_only, cudaStream_t st);
-    int upd_pair(int nq) const;                   // 2: the shard's tiles fit the 512-thread grid (two threads per point), else 1
-    cudaError_t launch_upd(int workers, bool pdl, const UpdArgs& a, int pair) { return launch_upd(workers, pdl, a, pair, stream()); }
-    cudaError_t launch_upd(int workers, bool pdl, const UpdArgs& a, int pair, cudaStream_t st);
+    UpdPlan plan(UpdRoute r, int rows, int n_hyp = 0) const;       // plan_update here, FASTLIO_B200_PAIR read at every plan
+    // the only launch of an update kernel: n is the count of the _n forms, log_stride k_update_batch's, grid.y = p.slots
+    cudaError_t launch_plan(const UpdPlan& p, const UpdArgs& a, cudaStream_t st, const int* n = nullptr, int log_stride = 0);
+    StateIn state_in_args(double R) const;       // k_state_in / k_batch_state_in's setup besides the caller's x26 / P
     // the device forms cover a single-rank filter (and the update a fused, solver-1 one); FL_ERR_STATE otherwise
     int device_form_scope(const char* what, bool update) const;
     // the UpdArgs of a launch of k_update / k_update_n
@@ -192,13 +195,8 @@ private:
     // once a device form has run (stream_bound_), by the host forms' binds; read_binding restores it for the host forms
     bool stream_bound_ = false;
     DeviceBuffer d_bind_;
-    int upd_n_capacity_[2][2] = {{0, 0}, {0, 0}};   // co-resident k_update_n blocks, capped at k_update's (the same tiles per block)
-    // k_update_wave / k_update_n_wave: co-resident blocks [EXTR] and the tagged partial rows (one per worker block)
-    int wave_capacity_[2] = {0, 0}, wave_n_capacity_[2] = {0, 0};
-    DeviceBuffer rows_;
-    bool use_wave(int workers, int pair, int mode) const { return mode == 0 && pair == 2 && workers + 1 <= wave_capacity_[extrinsic_est_ ? 1 : 0]; }
+    DeviceBuffer rows_;                // k_update_wave / k_update_n_wave: the tagged partial rows (one per worker block)
     int read_binding();
-    int batch_cap_[2] = {0, 0};        // co-resident k_update_batch<EXTR> blocks on this device
     int batch_nq_max_ = -1;            // the nq_max reserve_batch sized the batch buffers for (-1: not yet)
     DeviceBuffer b_body_, b_ctl_, b_pub_, b_partials_, b_nearest_, b_nearest_cnt_, b_selected_, b_plane_, b_srange_;
     int launches_ = 0;

@@ -851,7 +851,7 @@ __global__ void __launch_bounds__(UPD_THREADS, 2) k_update_batch(UpdArgs a, int 
 }
 
 // ============================================================================= one tile per worker block: k_update_wave
-// The single-GPU update (mode 0) when every tile of the scan has a worker block of its own, which is exactly when Filter::upd_pair
+// The single-GPU update (mode 0) when every tile of the scan has a worker block of its own, which is exactly when plan_update
 // picks two threads per point: the 512-thread block, the paired search and the tiles of k_update<EXTR, 2>, so the same bytes.
 // Thread t < 256 owns point tile + t for the whole launch, which removes three things from every pass's chain:
 //   * the point's state stays in shared memory (WavePoint): the body point, sqrt(|p_body|), the plane and the selected flag; a
