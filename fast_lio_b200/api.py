@@ -49,6 +49,44 @@ class FastLioError(RuntimeError):
     pass
 
 
+# ---- sensor preprocessing: the reference's raw point structs as numpy dtypes (the default layouts of Preprocess)
+LIDAR_AVIA, LIDAR_VELO16, LIDAR_OUST64, LIDAR_MARSIM = 1, 2, 3, 4          # enum LID_TYPE, preprocess.h:16
+TIME_SEC, TIME_MS, TIME_US, TIME_NS = 0, 1, 2, 3                           # enum TIME_UNIT, preprocess.h:17
+# livox_ros_driver::CustomPoint: 20 bytes
+CUSTOM_POINT = np.dtype({"names": ["offset_time", "x", "y", "z", "reflectivity", "tag", "line"],
+                         "formats": ["<u4", "<f4", "<f4", "<f4", "u1", "u1", "u1"],
+                         "offsets": [0, 4, 8, 12, 16, 17, 18], "itemsize": 20})
+# velodyne_ros::Point (preprocess.h:41-49): PCL_ADD_POINT4D, 16-byte aligned, 32 bytes
+VELODYNE_POINT = np.dtype({"names": ["x", "y", "z", "intensity", "time", "ring"],
+                           "formats": ["<f4", "<f4", "<f4", "<f4", "<f4", "<u2"],
+                           "offsets": [0, 4, 8, 16, 20, 24], "itemsize": 32})
+# ouster_ros::Point (preprocess.h:59-84): 48 bytes
+OUSTER_POINT = np.dtype({"names": ["x", "y", "z", "intensity", "t", "reflectivity", "ring", "ambient", "range"],
+                         "formats": ["<f4", "<f4", "<f4", "<f4", "<u4", "<u2", "u1", "<u2", "<u4"],
+                         "offsets": [0, 4, 8, 16, 20, 24, 26, 28, 32], "itemsize": 48})
+# pcl::PointXYZI (MARSIM): 32 bytes
+POINT_XYZI = np.dtype({"names": ["x", "y", "z", "intensity"], "formats": ["<f4"] * 4, "offsets": [0, 4, 8, 16], "itemsize": 32})
+DEFAULT_LAYOUT = {LIDAR_AVIA: CUSTOM_POINT, LIDAR_VELO16: VELODYNE_POINT, LIDAR_OUST64: OUSTER_POINT, LIDAR_MARSIM: POINT_XYZI}
+# fl_preprocess_params_t's offsets, in order, and the struct member each one is in the reference's point type
+OFFSET_FIELDS = ("x", "y", "z", "intensity", "time", "ring", "tag", "line")
+_FIELD_NAMES = {LIDAR_AVIA: {"intensity": "reflectivity", "time": "offset_time"}, LIDAR_OUST64: {"time": "t"}}
+
+
+def layout_offsets(dtype: np.dtype, lidar_type: int) -> list[int]:
+    """The 8 byte offsets (x, y, z, intensity, time, ring, tag, line) of a structured dtype for `lidar_type`, -1 where the dtype
+    has no such field; Avia's intensity is `reflectivity` and its time `offset_time`, Ouster's time is `t`."""
+    names = _FIELD_NAMES.get(lidar_type, {})
+    fields = dtype.fields or {}
+    return [int(fields[names.get(f, f)][1]) if names.get(f, f) in fields else -1 for f in OFFSET_FIELDS]
+
+
+class PreprocessParams(C.Structure):
+    """fl_preprocess_params_t"""
+    _fields_ = [("lidar_type", C.c_int), ("n_scans", C.c_int), ("scan_rate", C.c_int), ("time_unit", C.c_int),
+                ("point_filter_num", C.c_int), ("blind", C.c_double), ("point_step", C.c_int)] + \
+               [("off_" + f, C.c_int) for f in OFFSET_FIELDS]
+
+
 _lib = None
 
 # every symbol include/fastlio_b200.h declares (tests check that the library exports all of them)
@@ -71,6 +109,7 @@ SYMBOLS = [
     "fl_scan_reserve", "fl_scan_upload_device", "fl_scan_undistort_device", "fl_scan_voxel_downsample_device",
     "fl_filter_update_scan_device", "fl_map_delete_boxes_async", "fl_localmap_segment_device",
     "fl_filter_reserve_batch", "fl_filter_batch_plan", "fl_filter_update_batch_device",
+    "fl_preprocess_create", "fl_preprocess_destroy", "fl_preprocess_device", "fl_preprocess",
 ]
 
 
@@ -165,6 +204,10 @@ def load():
     L.fl_localmap_segment.argtypes = [C.c_void_p, C.c_void_p, _f64p, _f32p, C.POINTER(C.c_int)]
     L.fl_localmap_get.argtypes = [C.c_void_p, _f32p]
     L.fl_localmap_segment_device.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp]
+    L.fl_preprocess_create.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.POINTER(PreprocessParams), C.c_int]
+    L.fl_preprocess_destroy.argtypes = [_vp]
+    L.fl_preprocess_device.argtypes = [_vp, _vp, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp]
+    L.fl_preprocess.argtypes = [_vp, _vp, C.c_int, _f32p, _f32p, C.c_int, C.POINTER(C.c_float)]
     L.fl_comm_unique_id.argtypes = [C.c_char_p]
     L.fl_filter_comm_init.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_char_p]
     L.fl_filter_set_shard.argtypes = [C.c_void_p, C.c_int, C.c_int]
@@ -833,6 +876,89 @@ class LocalMap:
         b = np.zeros(6, dtype=np.float32)
         _check(self._L.fl_localmap_get(self.h, b))
         return b
+
+
+class Preprocess:
+    """Preprocess::process (src/preprocess.cpp) with feature extraction off, on the device: one raw LiDAR frame -> pl_surf, the
+    (xyzi, offset time in ms) rows fl_scan_upload[_device] take.  layout: the raw points' structured numpy dtype (default: the
+    reference's struct for lidar_type, DEFAULT_LAYOUT); its itemsize is point_step and its fields give the offsets."""
+
+    def __init__(self, device: int, lidar_type: int, n_scans: int, scan_rate: int = 10, time_unit: int = TIME_US,
+                 point_filter_num: int = 1, blind: float = 0.01, layout: np.dtype | None = None, n_raw_max: int = 65536):
+        self._L = load()
+        self.device = device
+        self.layout = np.dtype(DEFAULT_LAYOUT[lidar_type] if layout is None else layout)
+        self.n_raw_max = n_raw_max
+        off = layout_offsets(self.layout, lidar_type)
+        p = PreprocessParams(lidar_type, n_scans, scan_rate, time_unit, point_filter_num, blind, self.layout.itemsize, *off)
+        h = C.c_void_p()
+        _check(self._L.fl_preprocess_create(C.byref(h), device, C.byref(p), n_raw_max))
+        self.h = h
+
+    def close(self):
+        if getattr(self, "h", None):
+            self._L.fl_preprocess_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _raw_bytes(self, raw) -> np.ndarray:
+        raw = np.ascontiguousarray(raw)
+        if raw.dtype.fields is not None:
+            if raw.dtype.itemsize != self.layout.itemsize:
+                raise ValueError(f"raw: {raw.dtype.itemsize}-byte points, the layout has {self.layout.itemsize}")
+            return raw.reshape(-1).view(np.uint8)
+        return np.ascontiguousarray(raw, dtype=np.uint8).reshape(-1)
+
+    def process(self, raw):
+        """The host form (fl_preprocess): raw, a structured array of the layout (or its bytes).  Returns (xyzi (m, 4) float32,
+        offset_ms (m,) float32, last_ms), last_ms = pl_surf.points.back().curvature (0.0 when nothing is kept)."""
+        buf = self._raw_bytes(raw)
+        n = len(buf) // self.layout.itemsize
+        xyzi = np.empty((max(n, 1), 4), dtype=np.float32)
+        ms = np.empty(max(n, 1), dtype=np.float32)
+        last = C.c_float(0.0)
+        m = _check(self._L.fl_preprocess(self.h, buf.ctypes.data if n else None, n, xyzi, ms, n, C.byref(last)))
+        return xyzi[:m].copy(), ms[:m].copy(), last.value
+
+    def process_device(self, raw, n=None, n_max: int | None = None, xyzi=None, offset_ms=None, out2=None, last_ms=None):
+        """fl_preprocess_device on torch.cuda.current_stream(): raw a uint8 CUDA tensor (>= n_max * point_step bytes; (rows,
+        point_step) or flat), n an int32 CUDA tensor (1,) (None: all rows, copied from the host, so pass a tensor when capturing a
+        CUDA graph), n_max defaults to the number of rows.  The outputs (allocated when not given, n_max rows): xyzi (n_max, 4)
+        float32, offset_ms (n_max,) float32, out2 int32 (2,) = (kept, dropped rings), last_ms float32 (1,).  Returns them."""
+        import torch
+        dev = f"cuda:{self.device}"
+        step = self.layout.itemsize
+        if not isinstance(raw, torch.Tensor) or raw.dtype != torch.uint8 or not raw.is_contiguous() or raw.device != torch.device(dev):
+            raise TypeError(f"raw: expected a contiguous uint8 tensor on {dev}")
+        rows = raw.numel() // step
+        n_max = rows if n_max is None else n_max
+        if rows < n_max:
+            raise ValueError(f"raw: {rows} rows, fewer than n_max = {n_max}")
+        if n is None:
+            if torch.cuda.is_current_stream_capturing():
+                raise ValueError("n: pass an int32 CUDA tensor while capturing a CUDA graph")
+            n = torch.tensor([rows], dtype=torch.int32, device=dev)
+        xyzi = torch.empty((n_max, 4), dtype=torch.float32, device=dev) if xyzi is None else xyzi
+        offset_ms = torch.empty(n_max, dtype=torch.float32, device=dev) if offset_ms is None else offset_ms
+        out2 = torch.empty(2, dtype=torch.int32, device=dev) if out2 is None else out2
+        last_ms = torch.empty(1, dtype=torch.float32, device=dev) if last_ms is None else last_ms
+        for name, t, dt in (("n", n, torch.int32), ("xyzi", xyzi, torch.float32), ("offset_ms", offset_ms, torch.float32),
+                            ("out2", out2, torch.int32), ("last_ms", last_ms, torch.float32)):
+            if not isinstance(t, torch.Tensor) or t.dtype != dt or not t.is_contiguous() or t.device != torch.device(dev):
+                raise TypeError(f"{name}: expected a contiguous {dt} tensor on {dev}")
+        if xyzi.numel() < 4 * n_max or offset_ms.numel() < n_max or out2.numel() < 2 or n.numel() < 1 or last_ms.numel() < 1:
+            raise ValueError("an output tensor is smaller than n_max rows")
+        self._n = n                                    # kept alive until the stream has read it
+        stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        _check(self._L.fl_preprocess_device(self.h, raw.data_ptr() if n_max else None, n.data_ptr(), n_max,
+                                            xyzi.data_ptr() if n_max else None, offset_ms.data_ptr() if n_max else None,
+                                            out2.data_ptr(), last_ms.data_ptr(), stream))
+        return xyzi, offset_ms, out2, last_ms
 
 
 def host_register(arr: np.ndarray):

@@ -8,6 +8,7 @@
 
 #include "../../include/fastlio_b200.h"
 #include "filter.h"
+#include "preprocess.h"
 #include "scan.h"
 
 namespace fl {
@@ -570,6 +571,82 @@ int fl_localmap_segment_device(fl_localmap_t* l, fl_map_t* map, const double* x2
     // stays alive as long as the handle
     if (!l->map && l->cube.device_map()) { l->map = map; map_retain(map); }
     return rc;
+}
+
+// ------------------------------------------------------------------------------------ sensor preprocessing
+struct fl_preprocessor {
+    fl::Preprocessor* impl;
+    std::mutex mu;
+};
+
+int fl_preprocess_create(fl_preprocess_t** out, int device, const fl_preprocess_params_t* pp, int n_raw_max) {
+    if (!out) return FL_ERR_ARG;
+    *out = nullptr;
+    if (!pp) { fl::set_last_error("fl_preprocess_create: null parameters"); return FL_ERR_ARG; }
+    const fl_preprocess_params_t& p = *pp;
+    if (p.lidar_type < FL_LIDAR_AVIA || p.lidar_type > FL_LIDAR_MARSIM || p.time_unit < 0 || p.time_unit > 3 || p.n_scans < 1 ||
+        p.n_scans > 128 || p.point_filter_num < 1 || p.point_step < 1 || n_raw_max < 0 ||
+        (p.lidar_type == FL_LIDAR_VELO16 && p.scan_rate < 1)) {
+        fl::set_last_error("fl_preprocess_create: bad lidar_type %d, time_unit %d, n_scans %d, scan_rate %d, point_filter_num %d, "
+                           "point_step %d or n_raw_max %d", p.lidar_type, p.time_unit, p.n_scans, p.scan_rate, p.point_filter_num,
+                           p.point_step, n_raw_max);
+        return FL_ERR_ARG;
+    }
+    fl::PpParams q{};
+    q.type = p.lidar_type;
+    q.n_scans = p.n_scans;
+    q.pfn = p.point_filter_num;
+    q.step = p.point_step;
+    const int offs[8] = {p.off_x, p.off_y, p.off_z, p.off_intensity, p.off_time, p.off_ring, p.off_tag, p.off_line};
+    // the bytes each field occupies for this type (0: the type does not read it)
+    const int avia[8] = {4, 4, 4, 1, 4, 0, 1, 1}, velo[8] = {4, 4, 4, 4, 4, 2, 0, 0}, oust[8] = {4, 4, 4, 4, 4, 0, 0, 0},
+              sim[8] = {4, 4, 4, 4, 0, 0, 0, 0};
+    const int* size = p.lidar_type == FL_LIDAR_AVIA ? avia : p.lidar_type == FL_LIDAR_VELO16 ? velo : p.lidar_type == FL_LIDAR_OUST64 ? oust : sim;
+    for (int k = 0; k < 8; k++) {
+        q.off[k] = size[k] ? offs[k] : -1;
+        if (size[k] && (offs[k] < -1 || (offs[k] >= 0 && offs[k] + size[k] > p.point_step))) {
+            fl::set_last_error("fl_preprocess_create: field %d at offset %d does not fit point_step %d", k, offs[k], p.point_step);
+            return FL_ERR_ARG;
+        }
+    }
+    static const float scale[4] = {1.e3f, 1.f, 1.e-3f, 1.e-6f};     // preprocess.cpp:52-69
+    q.scale = scale[p.time_unit];
+    q.bb = p.blind * p.blind;
+    q.omega_l = 0.361 * p.scan_rate;
+    q.key_bits = 1;
+    while ((1 << q.key_bits) <= p.n_scans) q.key_bits++;
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) {
+        cudaGetLastError();
+        fl::set_last_error("fl_preprocess_create: no CUDA device %d", device);
+        return FL_ERR_ARG;
+    }
+    fl_preprocess_t* h = new (std::nothrow) fl_preprocess_t();
+    if (!h) return FL_ERR_CAPACITY;
+    h->impl = new (std::nothrow) fl::Preprocessor(device, q, n_raw_max);
+    if (!h->impl) { delete h; return FL_ERR_CAPACITY; }
+    const int rc = h->impl->init();
+    if (rc != FL_OK) { delete h->impl; delete h; return rc; }
+    *out = h;
+    return FL_OK;
+}
+int fl_preprocess_destroy(fl_preprocess_t* h) {
+    if (!h) return FL_OK;
+    delete h->impl;
+    delete h;
+    return FL_OK;
+}
+int fl_preprocess_device(fl_preprocess_t* h, const void* raw_device, const int* n_raw_device, int n_raw_max, float* xyzi_out_device,
+                         float* offset_ms_out_device, int* out2_device, float* last_ms_device, void* stream) {
+    if (!h || !h->impl) { fl::set_last_error("null preprocess handle"); return FL_ERR_ARG; }
+    std::lock_guard<std::mutex> lk(h->mu);
+    return h->impl->run_device(raw_device, n_raw_device, n_raw_max, xyzi_out_device, offset_ms_out_device, out2_device, last_ms_device,
+                               static_cast<cudaStream_t>(stream));
+}
+int fl_preprocess(fl_preprocess_t* h, const void* raw_host, int n_raw, float* xyzi_out, float* offset_ms_out, int cap, float* last_ms) {
+    if (!h || !h->impl) { fl::set_last_error("null preprocess handle"); return FL_ERR_ARG; }
+    std::lock_guard<std::mutex> lk(h->mu);
+    return h->impl->run_host(raw_host, n_raw, xyzi_out, offset_ms_out, cap, last_ms);
 }
 
 // ------------------------------------------------------------------------------------ multi-GPU

@@ -449,3 +449,103 @@ def make_problem(name_or_cfg, extrinsic_est_en: int = 0) -> Problem:
     scan = make_scan(scene, cfg.n_scan, xt, seed=cfg.seed + 1)
     xp, P = make_prior(xt, seed=cfg.seed + 2)
     return Problem(cfg, map_pts, scan, xt, xp, P, scene, extrinsic_est_en=extrinsic_est_en)
+
+
+# ---------------------------------------------------------------------------------------------------- raw sensor frames
+def _edge_rows(blind: float):
+    """Points inside the blind range and exactly on it (blind**2 in float, for blinds whose square is exact), and the origin."""
+    b = np.float32(blind)
+    return np.array([[b, 0, 0], [0, b, 0], [0, 0, -b], [b / 2, 0, 0], [0, 0, 0], [b * np.float32(1.001), 0, 0]], np.float32)
+
+
+def raw_frame(kind: str, seed: int = 0, blind: float = 0.5, n: int | None = None, rings: int | None = None,
+              cols: int | None = None, yaw0_deg: float = 37.0, times: bool = True):
+    """A deterministic raw LiDAR frame as its driver publishes it: a structured array of the reference's point struct
+    (fast_lio_b200.api.DEFAULT_LAYOUT).  Every kind carries points inside `blind`, exactly on it and at the origin.
+
+    avia      Livox rosette, n points (default 24 000) of 6 lines over 100 ms (offset_time in ns): about 5 % bad tags
+              (0x20 / 0x30), 3 % lines 6-7 (>= N_SCANS 6), 3 % repeats of the previous point.
+    velodyne  rings x cols (default 32 x 1800) in firing order (all rings of a column, in a fixed interleaved ring order), a
+              sweep from yaw0_deg clockwise through +-180 deg; `time` in us when `times`, else all 0 (the yaw path).
+    ouster    rings x cols (default 64 x 1024), ring-major, t in ns up to 1e8 (above 2**24).
+    marsim    n points (default 20 000) in a 60 m box, intensity in [0, 255].
+    """
+    from .api import CUSTOM_POINT, OUSTER_POINT, POINT_XYZI, VELODYNE_POINT
+    rng = np.random.default_rng(seed)
+    edge = _edge_rows(blind)
+    if kind == "avia":
+        n = 24000 if n is None else n
+        k = np.arange(n)
+        th = 2 * np.pi * k / 2400.0
+        rho = 0.35 * np.abs(np.sin(5.0 * th * 1.013))                      # rosette in the tangent plane
+        dist = rng.uniform(3.0, 40.0, n)
+        a = np.zeros(n, CUSTOM_POINT)
+        a["x"] = dist
+        a["y"] = dist * rho * np.cos(th)
+        a["z"] = dist * rho * np.sin(th)
+        a["offset_time"] = (k * (100_000_000 // max(n, 1))).astype(np.uint32)
+        a["reflectivity"] = rng.integers(0, 256, n)
+        a["line"] = k % 6
+        a["tag"] = rng.choice(np.array([0x00, 0x10, 0x01, 0x12], np.uint8), n)
+        bad = rng.random(n) < 0.05
+        a["tag"][bad] = rng.choice(np.array([0x20, 0x30, 0x21], np.uint8), bad.sum())
+        a["line"][rng.random(n) < 0.03] = rng.integers(6, 8)
+        rep = np.nonzero(rng.random(n) < 0.03)[0]
+        rep = rep[rep > 0]
+        for f in ("x", "y", "z"):
+            a[f][rep] = a[f][rep - 1]
+        where = rng.choice(np.arange(1, max(n, 2)), min(len(edge), max(n - 1, 0)), replace=False) if n > 1 else []
+        for j, w in enumerate(where):
+            a["x"][w], a["y"][w], a["z"][w] = edge[j]
+        return a
+    if kind == "velodyne":
+        rings = 32 if rings is None else rings
+        cols = 1800 if cols is None else cols
+        order = (np.arange(rings) * 7) % rings if rings % 7 else np.arange(rings)[::-1]   # interleaved firing order
+        col = np.repeat(np.arange(cols), rings)
+        ring = np.tile(order, cols).astype(np.uint16)
+        yaw = np.deg2rad(yaw0_deg - col * (360.0 / cols) + rng.normal(0, 0.01, col.size))
+        elev = np.deg2rad(-15.0 + 30.0 * ring / max(rings - 1, 1))
+        dist = rng.uniform(1.0, 60.0, col.size)
+        a = np.zeros(col.size, VELODYNE_POINT)
+        a["x"] = dist * np.cos(elev) * np.cos(yaw)
+        a["y"] = dist * np.cos(elev) * np.sin(yaw)
+        a["z"] = dist * np.sin(elev)
+        a["intensity"] = rng.uniform(0, 255, col.size)
+        a["ring"] = ring
+        a["time"] = (col * (100000.0 / cols)).astype(np.float32) if times else 0.0
+        where = rng.choice(np.arange(rings, col.size), len(edge), replace=False) if col.size > rings + len(edge) else []
+        for j, w in enumerate(where):
+            a["x"][w], a["y"][w], a["z"][w] = edge[j]
+        return a
+    if kind == "ouster":
+        rings = 64 if rings is None else rings
+        cols = 1024 if cols is None else cols
+        ring = np.repeat(np.arange(rings), cols)
+        col = np.tile(np.arange(cols), rings)
+        yaw = 2 * np.pi * col / cols
+        elev = np.deg2rad(-16.6 + 33.2 * ring / max(rings - 1, 1))
+        dist = rng.uniform(0.2, 80.0, col.size)
+        a = np.zeros(col.size, OUSTER_POINT)
+        a["x"] = dist * np.cos(elev) * np.cos(yaw)
+        a["y"] = dist * np.cos(elev) * np.sin(yaw)
+        a["z"] = dist * np.sin(elev)
+        a["intensity"] = rng.uniform(0, 4096, col.size)
+        a["t"] = (col * (100_000_000 // cols) + rng.integers(0, 97, col.size)).astype(np.uint32)
+        a["ring"] = ring
+        a["range"] = (dist * 1000).astype(np.uint32)
+        where = rng.choice(col.size, min(len(edge), col.size), replace=False)
+        for j, w in enumerate(where):
+            a["x"][w], a["y"][w], a["z"][w] = edge[j]
+        return a
+    if kind == "marsim":
+        n = 20000 if n is None else n
+        a = np.zeros(n, POINT_XYZI)
+        p = rng.uniform(-30.0, 30.0, (n, 3)).astype(np.float32)
+        a["x"], a["y"], a["z"] = p[:, 0], p[:, 1], p[:, 2]
+        a["intensity"] = rng.uniform(0, 255, n)
+        where = rng.choice(n, min(len(edge), n), replace=False)
+        for j, w in enumerate(where):
+            a["x"][w], a["y"][w], a["z"][w] = edge[j]
+        return a
+    raise ValueError(f"unknown raw frame kind {kind!r}")

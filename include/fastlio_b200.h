@@ -435,6 +435,57 @@ int fl_localmap_get(fl_localmap_t* l, float* box6);   /* LocalMap_Points as (min
 int fl_localmap_segment_device(fl_localmap_t* l, fl_map_t* map, const double* x26_device, const int* n_scan_device,
                                float* boxes18_device, int* out3_device, void* stream);
 
+/* ------------------------------------------------------------------ sensor preprocessing (DESIGN §4c)
+ * Preprocess::process (src/preprocess.cpp:44-87) with feature_enabled = 0, as every launch file runs it: the raw points of one
+ * LiDAR message in, Measures.lidar (pl_surf, the input of fl_scan_upload[_device]) out.  Paths: avia_handler :161-186,
+ * velodyne_handler :284-322 + :399-455, oust64_handler :253-279, sim_handler :458-481.  Feature extraction (give_feature)
+ * is not provided. */
+#define FL_LIDAR_AVIA 1          /* enum LID_TYPE, preprocess.h:16 */
+#define FL_LIDAR_VELO16 2
+#define FL_LIDAR_OUST64 3
+#define FL_LIDAR_MARSIM 4
+/* The raw layout: point_step bytes per point and the byte offset of each field (PointField.offset for a PointCloud2; the
+ * offsets of livox_ros_driver::CustomPoint for Avia), -1 where the field is absent (it then reads as 0, as PCL's fromROSMsg
+ * leaves a field it cannot match).  Offsets need no alignment.  Each type's fields have the types of the reference's structs:
+ *   AVIA   livox CustomPoint:       time = offset_time u32 (ns), x/y/z f32, intensity = reflectivity u8, tag u8, line u8
+ *   VELO16 velodyne_ros::Point:     x/y/z/intensity f32, time f32 (in time_unit), ring u16            preprocess.h:41-57
+ *   OUST64 ouster_ros::Point:       x/y/z/intensity f32, time = t u32 (in time_unit)                  preprocess.h:59-84
+ *   MARSIM pcl::PointXYZI:          x/y/z/intensity f32
+ * Fields a type does not read are ignored.  The scalars are the ROS parameters laserMapping.cpp:778-787 reads into Preprocess. */
+typedef struct fl_preprocess_params {
+    int lidar_type;          /* FL_LIDAR_* */
+    int n_scans;             /* preprocess/scan_line: N_SCANS, 1..128 (Avia: line < N_SCANS; Velodyne: rings per ring scan) */
+    int scan_rate;           /* preprocess/scan_rate: SCAN_RATE in Hz (Velodyne without point times; >= 1 there) */
+    int time_unit;           /* preprocess/timestamp_unit: 0 s, 1 ms, 2 us, 3 ns (Velodyne and Ouster) */
+    int point_filter_num;    /* point_filter_num >= 1 (MARSIM ignores it, as the reference does) */
+    double blind;            /* preprocess/blind in m */
+    int point_step;          /* bytes per raw point, >= 1 */
+    int off_x, off_y, off_z, off_intensity, off_time, off_ring, off_tag, off_line;
+} fl_preprocess_params_t;
+typedef struct fl_preprocessor fl_preprocess_t;  /* replaces Preprocess (p_pre, laserMapping.cpp:140) */
+/* A handle on `device` for raw frames of up to n_raw_max points: holds the parameters and a workspace sized once (cub's
+ * temporary storage, per-row and per-ring scratch, the host form's device copies).  FL_ERR_ARG for a bad type, unit, n_scans,
+ * scan_rate, point_filter_num or point_step, or a field that does not fit point_step. */
+int fl_preprocess_create(fl_preprocess_t** out, int device, const fl_preprocess_params_t* params, int n_raw_max);
+int fl_preprocess_destroy(fl_preprocess_t* h);
+/* p_pre->process(msg, ptr) in the LiDAR callback                      laserMapping.cpp:291, :327
+ * On the caller's stream: the first *n_raw_device (clamped to [0, n_raw_max]) points of raw_device (n_raw_max x point_step
+ * bytes) -> pl_surf in raw order: xyzi_out_device (4 floats per row: x, y, z, intensity) and offset_ms_out_device
+ * (PointType::curvature, the offset time in ms), exactly fl_scan_upload_device's inputs.  out2_device = (|pl_surf|, rows
+ * dropped for a ring >= n_scans on the Velodyne path without point times, which is undefined behaviour in the reference);
+ * last_ms_device (may be NULL) = pl_surf.points.back().curvature, which sync_packages (:381-399) reads for lidar_end_time
+ * (0 when nothing is kept).  Rows past |pl_surf| are not written.  The Velodyne offset times derived from the yaw use
+ * float(atan2(double, double)) where the reference uses atan2f (DESIGN §4c); everything else is bit-exact.
+ * No host synchronisation, allocation or launch sized from a device value, so the call can be captured into a CUDA graph.
+ * Host, wrong-device, null or misaligned pointers (xyzi 16-byte; offset times, n, out2, last_ms 4-byte) are FL_ERR_ARG; an
+ * n_raw_max above the handle's FL_ERR_CAPACITY; nothing is enqueued on a refusal.  Calls on one handle share its workspace:
+ * enqueue them in one stream order, and synchronise graph replays before a host-form call. */
+int fl_preprocess_device(fl_preprocess_t* h, const void* raw_device, const int* n_raw_device, int n_raw_max, float* xyzi_out_device,
+                         float* offset_ms_out_device, int* out2_device, float* last_ms_device, void* stream);
+/* The host form: the same launches on the handle's own stream, after the handle's last device-form call outside capture.
+ * Writes min(|pl_surf|, cap) rows, *last_ms (may be NULL) as above; returns |pl_surf| (>= 0) or an error (< 0). */
+int fl_preprocess(fl_preprocess_t* h, const void* raw_host, int n_raw, float* xyzi_out, float* offset_ms_out, int cap, float* last_ms);
+
 /* ------------------------------------------------------------------ multi-GPU (no reference counterpart)
  * scan points are sharded across ranks, the map is replicated, the 92 normal-equation doubles
  * are all-reduced once per pass (NCCL over NVLink) and every rank solves redundantly. */
