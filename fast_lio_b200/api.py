@@ -48,6 +48,8 @@ def decode_pass_logs(raw, passes: int) -> list:
 class FastLioError(RuntimeError):
     pass
 
+# the frames of Scan.frame / frame_device: as stored, RGBpointBodyLidarToIMU, RGBpointBodyToWorld (laserMapping.cpp:200-220)
+FRAME_LIDAR, FRAME_IMU, FRAME_WORLD = 0, 1, 2
 
 # ---- sensor preprocessing: the reference's raw point structs as numpy dtypes (the default layouts of Preprocess)
 LIDAR_AVIA, LIDAR_VELO16, LIDAR_OUST64, LIDAR_MARSIM = 1, 2, 3, 4          # enum LID_TYPE, preprocess.h:16
@@ -110,6 +112,7 @@ SYMBOLS = [
     "fl_filter_update_scan_device", "fl_map_delete_boxes_async", "fl_localmap_segment_device",
     "fl_filter_reserve_batch", "fl_filter_batch_plan", "fl_filter_update_batch_device",
     "fl_preprocess_create", "fl_preprocess_destroy", "fl_preprocess_device", "fl_preprocess",
+    "fl_scan_frame", "fl_scan_frame_device",
 ]
 
 
@@ -199,6 +202,8 @@ def load():
     L.fl_scan_undistort_device.argtypes = [_vp, _vp, _vp, C.c_int, _vp, _vp]
     L.fl_scan_voxel_downsample_device.argtypes = [_vp, C.c_float, _vp, _vp]
     L.fl_filter_update_scan_device.argtypes = [_vp, _vp, _vp, _vp, C.c_double, _vp, _vp]
+    L.fl_scan_frame.argtypes = [_vp, C.c_int, C.c_int, _vp, _f32p, C.c_int]
+    L.fl_scan_frame_device.argtypes = [_vp, C.c_int, C.c_int, _vp, _vp, _vp, C.c_int, _vp, _vp]
     L.fl_localmap_create.argtypes = [C.POINTER(C.c_void_p), C.c_double, C.c_float]
     L.fl_localmap_destroy.argtypes = [C.c_void_p]
     L.fl_localmap_segment.argtypes = [C.c_void_p, C.c_void_p, _f64p, _f32p, C.POINTER(C.c_int)]
@@ -823,6 +828,34 @@ class Scan:
             status = torch.empty(2, dtype=torch.int32, device=x.device)
         status = t._tensor(status, "status", None, torch.int32, (2,))
         _check(self._L.fl_filter_update_scan_device(filt.h, self.h, x.data_ptr(), P.data_ptr(), R, status.data_ptr(), t._stream()))
+        return status
+
+    def frame(self, which: int, frame: int, x26=None) -> np.ndarray:
+        """fl_scan_frame: the cloud `which` (0 feats_undistort, 1 feats_down_body) in FRAME_LIDAR / FRAME_IMU / FRAME_WORLD with
+        the state x26 (26 float64; unused, may be None, for FRAME_LIDAR), as an (n, 4) float32 array."""
+        x = None if x26 is None else np.ascontiguousarray(x26, dtype=np.float64).reshape(26)
+        xp = None if x is None else x.ctypes.data
+        n = _check(self._L.fl_scan_frame(self.h, which, frame, xp, np.zeros((1, 4), dtype=np.float32), 0))
+        out = np.zeros((max(n, 1), 4), dtype=np.float32)
+        _check(self._L.fl_scan_frame(self.h, which, frame, xp, out, n))
+        return out[:n].copy()
+
+    def frame_device(self, which: int, frame: int, x, out, n_io=None, status=None):
+        """fl_scan_frame_device: the device forms' cloud `which` in `frame` with the state x ((26,) float64 tensor; None for
+        FRAME_LIDAR) appended to out ((cap, 4) float32) at *n_io (int32 (1,); None: a zeroed position, copied from the host, so
+        pass a tensor when capturing), which advances by n when the cloud fits.  Returns status, an int32 tensor (2,) = (FL_OK,
+        FL_ERR_CAPACITY or FL_ERR_ARG, n), written on the current stream."""
+        import torch
+        t = self.tree
+        out = t._tensor(out, "out", 4)
+        if x is not None:
+            x = t._tensor(x, "x", None, torch.float64, (26,))
+        self._n_io = self._count(n_io, 0, "n_io")               # kept alive until the stream has read it
+        if status is None:
+            status = torch.empty(2, dtype=torch.int32, device=out.device)
+        status = t._tensor(status, "status", None, torch.int32, (2,))
+        _check(self._L.fl_scan_frame_device(self.h, which, frame, None if x is None else x.data_ptr(), out.data_ptr(),
+                                            self._n_io.data_ptr(), out.shape[0], status.data_ptr(), t._stream()))
         return status
 
 

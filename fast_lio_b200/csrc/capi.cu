@@ -509,6 +509,18 @@ int fl_filter_update_scan_device(fl_filter_t* f, fl_scan_t* s, double* x26_devic
     return f->impl->update_scan_on_stream(s->impl->down_dev(), s->impl->down_count_dev(), s->impl->dev_n_max(), x26_device, P_device, R,
                                           status2_device, static_cast<cudaStream_t>(stream));
 }
+// publish_frame_world / publish_frame_body / pointBodyToWorld                     laserMapping.cpp:177-220, :478-549, :909-921
+int fl_scan_frame(fl_scan_t* s, int which, int frame, const double* x26, float* out_xyzi, int cap) {
+    SCAN_HOST_GUARD(s);
+    int n = 0;
+    int rc = s->impl->frame(which, frame, x26, out_xyzi, cap, &n);
+    return rc == FL_OK ? n : rc;
+}
+int fl_scan_frame_device(fl_scan_t* s, int which, int frame, const double* x26_device, float* out_xyzi_device, int* n_io_device, int cap,
+                         int* status2_device, void* stream) {
+    SCAN_GUARD(s);
+    return s->impl->frame_on_stream(which, frame, x26_device, out_xyzi_device, n_io_device, cap, status2_device, static_cast<cudaStream_t>(stream));
+}
 
 // ------------------------------------------------------------------------------------ local-map cube
 int fl_localmap_create(fl_localmap_t** out, double cube_len, float det_range) {

@@ -8,6 +8,7 @@
 
 #include "common.cuh"
 #include "lie.cuh"
+#include "measure.cuh"
 #include "scan.h"
 
 namespace fl {
@@ -242,12 +243,46 @@ __global__ void k_vg_centroid(const float4* __restrict__ pts, const unsigned* __
     out[pos[i]] = make_float4(__fdiv_rn(sx, cnt), __fdiv_rn(sy, cnt), __fdiv_rn(sz, cnt), __fdiv_rn(si, cnt));
 }
 
+// ------------------------------------------------------------------------------------------------ clouds in a frame
+// The loops of publish_frame_world / publish_frame_body / the map's first Build (laserMapping.cpp:200-220, :177-186): row i of the
+// cloud into row pos + i of out, in FL_FRAME_LIDAR as stored, in FL_FRAME_IMU as p_this = R_LI p + t_LI and in FL_FRAME_WORLD as
+// rot p_this + pos -- body_to_world, the arithmetic of the update and k_map_incremental -- with the intensity passed through.
+// Device form: n = *n_dev clamped to [0, n], pos = *n_io, and nothing is written unless 0 <= pos and pos + n <= cap (k_frame_commit
+// then reports why); host form: n_dev and n_io null, pos 0.
+__global__ void k_frame(const float4* __restrict__ src, int n, const int* __restrict__ n_dev, const double* __restrict__ x, int frame,
+                        float4* __restrict__ out, const int* __restrict__ n_io, int cap) {
+    if (n_dev) n = min(max(*n_dev, 0), n);
+    const int pos = n_io ? *n_io : 0;
+    if (pos < 0 || pos > cap || n > cap - pos) return;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    float4 p = src[i];
+    if (frame != FL_FRAME_LIDAR) {
+        float wx, wy, wz;
+        const D3 p_this = body_to_world(load_pose(x), p, wx, wy, wz);
+        if (frame == FL_FRAME_IMU) { p.x = (float)p_this.x; p.y = (float)p_this.y; p.z = (float)p_this.z; }
+        else { p.x = wx; p.y = wy; p.z = wz; }
+    }
+    out[pos + i] = p;
+}
+
+// after k_frame: status2 = (FL_OK, n) and *n_io advanced by n, or (FL_ERR_ARG / FL_ERR_CAPACITY, n) with *n_io as it was
+__global__ void k_frame_commit(const int* __restrict__ n_dev, int n_max, int* __restrict__ n_io, int cap, int* __restrict__ status2) {
+    const int n = min(max(*n_dev, 0), n_max);
+    const int pos = *n_io;
+    const int st = (pos < 0 || pos > cap) ? FL_ERR_ARG : (n > cap - pos ? FL_ERR_CAPACITY : FL_OK);
+    if (st == FL_OK) *n_io = pos + n;
+    status2[0] = st;
+    status2[1] = n;
+}
+
 }  // namespace
 
 // ================================================================================================ ScanFrontEnd
 ScanFrontEnd::~ScanFrontEnd() {
     cudaSetDevice(map_->device());
     DeviceBuffer* all[] = {&raw_, &raw_alt_, &time_, &time_alt_, &down_, &keys_, &keys_alt_, &vals_, &vals_alt_, &heads_, &pos_, &cub_tmp_, &ctl_, &poses_,
+                           &frame_out_, &frame_x_,
                            &d_raw_, &d_time_, &d_sraw_, &d_stime_, &d_down_, &d_keys_, &d_keys_alt_, &d_vals_, &d_vals_alt_, &d_heads_, &d_pos_,
                            &d_cub_, &d_ctl_};
     for (DeviceBuffer* b : all) b->release();
@@ -368,6 +403,31 @@ int ScanFrontEnd::download(int which, float* out_xyzi, int cap, int* n) {
     const void* src = which == 0 ? raw_.ptr : down_.ptr;
     FL_CUDA(cudaMemcpyAsync(out_xyzi, src, sizeof(float4) * (size_t)take, cudaMemcpyDeviceToHost, map_->stream()));
     FL_CUDA(cudaStreamSynchronize(map_->stream()));
+    return FL_OK;
+}
+
+// the current cloud through k_frame into frame_out_, then read back (the kernel of the device form, so the bytes are the same)
+int ScanFrontEnd::frame(int which, int frame, const double* x26, float* out_xyzi, int cap, int* n) {
+    const int have = which == 0 ? n_raw_ : n_down_;
+    if (n) *n = have;
+    if ((which != 0 && which != 1) || frame < FL_FRAME_LIDAR || frame > FL_FRAME_WORLD || (frame != FL_FRAME_LIDAR && !x26)) {
+        set_last_error("scan frame: which must be 0 or 1, frame FL_FRAME_LIDAR / IMU / WORLD, and x26 non-null outside FL_FRAME_LIDAR");
+        return FL_ERR_ARG;
+    }
+    const int take = std::min(have, cap);
+    if (take <= 0) return FL_OK;
+    if (!out_xyzi) { set_last_error("scan frame: null buffer"); return FL_ERR_ARG; }
+    FL_CUDA(cudaSetDevice(map_->device()));
+    cudaStream_t st = map_->stream();
+    FL_CHECK(frame_out_.reserve(sizeof(float4) * (size_t)take));
+    FL_CHECK(frame_x_.reserve(sizeof(double) * XLEN));
+    if (frame != FL_FRAME_LIDAR) FL_CUDA(cudaMemcpyAsync(frame_x_.ptr, x26, sizeof(double) * XLEN, cudaMemcpyHostToDevice, st));
+    const int block = 256;
+    k_frame<<<(take + block - 1) / block, block, 0, st>>>(which == 0 ? raw_.as<float4>() : down_.as<float4>(), take, nullptr,
+                                                          frame_x_.as<double>(), frame, frame_out_.as<float4>(), nullptr, take);
+    FL_CUDA(cudaGetLastError());
+    FL_CUDA(cudaMemcpyAsync(out_xyzi, frame_out_.ptr, sizeof(float4) * (size_t)take, cudaMemcpyDeviceToHost, st));
+    FL_CUDA(cudaStreamSynchronize(st));
     return FL_OK;
 }
 
@@ -512,6 +572,35 @@ int ScanFrontEnd::voxel_downsample_on_stream(float leaf, int* d_n_out, cudaStrea
     FL_CHECK(map_->query_end(st, joined));
     dev_down_ = true;
     return FL_OK;
+}
+
+int ScanFrontEnd::frame_on_stream(int which, int frame, const double* d_x26, float* d_out, int* d_n_io, int cap, int* d_status2,
+                                  cudaStream_t st) {
+    const int dev = map_->device();
+    if ((which != 0 && which != 1) || frame < FL_FRAME_LIDAR || frame > FL_FRAME_WORLD || cap < 0) {
+        set_last_error("scan frame_device: which must be 0 or 1, frame FL_FRAME_LIDAR / IMU / WORLD, and cap >= 0");
+        return FL_ERR_ARG;
+    }
+    if (!device_ptr(d_out, dev, 16) || !device_ptr(d_n_io, dev, 4) || !device_ptr(d_status2, dev, 4) ||
+        ((frame != FL_FRAME_LIDAR || d_x26) && !device_ptr(d_x26, dev, 8))) {
+        set_last_error("scan frame_device: a buffer is not device memory on device %d (out 16-byte, x 8-byte, n_io and status "
+                       "4-byte aligned; x may be null only for FL_FRAME_LIDAR)", dev);
+        return FL_ERR_ARG;
+    }
+    if (!dev_uploaded_) { set_last_error("scan frame_device: no fl_scan_upload_device since the last host-form upload, undistort or down-sample"); return FL_ERR_STATE; }
+    if (which == 1 && !dev_down_) { set_last_error("scan frame_device: no fl_scan_voxel_downsample_device since the last device-form upload"); return FL_ERR_STATE; }
+    const int n = dev_n_max_;
+    ScanDevCtl* c = d_ctl_.as<ScanDevCtl>();
+    const float4* src = which == 1 ? d_down_.as<float4>() : dev_undistorted_ ? d_sraw_.as<float4>() : d_raw_.as<float4>();
+    const int* cnt = which == 1 ? &c->vg.total : &c->n_raw;
+    FL_CUDA(cudaSetDevice(dev));
+    bool joined = false;
+    FL_CHECK(map_->query_begin(st, &joined));
+    const int block = 256;
+    k_frame<<<std::max(1, (n + block - 1) / block), block, 0, st>>>(src, n, cnt, d_x26, frame, reinterpret_cast<float4*>(d_out), d_n_io, cap);
+    k_frame_commit<<<1, 1, 0, st>>>(cnt, n, d_n_io, cap, d_status2);
+    FL_CUDA(cudaGetLastError());
+    return map_->query_end(st, joined);
 }
 
 // Host forms after device forms: when the device forms produced the current cloud (their upload ran after the host forms' last

@@ -24,6 +24,8 @@ public:
     // feats_undistort -> feats_down_body; *n_out = number of occupied voxels (one 4-byte read-back)
     int voxel_downsample(float leaf, int* n_out);
     int download(int which, float* out_xyzi, int cap, int* n);   // which 0: raw / undistorted, 1: down-sampled
+    // that cloud in FL_FRAME_LIDAR / IMU / WORLD with the state x26 (host memory), at most cap rows; *n = the cloud's size
+    int frame(int which, int frame, const double* x26, float* out_xyzi, int cap, int* n);
     const float4* down_device() const { return down_.as<float4>(); }
     int down_count() const { return n_down_; }
     int raw_count() const { return n_raw_; }
@@ -36,6 +38,8 @@ public:
     int upload_on_stream(const float* d_xyzi, const float* d_offset_ms, const int* d_n, int n_max, cudaStream_t st);
     int undistort_on_stream(const double* d_poses, const int* d_n_pose, int n_pose_max, const double* d_x26_end, cudaStream_t st);
     int voxel_downsample_on_stream(float leaf, int* d_n_out, cudaStream_t st);
+    // the device forms' cloud `which` in a frame, appended at *d_n_io of d_out (cap rows) when it fits; d_status2 = (status, n)
+    int frame_on_stream(int which, int frame, const double* d_x26, float* d_out, int* d_n_io, int cap, int* d_status2, cudaStream_t st);
     // every host-form call first: takes over the device forms' cloud and counts when they produced the current one
     int settle();
     // the device forms' down-sampled cloud, its count in device memory, and its row bound (the n_max of their last upload)
@@ -51,6 +55,7 @@ private:
     Map* map_;
     int n_raw_ = 0, n_down_ = 0;
     DeviceBuffer raw_, raw_alt_, time_, time_alt_, down_, keys_, keys_alt_, vals_, vals_alt_, heads_, pos_, cub_tmp_, ctl_, poses_;
+    DeviceBuffer frame_out_, frame_x_;      // the host form of frame(): its rows before the read-back, and its state
     int* h_count_ = nullptr;        // pinned
     size_t undistort_smem_ = 48 * 1024;
     // device forms: uploaded (d_raw_, d_time_) -> time-sorted and de-skewed (d_sraw_, d_stime_) -> down-sampled (d_down_)

@@ -407,6 +407,35 @@ int fl_scan_voxel_downsample_device(fl_scan_t* s, float leaf_size, int* n_out_de
 int fl_filter_update_scan_device(fl_filter_t* f, fl_scan_t* s, double* x26_device, double* P_device, double R, int* status2_device,
                                  void* stream);
 
+/* ---- the scan's clouds in a frame: the clouds a FAST-LIO user consumes after map_incremental (laserMapping.cpp:980-982)
+ * which (as in fl_scan_download): 0 feats_undistort (de-skewed, or as uploaded), 1 feats_down_body.  Per row, float (x, y, z,
+ * intensity), the intensity passed through; the coordinates in FP64 with Eigen's _transformVector order, then rounded to float:
+ *   FL_FRAME_LIDAR  the rows as stored (fl_scan_download)
+ *   FL_FRAME_IMU    offset_R_L_I * p + offset_T_L_I                     RGBpointBodyLidarToIMU :211-220, publish_frame_body :532-549
+ *   FL_FRAME_WORLD  rot * (offset_R_L_I * p + offset_T_L_I) + pos       RGBpointBodyToWorld :200-209, publish_frame_world :478-529,
+ *                                                                        pointBodyToWorld :177-186 (the first scan's Build :909-921)
+ * with the state x26 (26 doubles) -- the arithmetic of the update and of map_incremental. */
+#define FL_FRAME_LIDAR 0
+#define FL_FRAME_IMU 1
+#define FL_FRAME_WORLD 2
+/* Host form: the current cloud (after the device forms' one, as the other host forms take it over), x26 in host memory (unused
+ * for FL_FRAME_LIDAR, may be NULL there).  Writes at most cap rows and returns the cloud's size; synchronous, the conventions of
+ * fl_scan_download. */
+int fl_scan_frame(fl_scan_t* s, int which, int frame, const double* x26, float* out_xyzi, int cap);
+/* Device form, on `stream` (the conventions of the device forms above; capturable).  When `stream` reaches the call it reads the
+ * cloud's device count n, x26_device and the append position *n_io_device.  If 0 <= *n_io_device and *n_io_device + n <= cap it
+ * writes rows [*n_io_device, *n_io_device + n) of out_xyzi_device and advances *n_io_device by n; otherwise it writes no row and
+ * leaves *n_io_device as it was.  status2_device = (status, n): FL_OK, FL_ERR_CAPACITY (the cloud did not fit) or FL_ERR_ARG
+ * (*n_io_device outside [0, cap]).  Rows outside the written range are never touched.  Publishing: zero *n_io_device before
+ * each scan (a memset node in the graph).  Accumulating (pcl_wait_save += , :521): keep appending, and drain out_xyzi_device on
+ * the host every pcd_save_interval scans, then zero *n_io_device.
+ * Refusals enqueue nothing, also on a capturing stream.  FL_ERR_ARG: a bad which or frame; cap < 0; a host, wrong-device or
+ * misaligned pointer (out 16 bytes, x26 8, n_io and status2 4); a null x26_device for FL_FRAME_IMU or FL_FRAME_WORLD.
+ * FL_ERR_STATE: which 0 without a device-form upload since the last host-form upload, undistort or voxel_downsample; which 1
+ * without a device-form voxel_downsample since that upload.  The output equals fl_scan_frame's byte for byte at the same count. */
+int fl_scan_frame_device(fl_scan_t* s, int which, int frame, const double* x26_device, float* out_xyzi_device, int* n_io_device,
+                         int cap, int* status2_device, void* stream);
+
 /* ------------------------------------------------------------------ local-map cube (SURVEY.md §8f row 2)
  * lasermap_fov_segment()                                            laserMapping.cpp:229-277
  * LocalMap_Points / Localmap_Initialized (:229-230) live in the handle; cube_len = cube_side_length (:774),
