@@ -97,6 +97,7 @@ SYMBOLS = [
     "fl_map_create", "fl_map_destroy", "fl_map_set_downsample", "fl_map_build", "fl_map_size", "fl_map_validnum",
     "fl_map_knn", "fl_map_nearest_search", "fl_map_add_points", "fl_map_delete_boxes", "fl_map_flatten", "fl_map_tree_range",
     "fl_map_rebuild", "fl_map_stats", "fl_map_add_boxes", "fl_map_box_search", "fl_map_radius_search", "fl_map_acquire_removed", "fl_map_set_cell_directory", "fl_map_dir_stats",
+    "fl_map_set_deterministic", "fl_map_get_deterministic",
     "fl_map_nearest_search_device", "fl_map_range_workspace_bytes", "fl_map_box_search_device", "fl_map_radius_search_device",
     "fl_map_build_device", "fl_map_add_points_device",
     "fl_filter_create", "fl_filter_destroy", "fl_filter_set_params", "fl_filter_set_solver", "fl_filter_set_search", "fl_filter_set_fused", "fl_filter_update",
@@ -152,6 +153,8 @@ def load():
     L.fl_map_stats.argtypes = [C.c_void_p, _i32p]
     L.fl_map_set_cell_directory.argtypes = [C.c_void_p, C.c_int, C.c_float]
     L.fl_map_dir_stats.argtypes = [C.c_void_p, _i32p]
+    L.fl_map_set_deterministic.argtypes = [C.c_void_p, C.c_int]
+    L.fl_map_get_deterministic.argtypes = [C.c_void_p, C.POINTER(C.c_int)]
     # device-buffer forms: raw device addresses and a cudaStream_t
     _vp = C.c_void_p
     L.fl_map_nearest_search_device.argtypes = [_vp, _vp, C.c_int, C.c_int, C.c_float, _vp, _vp, _vp, _vp]
@@ -254,6 +257,17 @@ class KdTree:
             self.close()
         except Exception:
             pass
+
+    # extension: the deterministic mode (fl_map_set_deterministic): k-NN answers, the down-sampling survivor, the update and
+    # flatten's row order depend only on the map's point set
+    def set_deterministic(self, on: bool):
+        _check(self._L.fl_map_set_deterministic(self.h, int(bool(on))))
+
+    @property
+    def deterministic(self) -> bool:
+        on = C.c_int(0)
+        _check(self._L.fl_map_get_deterministic(self.h, C.byref(on)))
+        return bool(on.value)
 
     # KD_TREE::set_downsample_param
     def set_downsample_param(self, v: float):

@@ -232,6 +232,16 @@ int fl_map_set_cell_directory(fl_map_t* m, int on, float cell_size) {
     m->impl->set_cell_directory(on != 0, cell_size > 0.f ? cell_size : 0.f);
     return m->impl->build_directory();
 }
+int fl_map_set_deterministic(fl_map_t* m, int on) {
+    MAP_GUARD(m);
+    return m->impl->set_deterministic(on != 0);
+}
+int fl_map_get_deterministic(fl_map_t* m, int* on) {
+    MAP_GUARD(m);
+    if (!on) { fl::set_last_error("fl_map_get_deterministic: null output"); return FL_ERR_ARG; }
+    *on = m->impl->deterministic() ? 1 : 0;
+    return FL_OK;
+}
 int fl_map_dir_stats(fl_map_t* m, int* out6) {
     MAP_READ_GUARD(m);
     if (!out6) return FL_ERR_ARG;

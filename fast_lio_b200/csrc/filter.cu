@@ -1058,13 +1058,22 @@ int Filter::init() {
         {(const void*)k_update_n<false, 1>, (const void*)k_update_n<true, 1>}, {(const void*)k_update_n<false, 2>, (const void*)k_update_n<true, 2>},
         {(const void*)k_update_wave<false>, (const void*)k_update_wave<true>}, {(const void*)k_update_n_wave<false>, (const void*)k_update_n_wave<true>},
         {(const void*)k_update_batch<false>, (const void*)k_update_batch<true>}};
+    const void* const upd_fn_det[UK_COUNT][2] = {  // the keyed-tie-rule forms: a kernel's cap holds for both of its forms
+        {(const void*)k_update_det<false, 1>, (const void*)k_update_det<true, 1>}, {(const void*)k_update_det<false, 2>, (const void*)k_update_det<true, 2>},
+        {(const void*)k_update_n_det<false, 1>, (const void*)k_update_n_det<true, 1>}, {(const void*)k_update_n_det<false, 2>, (const void*)k_update_n_det<true, 2>},
+        {(const void*)k_update_wave_det<false>, (const void*)k_update_wave_det<true>}, {(const void*)k_update_n_wave_det<false>, (const void*)k_update_n_wave_det<true>},
+        {(const void*)k_update_batch_det<false>, (const void*)k_update_batch_det<true>}};
     upd_caps_.threads = UPD_THREADS;
     upd_caps_.wave_smem = (int)sizeof(WavePoint);      // a wave block's tile of points in dynamic shared memory
     for (int k = 0; k < UK_COUNT; k++)
         for (int e = 0; e < 2; e++) {
             const int smem = k == UK_WAVE || k == UK_N_WAVE ? upd_caps_.wave_smem : 0;
             if (smem) FL_CUDA(cudaFuncSetAttribute(upd_fn[k][e], cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+            if (smem) FL_CUDA(cudaFuncSetAttribute(upd_fn_det[k][e], cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
             FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, upd_fn[k][e], upd_kernel_pair(k) * UPD_THREADS, smem));
+            int occ_det = 0;
+            FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_det, upd_fn_det[k][e], upd_kernel_pair(k) * UPD_THREADS, smem));
+            occ = std::min(occ, occ_det);
             int& cap = upd_caps_.blocks[k][e];
             cap = sms_ * (k == UK_UPDATE1 || k == UK_N1 ? std::max(1, occ) : occ);
             const int host = k == UK_N1 ? UK_UPDATE1 : k == UK_N2 ? UK_UPDATE2 : k == UK_N_WAVE ? UK_WAVE : -1;
@@ -1224,6 +1233,11 @@ int Filter::run_passes() {
     if (scan_.q_end > scan_.Q) { set_last_error("shard exceeds the scan"); return FL_ERR_ARG; }
     neighbours_complete_ = false;
     launches_ = 0;
+    if (!fused() && map_->deterministic()) {
+        set_last_error("update: the deterministic map mode runs k_update only; this filter uses %s",
+                       solver_ != 1 ? "solver mode 0" : "the two-kernels-per-pass chain (fused 0)");
+        return FL_ERR_STATE;
+    }
     if (fused()) {
         cudaStream_t st = stream();
         if (nranks_ > 1 && !p2p_on_) {
@@ -1282,12 +1296,22 @@ int Filter::launch_update(int max_passes, int mode, int search_only, cudaStream_
 
 UpdPlan Filter::plan(UpdRoute r, int rows, int n_hyp) const {
     const char* e = getenv("FASTLIO_B200_PAIR");
-    return plan_update(upd_caps_, r, rows, extrinsic_est_, e && e[0] == '1', n_hyp);
+    return plan_update(upd_caps_, r, rows, extrinsic_est_, e && e[0] == '1', n_hyp, map_->deterministic());
 }
 
 template <bool E>
 static cudaError_t launch_upd_kernel(const UpdPlan& p, bool pdl, cudaStream_t st, const UpdArgs& a, const int* n, unsigned long long* rows, int log_stride) {
     const dim3 grid((unsigned)p.grid_x, (unsigned)p.slots);
+    if (p.det) switch (p.kernel) {           // the keyed tie rule (fl_map_set_deterministic)
+    case UK_UPDATE1: return launch_pdl(k_update_det<E, 1>, grid, p.block, st, pdl, a);
+    case UK_UPDATE2: return launch_pdl(k_update_det<E, 2>, grid, p.block, st, pdl, a);
+    case UK_N1: return launch_pdl(k_update_n_det<E, 1>, grid, p.block, st, pdl, a, n);
+    case UK_N2: return launch_pdl(k_update_n_det<E, 2>, grid, p.block, st, pdl, a, n);
+    case UK_WAVE: return launch_pdl_smem(k_update_wave_det<E>, grid, p.block, p.smem, st, pdl, a, rows);
+    case UK_N_WAVE: return launch_pdl_smem(k_update_n_wave_det<E>, grid, p.block, p.smem, st, pdl, a, n, rows);
+    case UK_BATCH: return launch_pdl(k_update_batch_det<E>, grid, p.block, st, pdl, a, log_stride);
+    default: return cudaErrorInvalidValue;
+    }
     switch (p.kernel) {
     case UK_UPDATE1: return launch_pdl(k_update<E, 1>, grid, p.block, st, pdl, a);
     case UK_UPDATE2: return launch_pdl(k_update<E, 2>, grid, p.block, st, pdl, a);

@@ -413,7 +413,7 @@ __global__ void __launch_bounds__(256) k_halo_fix(MapView m, const unsigned* __r
 // GATED (fl_map_nearest_search for k <= KNN_K, both forms): a query with a non-finite coordinate is searched at the origin
 // (so fl_map_dir_stats counts it as a walk from there) and finds nothing; every other row keeps its leading entries with
 // d2 <= md2.  Dropped entries are (0, 0, 0, 0) with d2 = +inf.
-template <bool GATED>
+template <bool GATED, bool DET = false>
 __device__ __forceinline__ void knn_batch(const MapView& m, const float4* __restrict__ q, int nq, int k, float md2,
                                           float4* __restrict__ out_pts, float* __restrict__ out_d2, int* __restrict__ out_cnt,
                                           WalkPool& pool) {
@@ -431,7 +431,7 @@ __device__ __forceinline__ void knn_batch(const MapView& m, const float4* __rest
             finite = isfinite(qq.x) && isfinite(qq.y) && isfinite(qq.z);
             if (!finite) qq.x = qq.y = qq.z = 0.f;
         }
-        TBest kb;
+        TBestT<DET> kb;
         knn_block(m, active, qq.x, qq.y, qq.z, kb, pool, phase);
         if (active) {
             float4 p[KNN_K];
@@ -469,18 +469,33 @@ __global__ void __launch_bounds__(128) k_knn_batch_gated(MapView m, const float4
     knn_batch<true>(m, q, nq, k, md2, out_pts, out_d2, out_cnt, pool);
 }
 
+// the keyed tie rule (fl_map_set_deterministic, map.cuh "tie rules"): kernels of their own, so the default ones keep their code
+__global__ void __launch_bounds__(128) k_knn_batch_det(MapView m, const float4* __restrict__ q, int nq, int k,
+                                                        float4* __restrict__ out_pts, float* __restrict__ out_d2,
+                                                        int* __restrict__ out_cnt) {
+    __shared__ WalkPool pool;
+    knn_batch<false, true>(m, q, nq, k, 0.f, out_pts, out_d2, out_cnt, pool);
+}
+__global__ void __launch_bounds__(128) k_knn_batch_gated_det(MapView m, const float4* __restrict__ q, int nq, int k, float md2,
+                                                              float4* __restrict__ out_pts, float* __restrict__ out_d2,
+                                                              int* __restrict__ out_cnt) {
+    __shared__ WalkPool pool;
+    knn_batch<true, true>(m, q, nq, k, md2, out_pts, out_d2, out_cnt, pool);
+}
+
 // Nearest_Search(point, k, .., max_dist) for 6 <= k <= 32: one warp per query, the k-best list one entry per lane (KBestK),
 // seeded from the cell directory (knn_seed_k) and completed by the BVH walk where the seed is not proven.  A query with a
 // non-finite coordinate, or a NaN md2, finds nothing.  Lane j writes entry j of the row.
-__global__ void __launch_bounds__(256) k_knn_k(MapView m, const float4* __restrict__ q, int nq, int k, float md2,
-                                                float4* __restrict__ out_pts, float* __restrict__ out_d2, int* __restrict__ out_cnt) {
+template <bool DET>
+__device__ __forceinline__ void knn_k(const MapView& m, const float4* __restrict__ q, int nq, int k, float md2,
+                                      float4* __restrict__ out_pts, float* __restrict__ out_d2, int* __restrict__ out_cnt) {
     const int lane = threadIdx.x & 31;
     const int warps = (gridDim.x * blockDim.x) >> 5;
     const float gate = nextafterf(md2, INFINITY);
     int walked = 0;
     for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < nq; i += warps) {
         const float4 qq = __ldg(&q[i]);
-        KBestK kb;
+        KBestKT<DET> kb;
         kb.init(k, gate);
         if (isfinite(qq.x) && isfinite(qq.y) && isfinite(qq.z) && !isnan(md2) && !knn_seed_k(m, qq.x, qq.y, qq.z, md2, kb, lane)) {
             walked++;
@@ -492,6 +507,14 @@ __global__ void __launch_bounds__(256) k_knn_k(MapView m, const float4* __restri
         if (lane == 0) out_cnt[i] = cnt;
     }
     if (lane == 0 && walked && m.dir.cap && m.dir.n_walked) atomicAdd(m.dir.n_walked, walked);
+}
+__global__ void __launch_bounds__(256) k_knn_k(MapView m, const float4* __restrict__ q, int nq, int k, float md2,
+                                                float4* __restrict__ out_pts, float* __restrict__ out_d2, int* __restrict__ out_cnt) {
+    knn_k<false>(m, q, nq, k, md2, out_pts, out_d2, out_cnt);
+}
+__global__ void __launch_bounds__(256) k_knn_k_det(MapView m, const float4* __restrict__ q, int nq, int k, float md2,
+                                                    float4* __restrict__ out_pts, float* __restrict__ out_d2, int* __restrict__ out_cnt) {
+    knn_k<true>(m, q, nq, k, md2, out_pts, out_d2, out_cnt);
 }
 
 // Delete_Point_Boxes: every slot tests itself against the boxes (half-open, ikd_Tree.cpp:796).
@@ -593,6 +616,22 @@ __global__ void k_compact(MapView m, int n_leaf_used, float4* __restrict__ out, 
     }
 }
 
+// fl_map_flatten in the deterministic mode: the compacted rows sorted by (x, y, z, intensity) as order-preserving integers of their
+// bits (ord_bits), by two stable 64-bit radix sorts, least significant half first: (z, intensity), then (x, y).
+__global__ void k_flatten_keys(const float4* __restrict__ rows, const unsigned* __restrict__ perm, int n, bool xy,
+                               unsigned long long* __restrict__ keys, unsigned* __restrict__ vals) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const unsigned r = perm ? perm[i] : (unsigned)i;
+    const float4 p = rows[r];
+    keys[i] = xy ? ((unsigned long long)ord_bits(p.x) << 32) | ord_bits(p.y) : ((unsigned long long)ord_bits(p.z) << 32) | ord_bits(p.w);
+    vals[i] = r;
+}
+__global__ void k_gather_rows(const float4* __restrict__ rows, const unsigned* __restrict__ perm, int n, float4* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = rows[perm[i]];
+}
+
 // ----------------------------------------------------------------------------- Add_Points
 // Voxel of a point exactly as Add_Points computes it (ikd_Tree.cpp:491-499): float division,
 // float floor, float multiply.
@@ -633,7 +672,10 @@ __global__ void k_group_heads(const unsigned long long* __restrict__ keys, int n
     if (r < n && (r == 0 || keys[r] != keys[r - 1])) group_start[atomicAdd(&counters[C_GROUPS], 1)] = r;
 }
 
-struct BoxScan {       // pass 1: count the valid points inside the voxel and find the one closest to its centre
+// pass 1: count the valid points inside the voxel and find the one closest to its centre.  DET (fl_map_set_deterministic): of
+// points at bit-equal distances the one with the smallest (x, y, z, intensity) counts as the closest (map.cuh, "tie rules")
+template <bool DET = false>
+struct BoxScan {
     const MapView& m; const VoxelBox& vb; int lane;
     int count = 0; float best_d = INFINITY; int best_slot = -1;
     __device__ BoxScan(const MapView& m_, const VoxelBox& vb_, int lane_) : m(m_), vb(vb_), lane(lane_) {}
@@ -648,9 +690,14 @@ struct BoxScan {       // pass 1: count the valid points inside the voxel and fi
                 const float d = in ? sq_dist3(p.x, p.y, p.z, vb.mid[0], vb.mid[1], vb.mid[2]) : INFINITY;
                 const unsigned key = in ? __float_as_uint(d) : 0xffffffffu;
                 const unsigned best = __reduce_min_sync(FULL, key);
-                if (__uint_as_float(best) < best_d) {       // strict: the first one found wins ties (ikd_Tree.cpp:508)
-                    best_d = __uint_as_float(best);
-                    best_slot = l * LEAF + (__ffs(__ballot_sync(FULL, key == best)) - 1);
+                if constexpr (!DET) {
+                    if (__uint_as_float(best) < best_d) {       // strict: the first one found wins ties (ikd_Tree.cpp:508)
+                        best_d = __uint_as_float(best);
+                        best_slot = l * LEAF + (__ffs(__ballot_sync(FULL, key == best)) - 1);
+                    }
+                } else if (__uint_as_float(best) <= best_d) {
+                    const int cand = l * LEAF + warp_key_min<false>(m, __ballot_sync(FULL, key == best), p, slot, lane);
+                    if (__uint_as_float(best) < best_d || key_less<false>(m, cand, best_slot)) { best_d = __uint_as_float(best); best_slot = cand; }
                 }
             }
             l = m.next[l];
@@ -678,11 +725,12 @@ __device__ __forceinline__ bool same_point(const float4& a, const float4& b) {  
 // runs into them and n may be n_max).  Reproduces the sequential per-point semantics of
 // Add_Points(downsample_on = true) (ikd_Tree.cpp:489-521) for all batch points that fall
 // into the voxel, in their original order (the sort is stable).
-__global__ void __launch_bounds__(256) k_downsample_resolve(MapView m, const float4* __restrict__ batch,
-                                                             const unsigned long long* __restrict__ keys,
-                                                             const unsigned* __restrict__ vals, int n,
-                                                             const int* __restrict__ group_start, float ds,
-                                                             float4* __restrict__ insert_list, int* counters) {
+template <bool DET>
+__device__ __forceinline__ void downsample_resolve(const MapView& m, const float4* __restrict__ batch,
+                                                   const unsigned long long* __restrict__ keys,
+                                                   const unsigned* __restrict__ vals, int n,
+                                                   const int* __restrict__ group_start, float ds,
+                                                   float4* __restrict__ insert_list, int* counters) {
     const int lane = threadIdx.x & 31;
     const int warps = (gridDim.x * blockDim.x) >> 5;
     const int n_groups = counters[C_GROUPS];
@@ -692,7 +740,7 @@ __global__ void __launch_bounds__(256) k_downsample_resolve(MapView m, const flo
         const float4 first = batch[vals[r0]];
         VoxelBox vb;
         voxel_box(first, ds, vb);
-        BoxScan scan(m, vb, lane);
+        BoxScan<DET> scan(m, vb, lane);
         box_query(m, vb.bmin, vb.bmax, scan, lane);
         // ---- sequential resolution (warp-uniform scalar work)
         int cur_count = scan.count;
@@ -728,6 +776,20 @@ __global__ void __launch_bounds__(256) k_downsample_resolve(MapView m, const flo
             }
         }
     }
+}
+__global__ void __launch_bounds__(256) k_downsample_resolve(MapView m, const float4* __restrict__ batch,
+                                                             const unsigned long long* __restrict__ keys,
+                                                             const unsigned* __restrict__ vals, int n,
+                                                             const int* __restrict__ group_start, float ds,
+                                                             float4* __restrict__ insert_list, int* counters) {
+    downsample_resolve<false>(m, batch, keys, vals, n, group_start, ds, insert_list, counters);
+}
+__global__ void __launch_bounds__(256) k_downsample_keyed(MapView m, const float4* __restrict__ batch,
+                                                                 const unsigned long long* __restrict__ keys,
+                                                                 const unsigned* __restrict__ vals, int n,
+                                                                 const int* __restrict__ group_start, float ds,
+                                                                 float4* __restrict__ insert_list, int* counters) {
+    downsample_resolve<true>(m, batch, keys, vals, n, group_start, ds, insert_list, counters);
 }
 
 // One warp per new point: descend towards the nearest child box to the home leaf, claim a free slot there or
@@ -1368,6 +1430,12 @@ int Map::build(const float* pts_xyzi, int n) {
 // The one launch of a batched nearest search on `st`: fl_map_knn's k_knn_batch (ungated), or fl_map_nearest_search's
 // k_knn_batch_gated (k <= KNN_K) or k_knn_k.
 void Map::launch_knn(bool gated, const float4* q, int nq, int k, float md2, float4* p, float* d2, int* cnt, cudaStream_t st) {
+    if (det_) {                  // the keyed tie rule
+        if (!gated) k_knn_batch_det<<<blocks_for(nq, 128, 1 << 20), 128, 0, st>>>(v_, q, nq, k, p, d2, cnt);
+        else if (k <= KNN_K) k_knn_batch_gated_det<<<blocks_for(nq, 128, 1 << 20), 128, 0, st>>>(v_, q, nq, k, md2, p, d2, cnt);
+        else k_knn_k_det<<<resident_blocks(k_knn_k_det, 256, (long long)nq * 32, n_sm_), 256, 0, st>>>(v_, q, nq, k, md2, p, d2, cnt);
+        return;
+    }
     if (!gated) k_knn_batch<<<blocks_for(nq, 128, 1 << 20), 128, 0, st>>>(v_, q, nq, k, p, d2, cnt);
     else if (k <= KNN_K) k_knn_batch_gated<<<blocks_for(nq, 128, 1 << 20), 128, 0, st>>>(v_, q, nq, k, md2, p, d2, cnt);
     else k_knn_k<<<resident_blocks(k_knn_k, 256, (long long)nq * 32, n_sm_), 256, 0, st>>>(v_, q, nq, k, md2, p, d2, cnt);
@@ -1549,6 +1617,13 @@ int Map::add_boxes(const float* boxes6, int nb, int* revived) {
     return FL_OK;
 }
 
+int Map::set_deterministic(bool on) {
+    FL_CUDA(cudaSetDevice(device_));
+    FL_CUDA(cudaStreamSynchronize(stream_));     // work already queued on the handle's stream runs under the mode it was queued in
+    det_ = on;
+    return FL_OK;
+}
+
 int Map::flatten(float* out_xyzi, int cap, int* n_out) {
     FL_CUDA(cudaSetDevice(device_));
     FL_CHECK(src_.reserve(sizeof(float4) * (size_t)std::max(1, n_valid_)));
@@ -1561,8 +1636,30 @@ int Map::flatten(float* out_xyzi, int cap, int* n_out) {
     const int n = h_counters_[C_COMPACT];
     if (n != n_valid_) { set_last_error("flatten: %d valid points on device, host expected %d", n, n_valid_); return FL_ERR_STATE; }
     if (n_out) *n_out = n;
+    const float4* rows = src_.as<float4>();
+    if (det_ && out_xyzi && cap > 0 && n > 1) {
+        FL_CHECK(keys_in_.reserve(sizeof(unsigned long long) * (size_t)n));
+        FL_CHECK(keys_out_.reserve(sizeof(unsigned long long) * (size_t)n));
+        FL_CHECK(vals_in_.reserve(sizeof(unsigned) * (size_t)n));
+        FL_CHECK(vals_out_.reserve(sizeof(unsigned) * (size_t)n));
+        FL_CHECK(scratch3_.reserve(sizeof(float4) * (size_t)n));
+        size_t tmp = 0;
+        FL_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp, keys_in_.as<unsigned long long>(), keys_out_.as<unsigned long long>(),
+                                                vals_in_.as<unsigned>(), vals_out_.as<unsigned>(), n, 0, 64, stream_));
+        FL_CHECK(cub_tmp_.reserve(tmp));
+        for (int xy = 0; xy < 2; xy++) {
+            k_flatten_keys<<<blocks_for(n, 256, 1 << 30), 256, 0, stream_>>>(rows, xy ? vals_out_.as<unsigned>() : nullptr, n, xy != 0,
+                                                                             keys_in_.as<unsigned long long>(), vals_in_.as<unsigned>());
+            tmp = cub_tmp_.bytes;
+            FL_CUDA(cub::DeviceRadixSort::SortPairs(cub_tmp_.ptr, tmp, keys_in_.as<unsigned long long>(), keys_out_.as<unsigned long long>(),
+                                                    vals_in_.as<unsigned>(), vals_out_.as<unsigned>(), n, 0, 64, stream_));
+        }
+        k_gather_rows<<<blocks_for(n, 256, 1 << 30), 256, 0, stream_>>>(rows, vals_out_.as<unsigned>(), n, scratch3_.as<float4>());
+        FL_CUDA(cudaGetLastError());
+        rows = scratch3_.as<float4>();
+    }
     if (out_xyzi && cap > 0) {
-        FL_CUDA(cudaMemcpyAsync(out_xyzi, src_.ptr, sizeof(float4) * (size_t)std::min(n, cap), cudaMemcpyDeviceToHost, stream_));
+        FL_CUDA(cudaMemcpyAsync(out_xyzi, rows, sizeof(float4) * (size_t)std::min(n, cap), cudaMemcpyDeviceToHost, stream_));
         FL_CUDA(cudaStreamSynchronize(stream_));
     }
     return FL_OK;
@@ -1911,7 +2008,7 @@ int Map::add_points_host(const float4* d_pts, int n, bool downsample_on, int* ad
     FL_CUDA(cub::DeviceRadixSort::SortPairs(cub_tmp_.ptr, tmp, keys_in_.as<unsigned long long>(), keys_out_.as<unsigned long long>(),
                                             vals_in_.as<unsigned>(), vals_out_.as<unsigned>(), n, 0, 63, stream_));
     k_group_heads<<<blocks_for(n, 256, 1 << 30), 256, 0, stream_>>>(keys_out_.as<unsigned long long>(), n, scratch2_.as<int>(), d_cnt, nullptr);
-    k_downsample_resolve<<<blocks_for((long long)n * 32, 256), 256, 0, stream_>>>(
+    (det_ ? k_downsample_keyed : k_downsample_resolve)<<<blocks_for((long long)n * 32, 256), 256, 0, stream_>>>(
         v_, d_pts, keys_out_.as<unsigned long long>(), vals_out_.as<unsigned>(), n, scratch2_.as<int>(), downsample_,
         scratch3_.as<float4>(), d_cnt);
     FL_CUDA(cudaGetLastError());
@@ -2104,7 +2201,7 @@ int Map::enqueue_add(const float4* pts, int slot, bool downsample_on, int n_max,
         size_t tmp = a_cub_.bytes;
         FL_CUDA(cub::DeviceRadixSort::SortPairs(a_cub_.ptr, tmp, ki, ko, a_vals_in_.as<unsigned>(), a_vals_out_.as<unsigned>(), n_max, 0, 64, st));
         k_group_heads<<<blocks_for(n_max, 256, 1 << 30), 256, 0, st>>>(ko, n_max, a_groups_.as<int>(), d_cnt, &d_cnt[slot]);
-        k_downsample_resolve<<<blocks_for((long long)n_max * 32, 256), 256, 0, st>>>(
+        (det_ ? k_downsample_keyed : k_downsample_resolve)<<<blocks_for((long long)n_max * 32, 256), 256, 0, st>>>(
             v_, pts, ko, a_vals_out_.as<unsigned>(), n_max, a_groups_.as<int>(), downsample_, a_ins_.as<float4>(), d_cnt);
         FL_CHECK(enqueue_insert(a_ins_.as<float4>(), &d_cnt[C_NINSERT], n_max, st));
     } else {

@@ -77,10 +77,71 @@ __device__ __forceinline__ bool slot_valid(const float4& p) { return __float_as_
 // +inf (0x7f800000) can serve as the "no candidate" marker of the integer warp reductions.
 constexpr unsigned INF_BITS = 0x7f800000u;
 
+// ----------------------------------------------------------------------------- tie rules
+// Every k-best list below takes a tie rule as its template parameter DET:
+//   false (the default): a candidate enters only if strictly closer than the k-th best, so of two points at bit-equal squared
+//          distances the one visited first wins -- the reference's rule (ikd_Tree.cpp:1088), whose visiting order here is the
+//          slot order of leaves and halo lists, which racing inserts make run-dependent;
+//   true  (fl_map_set_deterministic): candidates are ranked by the total order (d2, x, y, z, intensity), the coordinates and
+//          the intensity compared as order-preserving integers of their bits (key_less), so the k best are a function of the
+//          SET of valid points.  The key is read from the map (m.pts / m.payload) only when a candidate's d2 equals an entry's,
+//          the rare path: nothing extra is carried in registers.
+__device__ __forceinline__ unsigned ord_bits(float f) {            // float order, with -0 below +0
+    const unsigned u = __float_as_uint(f);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+// (x, y, z, intensity) of the point in slot a strictly below that of slot b.  NC: read-only (non-coherent) loads, for kernels that
+// write no slot; the down-sampling kernel, whose warps retire slots while others read, uses plain loads (NC = false).
+template <bool NC = true>
+__device__ __forceinline__ float4 map_pt(const MapView& m, int i) { if constexpr (NC) return __ldg(&m.pts[i]); else return m.pts[i]; }
+template <bool NC = true>
+__device__ __forceinline__ float map_payload(const MapView& m, int i) { if constexpr (NC) return __ldg(&m.payload[i]); else return m.payload[i]; }
+template <bool NC = true>
+__device__ __forceinline__ bool key_less(const MapView& m, int a, int b) {
+    const float4 pa = map_pt<NC>(m, a), pb = map_pt<NC>(m, b);
+    if (pa.x != pb.x || __float_as_uint(pa.x) != __float_as_uint(pb.x)) return ord_bits(pa.x) < ord_bits(pb.x);
+    if (pa.y != pb.y || __float_as_uint(pa.y) != __float_as_uint(pb.y)) return ord_bits(pa.y) < ord_bits(pb.y);
+    if (pa.z != pb.z || __float_as_uint(pa.z) != __float_as_uint(pb.z)) return ord_bits(pa.z) < ord_bits(pb.z);
+    return ord_bits(map_payload<NC>(m, a)) < ord_bits(map_payload<NC>(m, b));
+}
+// candidate (nd, slot nidx) ranks before the entry (d, slot idx; idx < 0: empty) under the keyed order
+__device__ __forceinline__ bool key_before(const MapView& m, float nd, int nidx, float d, int idx) {
+    if (nd != d) return nd < d;
+    return idx >= 0 && key_less(m, nidx, idx);
+}
+// y, z, intensity (p.w) of a below those of b: the keyed order of two fetched neighbours with equal x
+__device__ __forceinline__ bool yzi_less(const float4& a, const float4& b) {
+    if (ord_bits(a.y) != ord_bits(b.y)) return ord_bits(a.y) < ord_bits(b.y);
+    if (ord_bits(a.z) != ord_bits(b.z)) return ord_bits(a.z) < ord_bits(b.z);
+    return ord_bits(a.w) < ord_bits(b.w);
+}
+// The lane of `tied` (lanes whose candidates have bit-equal d2) that holds the smallest key; p: the lane's point, slot its slot
+template <bool NC = true>
+__device__ __forceinline__ int warp_key_min(const MapView& m, unsigned tied, const float4& p, int slot, int lane) {
+    if ((tied & (tied - 1)) == 0) return __ffs(tied) - 1;
+    bool in = (tied >> lane) & 1u;
+    unsigned v = __reduce_min_sync(FULL, in ? ord_bits(p.x) : 0xffffffffu);
+    in = in && ord_bits(p.x) == v;
+    v = __reduce_min_sync(FULL, in ? ord_bits(p.y) : 0xffffffffu);
+    in = in && ord_bits(p.y) == v;
+    v = __reduce_min_sync(FULL, in ? ord_bits(p.z) : 0xffffffffu);
+    in = in && ord_bits(p.z) == v;
+    unsigned t = __ballot_sync(FULL, in);
+    if (t & (t - 1)) {
+        const unsigned ki = in ? ord_bits(map_payload<NC>(m, slot)) : 0xffffffffu;
+        v = __reduce_min_sync(FULL, ki);
+        t = __ballot_sync(FULL, in && ki == v);
+    }
+    return __ffs(t) - 1;
+}
+
 // Lane j < K holds the j-th best (distance, slot); other lanes hold +inf.  Mirrors MANUAL_HEAP
 // + PointType_CMP (ikd_Tree.h:93-201) in effect: a candidate enters only if strictly closer
 // than the current k-th best (ikd_Tree.cpp:1088); `w` caches that k-th best, warp-uniform.
-struct KBest {
+// DET: the keyed order instead (see the tie rules above).
+template <bool DET>
+struct KBestT {
+    static constexpr bool det = DET;
     float d;
     int idx;
     float w;
@@ -88,25 +149,38 @@ struct KBest {
     __device__ __forceinline__ void init() { d = INFINITY; idx = -1; w = INFINITY; n = 0; }
     __host__ __device__ static constexpr int cap() { return KNN_K; }
     __device__ __forceinline__ static constexpr bool gated(unsigned) { return false; }       // no distance gate
-    // nd, nidx warp-uniform, nd < w
-    __device__ __forceinline__ void insert(float nd, int nidx, int lane) {
+    // nd, nidx warp-uniform, nd < w (DET: or nd == w and a key below the k-th entry's)
+    __device__ __forceinline__ void insert(float nd, int nidx, int lane, const MapView& m) {
         const float up_d = __shfl_up_sync(FULL, d, 1);
         const int up_i = __shfl_up_sync(FULL, idx, 1);
-        if (lane < KNN_K && nd < d) {
-            const bool take_prev = lane > 0 && nd < up_d;
-            d = take_prev ? up_d : nd;
-            idx = take_prev ? up_i : nidx;
+        if constexpr (!DET) {
+            if (lane < KNN_K && nd < d) {
+                const bool take_prev = lane > 0 && nd < up_d;
+                d = take_prev ? up_d : nd;
+                idx = take_prev ? up_i : nidx;
+            }
+        } else {
+            const bool lt = lane < KNN_K && key_before(m, nd, nidx, d, idx);
+            const bool up_lt = __shfl_up_sync(FULL, (int)lt, 1) != 0;
+            if (lt) {
+                const bool take_prev = lane > 0 && up_lt;
+                d = take_prev ? up_d : nd;
+                idx = take_prev ? up_i : nidx;
+            }
         }
         w = __shfl_sync(FULL, d, KNN_K - 1);
     }
 };
+using KBest = KBestT<false>;
 
 // The same list for a runtime k (1..32, lanes 0..k-1) with the distance gate of Nearest_Search's max_dist
 // (ikd_Tree.cpp:1067-1088): a point is admitted while the list is not full when d2 <= md2, and once it is full when d2 is
 // strictly below the k-th best.  gate = nextafterf(md2, +inf), so "strictly below w = min(k-th best, gate)" says both.
 // Every box of the walk is pruned against w as well, which is the reference's box_dist > md2 cut-off.
 constexpr int KNN_KMAX = 32;
-struct KBestK {
+template <bool DET>
+struct KBestKT {
+    static constexpr bool det = DET;
     float d;
     int idx;
     float w;
@@ -117,17 +191,28 @@ struct KBestK {
     __device__ __forceinline__ int cap() const { return k; }
     // while the list is not full, w is the gate: the first leaf of a query stops at it
     __device__ __forceinline__ bool gated(unsigned best) const { return best >= __float_as_uint(w); }
-    __device__ __forceinline__ void insert(float nd, int nidx, int lane) {
+    __device__ __forceinline__ void insert(float nd, int nidx, int lane, const MapView& m) {
         const float up_d = __shfl_up_sync(FULL, d, 1);
         const int up_i = __shfl_up_sync(FULL, idx, 1);
-        if (lane < k && nd < d) {
-            const bool take_prev = lane > 0 && nd < up_d;
-            d = take_prev ? up_d : nd;
-            idx = take_prev ? up_i : nidx;
+        if constexpr (!DET) {
+            if (lane < k && nd < d) {
+                const bool take_prev = lane > 0 && nd < up_d;
+                d = take_prev ? up_d : nd;
+                idx = take_prev ? up_i : nidx;
+            }
+        } else {
+            const bool lt = lane < k && key_before(m, nd, nidx, d, idx);
+            const bool up_lt = __shfl_up_sync(FULL, (int)lt, 1) != 0;
+            if (lt) {
+                const bool take_prev = lane > 0 && up_lt;
+                d = take_prev ? up_d : nd;
+                idx = take_prev ? up_i : nidx;
+            }
         }
         w = fminf(__shfl_sync(FULL, d, k - 1), gate);
     }
 };
+using KBestK = KBestKT<false>;
 
 // Visit one leaf bucket (and its overflow chain): each lane scores one slot, then the
 // (at most K) improving candidates are extracted in ascending order.
@@ -145,7 +230,9 @@ __device__ __forceinline__ void knn_leaf(const MapView& m, int leaf, float qx, f
             for (int r = 0; r < kb.cap(); r++) {
                 best = __reduce_min_sync(FULL, key);
                 if (best == INF_BITS || kb.gated(best)) break;
-                const int src = __ffs(__ballot_sync(FULL, key == best)) - 1;
+                int src;
+                if constexpr (KB::det) src = warp_key_min(m, __ballot_sync(FULL, key == best), p, leaf * LEAF + lane, lane);
+                else src = __ffs(__ballot_sync(FULL, key == best)) - 1;
                 if (lane == r) { kb.d = __uint_as_float(best); kb.idx = leaf * LEAF + src; }
                 if (lane == src) key = INF_BITS;
                 kb.n = r + 1;
@@ -157,11 +244,22 @@ __device__ __forceinline__ void knn_leaf(const MapView& m, int leaf, float qx, f
 #pragma unroll 1
         while (true) {
             const unsigned best = __reduce_min_sync(FULL, key);
-            if (best >= __float_as_uint(kb.w)) break;       // nothing strictly closer than the k-th best is left (covers the marker)
-            const int src = __ffs(__ballot_sync(FULL, key == best)) - 1;
-            const int cidx = leaf * LEAF + src;
+            int src, cidx;
+            if constexpr (!KB::det) {
+                if (best >= __float_as_uint(kb.w)) break;       // nothing strictly closer than the k-th best is left (covers the marker)
+                src = __ffs(__ballot_sync(FULL, key == best)) - 1;
+                cidx = leaf * LEAF + src;
+            } else {
+                if (best > __float_as_uint(kb.w) || best == INF_BITS) break;
+                src = warp_key_min(m, __ballot_sync(FULL, key == best), p, leaf * LEAF + lane, lane);
+                cidx = leaf * LEAF + src;
+                if (best == __float_as_uint(kb.w)) {            // rare: ties the k-th best -- enters only with a smaller key
+                    const int kth = __shfl_sync(FULL, kb.idx, kb.cap() - 1);
+                    if (kth < 0 || !key_less(m, cidx, kth)) break;      // the smallest tied key does not: no tied point does
+                }
+            }
             // a walk seeded with candidates found elsewhere (knn_block) meets them again here: never list a slot twice
-            if (!__any_sync(FULL, lane < kb.cap() && kb.idx == cidx)) kb.insert(__uint_as_float(best), cidx, lane);
+            if (!__any_sync(FULL, lane < kb.cap() && kb.idx == cidx)) kb.insert(__uint_as_float(best), cidx, lane, m);
             if (lane == src) key = INF_BITS;
         }
         leaf = nxt;
@@ -173,7 +271,9 @@ __device__ __forceinline__ void knn_leaf(const MapView& m, int leaf, float qx, f
 // return -- the pruning rule of KD_TREE::Search (ikd_Tree.cpp:1097-1243).  The ordering key is
 // the box distance with its low 5 mantissa bits traded for the lane id; a child is skipped only
 // when even that rounded-DOWN distance is not below the k-th best, so pruning never drops a
-// child that could matter (it may visit one whose distance ties the bound within 2^-18).
+// child that could matter (it may visit one whose distance ties the bound within 2^-18).  Under the keyed
+// rule a point at exactly the k-th distance can still enter, so a child is skipped only when its rounded-down
+// distance is strictly above the bound.
 template <int L, class KB = KBest>
 __device__ __forceinline__ void knn_node(const MapView& m, int node, float qx, float qy, float qz,
                                          KB& kb, int lane) {
@@ -187,7 +287,8 @@ __device__ __forceinline__ void knn_node(const MapView& m, int node, float qx, f
 #pragma unroll 1
     while (true) {
         const unsigned best = __reduce_min_sync(FULL, key);
-        if ((best & ~31u) >= __float_as_uint(kb.w)) break;
+        // keyed: a box at exactly the bound may hold a winner; one at +inf (an empty entity, or nothing left) never does
+        if (KB::det ? (best & ~31u) > __float_as_uint(kb.w) || (best & ~31u) >= INF_BITS : (best & ~31u) >= __float_as_uint(kb.w)) break;
         const int c = best & 31;
         if (lane == c) key = 0xffffffffu;
         if constexpr (L == 1) knn_leaf<KB>(m, node * FAN + c, qx, qy, qz, kb, lane);
@@ -214,7 +315,7 @@ __device__ __forceinline__ void knn_root(const MapView& m, float qx, float qy, f
 #pragma unroll 1
     while (true) {
         const unsigned best = __reduce_min_sync(FULL, min(k0, k1));
-        if ((best & ~63u) >= __float_as_uint(kb.w)) break;
+        if (KB::det ? (best & ~63u) > __float_as_uint(kb.w) || (best & ~63u) >= INF_BITS : (best & ~63u) >= __float_as_uint(kb.w)) break;
         const int c = best & 63;
         if (lane == (c & 31)) { if (c < 32) k0 = 0xffffffffu; else k1 = 0xffffffffu; }
         if constexpr (L == 1) knn_leaf<KB>(m, c, qx, qy, qz, kb, lane);
@@ -236,7 +337,8 @@ __device__ __forceinline__ void knn_query_from(const MapView& m, float qx, float
     }
 }
 
-__device__ __forceinline__ void knn_query(const MapView& m, float qx, float qy, float qz, KBest& kb, int lane) {
+template <bool DET = false>
+__device__ __forceinline__ void knn_query(const MapView& m, float qx, float qy, float qz, KBestT<DET>& kb, int lane) {
     kb.init();
     knn_query_from(m, qx, qy, qz, kb, lane);
 }
@@ -335,29 +437,51 @@ __device__ __forceinline__ unsigned cell_slot(unsigned long long key, unsigned c
     return __umulhi((unsigned)(h >> 32) ^ (unsigned)h, cap);
 }
 
-struct TBest {                       // k best of one thread, ascending; empty entries: (+inf, -1)
+template <bool DET>
+struct TBestT {                      // k best of one thread, ascending; empty entries: (+inf, -1)
     float d[KNN_K];
     int idx[KNN_K];
     __device__ __forceinline__ void init() {
 #pragma unroll
         for (int i = 0; i < KNN_K; i++) { d[i] = INFINITY; idx[i] = -1; }
     }
-    __device__ __forceinline__ void insert(float nd, int nidx) {       // nd < d[K-1]; equal distances keep their arrival order
+    // the candidate ranks before the k-th entry: it enters the list
+    __device__ __forceinline__ bool admits(const MapView& m, float nd, int nidx) const {
+        if constexpr (DET) return key_before(m, nd, nidx, d[KNN_K - 1], idx[KNN_K - 1]);
+        else return nd < d[KNN_K - 1];
+    }
+    // admits(nd, nidx); equal distances keep their arrival order (DET: their key order)
+    __device__ __forceinline__ void insert(float nd, int nidx, const MapView& m) {
         // a halo list may name a slot twice (a slot re-used by a later insert keeps its old listings): never keep it twice
         bool dup = false;
 #pragma unroll
         for (int i = 0; i < KNN_K; i++) dup |= idx[i] == nidx;
         if (dup) return;
+        if constexpr (!DET) {
 #pragma unroll
-        for (int i = KNN_K - 1; i > 0; i--) {
-            const bool shift = nd < d[i - 1];
-            const bool here = !shift && nd < d[i];
-            d[i] = shift ? d[i - 1] : (here ? nd : d[i]);
-            idx[i] = shift ? idx[i - 1] : (here ? nidx : idx[i]);
+            for (int i = KNN_K - 1; i > 0; i--) {
+                const bool shift = nd < d[i - 1];
+                const bool here = !shift && nd < d[i];
+                d[i] = shift ? d[i - 1] : (here ? nd : d[i]);
+                idx[i] = shift ? idx[i - 1] : (here ? nidx : idx[i]);
+            }
+            if (nd < d[0]) { d[0] = nd; idx[0] = nidx; }
+        } else {
+            bool lt[KNN_K];
+#pragma unroll
+            for (int i = 0; i < KNN_K; i++) lt[i] = key_before(m, nd, nidx, d[i], idx[i]);
+#pragma unroll
+            for (int i = KNN_K - 1; i > 0; i--) {
+                const bool shift = lt[i - 1];
+                const bool here = !shift && lt[i];
+                d[i] = shift ? d[i - 1] : (here ? nd : d[i]);
+                idx[i] = shift ? idx[i - 1] : (here ? nidx : idx[i]);
+            }
+            if (lt[0]) { d[0] = nd; idx[0] = nidx; }
         }
-        if (nd < d[0]) { d[0] = nd; idx[0] = nidx; }
     }
 };
+using TBest = TBestT<false>;
 
 // the entry of cell `key`: (start, cnt) of its halo list.  Returns 1: usable; 0: no entry (no point within a cell's width of
 // that cell); -1: over-full (or being set up) -- the BVH walk must answer
@@ -379,17 +503,19 @@ __device__ __forceinline__ int cell_list(const CellDir& D, unsigned long long ke
 }
 
 // one candidate (a deleted point keeps its listings: it is skipped by its flag)
-__device__ __forceinline__ void cell_consider(const float4& p, int idx, float qx, float qy, float qz, TBest& kb) {
+template <bool DET>
+__device__ __forceinline__ void cell_consider(const MapView& m, const float4& p, int idx, float qx, float qy, float qz, TBestT<DET>& kb) {
     if (slot_valid(p)) {
         const float dd = sq_dist3(qx, qy, qz, p.x, p.y, p.z);
-        if (dd < kb.d[KNN_K - 1]) kb.insert(dd, idx);
+        if (kb.admits(m, dd, idx)) kb.insert(dd, idx, m);
     }
 }
 
 // Score the halo list [start, start + cnt), eight candidates at a time: their point loads are issued together and the indices of
 // the next eight are fetched while these are scored (a scan is only a few warps per SM: the chain of dependent loads of one
 // thread IS the run time -- probe, first indices, then one round trip per eight candidates).
-__device__ __forceinline__ void cell_scan_list(const MapView& m, int start, int cnt, float qx, float qy, float qz, TBest& kb) {
+template <bool DET>
+__device__ __forceinline__ void cell_scan_list(const MapView& m, int start, int cnt, float qx, float qy, float qz, TBestT<DET>& kb) {
     const int4* list = reinterpret_cast<const int4*>(m.dir.lists + start);
     const int nchunks = (cnt + 7) >> 3;
     int4 ia = __ldg(&list[0]), ib = make_int4(0, 0, 0, 0);
@@ -410,14 +536,14 @@ __device__ __forceinline__ void cell_scan_list(const MapView& m, int start, int 
         int4 na = ia, nb = ib;
         if (n8 > 8) na = __ldg(&list[2 * c + 2]);
         if (n8 > 12) nb = __ldg(&list[2 * c + 3]);
-        cell_consider(p0, ia.x, qx, qy, qz, kb);
-        cell_consider(p1, ia.y, qx, qy, qz, kb);
-        cell_consider(p2, ia.z, qx, qy, qz, kb);
-        cell_consider(p3, ia.w, qx, qy, qz, kb);
-        cell_consider(p4, ib.x, qx, qy, qz, kb);
-        cell_consider(p5, ib.y, qx, qy, qz, kb);
-        cell_consider(p6, ib.z, qx, qy, qz, kb);
-        cell_consider(p7, ib.w, qx, qy, qz, kb);
+        cell_consider(m, p0, ia.x, qx, qy, qz, kb);
+        cell_consider(m, p1, ia.y, qx, qy, qz, kb);
+        cell_consider(m, p2, ia.z, qx, qy, qz, kb);
+        cell_consider(m, p3, ia.w, qx, qy, qz, kb);
+        cell_consider(m, p4, ib.x, qx, qy, qz, kb);
+        cell_consider(m, p5, ib.y, qx, qy, qz, kb);
+        cell_consider(m, p6, ib.z, qx, qy, qz, kb);
+        cell_consider(m, p7, ib.w, qx, qy, qz, kb);
         ia = na; ib = nb;
     }
 }
@@ -436,8 +562,10 @@ __device__ __forceinline__ float cell_block_dist(const CellDir& D, float qx, flo
     return fminf(fminf(gx, gy), gz);
 }
 
-// k-NN of one query by one thread.  Returns true when kb is PROVEN to be the exact answer.
-__device__ __forceinline__ bool cell_knn(const MapView& m, float qx, float qy, float qz, TBest& kb) {
+// k-NN of one query by one thread.  Returns true when kb is PROVEN to be the exact answer.  The proof is strict: a point
+// outside the block is farther than the k-th best, so it can neither be closer nor tie it (the keyed rule admits ties).
+template <bool DET>
+__device__ __forceinline__ bool cell_knn(const MapView& m, float qx, float qy, float qz, TBestT<DET>& kb) {
     const CellDir& D = m.dir;
     kb.init();
     if (D.cap == 0u) return false;
@@ -468,7 +596,8 @@ struct WalkPool {
     float rd[WALK_POOL][KNN_K];    // in: the k candidates the thread search found (a bound for the walk; +inf / -1 when it found fewer); out: the answer
     int ri[WALK_POOL][KNN_K];
 };
-__device__ __forceinline__ void knn_block(const MapView& m, bool active, float qx, float qy, float qz, TBest& kb, WalkPool& W, int& phase) {
+template <bool DET>
+__device__ __forceinline__ void knn_block(const MapView& m, bool active, float qx, float qy, float qz, TBestT<DET>& kb, WalkPool& W, int& phase) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
     bool exact = true;
     if (active) exact = cell_knn(m, qx, qy, qz, kb);
@@ -491,7 +620,7 @@ __device__ __forceinline__ void knn_block(const MapView& m, bool active, float q
     for (int i = warp; i < n; i += nwarps) {
         // the walk starts from what the thread search found: with the k-th distance as its bound it only enters boxes that cut
         // the known ball (a handful of dependent loads instead of a full descent)
-        KBest w;
+        KBestT<DET> w;
         w.init();
         if (lane < KNN_K) { w.d = W.rd[i][lane]; w.idx = W.ri[i][lane]; }
         w.w = __shfl_sync(FULL, w.d, KNN_K - 1);
@@ -505,7 +634,7 @@ __device__ __forceinline__ void knn_block(const MapView& m, bool active, float q
     while (todo) {
         const int src = __ffs(todo) - 1;
         todo &= todo - 1;
-        KBest w;
+        KBestT<DET> w;
         knn_query(m, __shfl_sync(FULL, qx, src), __shfl_sync(FULL, qy, src), __shfl_sync(FULL, qz, src), w, lane);
 #pragma unroll
         for (int j = 0; j < KNN_K; j++) {
@@ -523,8 +652,10 @@ __device__ __forceinline__ void knn_block(const MapView& m, bool active, float q
 }
 
 // The neighbours as the caller sees them: coordinates + intensity, nearest first; candidates whose squared distances
-// differ by less than 1e-10 are ordered by x like PointType_CMP does for the reference's heap (ikd_Tree.h:102-108).
-__device__ __forceinline__ int knn_fetch(const MapView& m, TBest& kb, float4 (&p)[KNN_K]) {
+// differ by less than 1e-10 are ordered by x like PointType_CMP does for the reference's heap (ikd_Tree.h:102-108).  DET: those
+// with equal x as well by (y, z, intensity), so the order is a function of the neighbours alone.
+template <bool DET>
+__device__ __forceinline__ int knn_fetch(const MapView& m, TBestT<DET>& kb, float4 (&p)[KNN_K]) {
     int cnt = 0;
 #pragma unroll
     for (int j = 0; j < KNN_K; j++) {
@@ -539,7 +670,8 @@ __device__ __forceinline__ int knn_fetch(const MapView& m, TBest& kb, float4 (&p
         for (int pass = 0; pass < KNN_K - 1; pass++) {
 #pragma unroll
             for (int j = 0; j + 1 < KNN_K - pass; j++) {
-                if (kb.idx[j + 1] >= 0 && fabsf(kb.d[j + 1] - kb.d[j]) < 1e-10f && p[j + 1].x < p[j].x) {
+                if (kb.idx[j + 1] >= 0 && fabsf(kb.d[j + 1] - kb.d[j]) < 1e-10f &&
+                    (p[j + 1].x < p[j].x || (DET && p[j + 1].x == p[j].x && yzi_less(p[j + 1], p[j])))) {
                     const float4 tp = p[j]; p[j] = p[j + 1]; p[j + 1] = tp;
                     const float td = kb.d[j]; kb.d[j] = kb.d[j + 1]; kb.d[j + 1] = td;
                     const int ti = kb.idx[j]; kb.idx[j] = kb.idx[j + 1]; kb.idx[j + 1] = ti;
@@ -570,7 +702,11 @@ __device__ __forceinline__ int knn_fetch_warp(const MapView& m, KB& kb, float4& 
             const bool both = partner >= 0 && lane < cnt && partner < cnt;
             if (both && fabsf(od - kb.d) < 1e-10f) {
                 const bool lower = lane < partner;                                    // the lower lane keeps the smaller x
-                const bool take = lower ? (ox < p.x) : (ox > p.x);
+                bool take = lower ? (ox < p.x) : (ox > p.x);
+                if constexpr (KB::det) {
+                    const float4 o = make_float4(ox, oy, oz, ow);
+                    if (ox == p.x) take = lower ? yzi_less(o, p) : yzi_less(p, o);
+                }
                 if (take) { kb.d = od; kb.idx = oi; p = make_float4(ox, oy, oz, ow); }
             }
         }
@@ -583,7 +719,8 @@ __device__ __forceinline__ int knn_fetch_warp(const MapView& m, KB& kb, float4& 
 // list is PROVEN to be the exact answer: every point outside the block is at least g away (cell_block_dist), so the list is
 // final when it holds k entries and the k-th is below g^2, or when md2 < g^2 (every admissible point lies in the block, however
 // few there are).  Otherwise the list seeds the BVH walk (knn_query_from), which only adds what the block did not hold.
-__device__ __forceinline__ bool knn_seed_k(const MapView& m, float qx, float qy, float qz, float md2, KBestK& kb, int lane) {
+template <bool DET>
+__device__ __forceinline__ bool knn_seed_k(const MapView& m, float qx, float qy, float qz, float md2, KBestKT<DET>& kb, int lane) {
     const CellDir& D = m.dir;
     if (D.cap == 0u) return false;
     const float inv = D.inv_cell;
@@ -599,19 +736,31 @@ __device__ __forceinline__ bool knn_seed_k(const MapView& m, float qx, float qy,
     for (int b = 0; b < cnt; b += 32) {
         unsigned key = INF_BITS;
         int slot = -1;
+        float4 p = make_float4(0.f, 0.f, 0.f, 0.f);
         if (b + lane < cnt) {
             slot = __ldg(&D.lists[start + b + lane]);
-            const float4 p = __ldg(&m.pts[slot]);
+            p = __ldg(&m.pts[slot]);
             if (slot_valid(p)) key = __float_as_uint(sq_dist3(qx, qy, qz, p.x, p.y, p.z));
         }
 #pragma unroll 1
         while (true) {
             const unsigned best = __reduce_min_sync(FULL, key);
-            if (best >= __float_as_uint(kb.w)) break;
-            const int src = __ffs(__ballot_sync(FULL, key == best)) - 1;
-            const int cidx = __shfl_sync(FULL, slot, src);
+            int src, cidx;
+            if constexpr (!DET) {
+                if (best >= __float_as_uint(kb.w)) break;
+                src = __ffs(__ballot_sync(FULL, key == best)) - 1;
+                cidx = __shfl_sync(FULL, slot, src);
+            } else {                                    // the keyed rule, as in knn_leaf
+                if (best > __float_as_uint(kb.w) || best == INF_BITS) break;
+                src = warp_key_min(m, __ballot_sync(FULL, key == best), p, slot, lane);
+                cidx = __shfl_sync(FULL, slot, src);
+                if (best == __float_as_uint(kb.w)) {
+                    const int kth = __shfl_sync(FULL, kb.idx, kb.k - 1);
+                    if (kth < 0 || !key_less(m, cidx, kth)) break;
+                }
+            }
             // a list may name a slot twice: never list it twice
-            if (!__any_sync(FULL, lane < kb.k && kb.idx == cidx)) kb.insert(__uint_as_float(best), cidx, lane);
+            if (!__any_sync(FULL, lane < kb.k && kb.idx == cidx)) kb.insert(__uint_as_float(best), cidx, lane, m);
             if (lane == src) key = INF_BITS;
         }
     }

@@ -105,6 +105,9 @@ public:
     int size() const { return n_valid_ + n_tomb_; }       // KD_TREE::size()  (valid + lazily deleted; settle(false) first)
     int validnum() const { return n_valid_; }             // KD_TREE::validnum()
     void set_downsample(float v) { downsample_ = v; }
+    // the keyed tie rule of k-NN and down-sampling (map.cuh, "tie rules") and flatten's sorted rows; waits for the stream first
+    int set_deterministic(bool on);
+    bool deterministic() const { return det_; }
     float downsample() const { return downsample_; }
     int tree_range(float* box6);
 
@@ -171,6 +174,7 @@ private:
     bool record_removed_ = false;
     int n_removed_ = 0;
     bool dir_enabled_ = true;
+    bool det_ = false;          // fl_map_set_deterministic
     float cell_override_ = 0.f;           // 0: cell edge = 2 x downsample size
     size_t dir_min_cap_ = 0, dir_min_pool_ = 0;
     int n_dir_rebuilds_ = 0;

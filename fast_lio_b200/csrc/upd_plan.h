@@ -25,13 +25,15 @@ struct UpdPlan {
     int grid_x, slots, waves;  // workers + 1; batch: hypotheses per wave (0: one does not fit) and waves for n_hyp, else 1 and 1
     int block, smem;           // threads per block, dynamic shared memory bytes
     bool pdl;                  // may overlap its predecessor (programmatic dependent launch, when the filter has it on)
+    bool det;                  // the keyed-tie-rule instantiation of `kernel` (the map's deterministic mode)
 };
 
 // Every co-resident block works (a searching pass wants many warps in flight), one thread per point in full warps.  Two threads
 // per point when the tiles all fit the co-resident 512-thread grid, so the tiles, workers and partial rows are those of the
 // one-thread form; larger scans keep one thread per point rather than idle half the warps on passes that do not search, and
-// one_thread (FASTLIO_B200_PAIR=1) forces it.  The paired mode-0 update runs the wave kernel when its grid fits.
-inline UpdPlan plan_update(const UpdCaps& c, UpdRoute r, int rows, bool extr, bool one_thread, int n_hyp = 0) {
+// one_thread (FASTLIO_B200_PAIR=1) forces it.  The paired mode-0 update runs the wave kernel when its grid fits.  det picks the
+// keyed-tie-rule instantiation of the same kernel: same grid, block and shared memory (its caps are those of both forms).
+inline UpdPlan plan_update(const UpdCaps& c, UpdRoute r, int rows, bool extr, bool one_thread, int n_hyp = 0, bool det = false) {
     auto cap = [&](UpdKernel k) { return c.blocks[k][extr ? 1 : 0]; };
     const int tiles = (rows + c.threads - 1) / c.threads;
     UpdPlan p{};
@@ -59,6 +61,7 @@ inline UpdPlan plan_update(const UpdCaps& c, UpdRoute r, int rows, bool extr, bo
     p.grid_x = p.workers + 1;
     p.block = p.pair * c.threads;
     p.smem = p.kernel == UK_WAVE || p.kernel == UK_N_WAVE ? c.wave_smem : 0;
+    p.det = det;
     return p;
 }
 

@@ -119,7 +119,8 @@ __device__ __forceinline__ void pub_publish(unsigned long long* pub, unsigned ta
 // be in the answer (tests/test_update_pair_merge.py checks the rule on the CPU).
 
 // cell_scan_list over the chunks [c0, c1) of the halo list [start, start + cnt)
-__device__ __forceinline__ void cell_scan_chunks(const MapView& m, int start, int cnt, int c0, int c1, float qx, float qy, float qz, TBest& kb) {
+template <bool DET>
+__device__ __forceinline__ void cell_scan_chunks(const MapView& m, int start, int cnt, int c0, int c1, float qx, float qy, float qz, TBestT<DET>& kb) {
     const int4* list = reinterpret_cast<const int4*>(m.dir.lists + start);
     int4 ia = make_int4(0, 0, 0, 0), ib = make_int4(0, 0, 0, 0);
     if (c0 < c1) {
@@ -144,14 +145,14 @@ __device__ __forceinline__ void cell_scan_chunks(const MapView& m, int start, in
             na = __ldg(&list[2 * c + 2]);
             if (n8 > 12) nb = __ldg(&list[2 * c + 3]);
         }
-        cell_consider(p0, ia.x, qx, qy, qz, kb);
-        cell_consider(p1, ia.y, qx, qy, qz, kb);
-        cell_consider(p2, ia.z, qx, qy, qz, kb);
-        cell_consider(p3, ia.w, qx, qy, qz, kb);
-        cell_consider(p4, ib.x, qx, qy, qz, kb);
-        cell_consider(p5, ib.y, qx, qy, qz, kb);
-        cell_consider(p6, ib.z, qx, qy, qz, kb);
-        cell_consider(p7, ib.w, qx, qy, qz, kb);
+        cell_consider(m, p0, ia.x, qx, qy, qz, kb);
+        cell_consider(m, p1, ia.y, qx, qy, qz, kb);
+        cell_consider(m, p2, ia.z, qx, qy, qz, kb);
+        cell_consider(m, p3, ia.w, qx, qy, qz, kb);
+        cell_consider(m, p4, ib.x, qx, qy, qz, kb);
+        cell_consider(m, p5, ib.y, qx, qy, qz, kb);
+        cell_consider(m, p6, ib.z, qx, qy, qz, kb);
+        cell_consider(m, p7, ib.w, qx, qy, qz, kb);
         ia = na; ib = nb;
     }
 }
@@ -164,12 +165,15 @@ struct PairXch {
 
 // The owner's merge: its TBest holds what cell_scan_list holds after the owner's chunks; the partner's entries go in after
 // them, in the partner's order, through the same insert (equal distances keep their arrival order, a held slot is refused).
-__device__ __forceinline__ void pair_merge(const PairXch& X, int lane, TBest& kb) {
+// DET: the insert ranks by the keyed order, so the merge is the k smallest of both lists under it -- the answer of the whole
+// list's scan, since a listing the partner dropped has k distinct slots ahead of it under that order.
+template <bool DET>
+__device__ __forceinline__ void pair_merge(const MapView& m, const PairXch& X, int lane, TBestT<DET>& kb) {
 #pragma unroll
     for (int j = 0; j < KNN_K; j++) {
         const float d = X.d[j][lane];
         const int i = X.idx[j][lane];
-        if (i >= 0 && d < kb.d[KNN_K - 1]) kb.insert(d, i);
+        if (i >= 0 && kb.admits(m, d, i)) kb.insert(d, i, m);
     }
 }
 
@@ -179,7 +183,8 @@ __device__ __forceinline__ void pair_sync(int warp) { asm volatile("bar.sync %0,
 // knn_block for the 512-thread block: every thread calls it; kb is the answer for owners (threadIdx.x < UPD_THREADS), the
 // partner's kb is undefined.  The thread search is the paired scan above; what it cannot prove goes through the same walk pool,
 // walked by all 16 warps, and pool overflow is walked by the owner's warp.  `stage` is the owner warp's stage slice.
-__device__ __forceinline__ void knn_block_pair(const MapView& m, bool active, float qx, float qy, float qz, TBest& kb, WalkPool& W,
+template <bool DET>
+__device__ __forceinline__ void knn_block_pair(const MapView& m, bool active, float qx, float qy, float qz, TBestT<DET>& kb, WalkPool& W,
                                                int& phase, double* stage) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
     const bool owner = threadIdx.x < UPD_THREADS;
@@ -210,7 +215,7 @@ __device__ __forceinline__ void knn_block_pair(const MapView& m, bool active, fl
     if (owner && active) {
         exact = false;
         if (listed) {
-            pair_merge(X, lane, kb);
+            pair_merge(m, X, lane, kb);
             if (kb.idx[KNN_K - 1] >= 0) {
                 const float g = cell_block_dist(D, qx, qy, qz, ix, iy, iz);
                 exact = kb.d[KNN_K - 1] < g * g;
@@ -234,7 +239,7 @@ __device__ __forceinline__ void knn_block_pair(const MapView& m, bool active, fl
     if (threadIdx.x == 0) W.n[(phase + 1) & 1] = 0;
     phase++;
     for (int i = warp; i < n; i += nwarps) {
-        KBest w;
+        KBestT<DET> w;
         w.init();
         if (lane < KNN_K) { w.d = W.rd[i][lane]; w.idx = W.ri[i][lane]; }
         w.w = __shfl_sync(FULL, w.d, KNN_K - 1);
@@ -247,7 +252,7 @@ __device__ __forceinline__ void knn_block_pair(const MapView& m, bool active, fl
     while (todo) {
         const int src = __ffs(todo) - 1;
         todo &= todo - 1;
-        KBest w;
+        KBestT<DET> w;
         knn_query(m, __shfl_sync(FULL, qx, src), __shfl_sync(FULL, qy, src), __shfl_sync(FULL, qz, src), w, lane);
 #pragma unroll
         for (int j = 0; j < KNN_K; j++) {
@@ -270,7 +275,7 @@ __device__ __forceinline__ void knn_block_pair(const MapView& m, bool active, fl
 // straight into the plane fit; they are stored once (map_incremental reads them, laserMapping.cpp:438-460).  Returns true when
 // the point contributes a row.  PAIR = 2: the partner threads (threadIdx.x >= UPD_THREADS) call it on searching passes only,
 // for the paired search, and return false.
-template <bool EXTR, int PAIR>
+template <bool EXTR, int PAIR, bool DET>
 __device__ __forceinline__ bool measure_fused(const MapView& m, const ScanView& sc, int q, bool active, const PoseS& s, bool searched,
                                               bool search_only, WalkPool& walks, int& phase, double* stage, double* h, double& z, float& absres) {
     float4 pb = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -283,7 +288,7 @@ __device__ __forceinline__ bool measure_fused(const MapView& m, const ScanView& 
     bool sel = false;
     float pabcd[4] = {0.f, 0.f, 0.f, 0.f};
     if (searched) {                                                         // :667
-        TBest kb;
+        TBestT<DET> kb;
         if constexpr (PAIR == 1) {
             knn_block(m, active, wx, wy, wz, kb, walks, phase);                    // :670 (block-wide: two barriers)
         } else {
@@ -683,7 +688,7 @@ __device__ void sol_pass(SolverSm& S, FilterCtl* ctl, PassLog* logs, unsigned lo
 // PAIR = 1, so both forms give the same bytes.
 // The body is shared by k_update (the scan's points [q_begin, q_end)) and k_update_n (a point count in device memory): q1 is
 // the end of the points the workers measure.
-template <bool EXTR, int PAIR>
+template <bool EXTR, int PAIR, bool DET = false>
 __device__ __forceinline__ void update_body(const UpdArgs& a, const int q1) {
     static_assert(PAIR == 1 || PAIR == 2, "one or two threads per point");
     static_assert(sizeof(PairXch) <= sizeof(double) * WorkerSm<EXTR>::STAGE, "the partner's list fits the owner warp's stage slice");
@@ -748,7 +753,7 @@ __device__ __forceinline__ void update_body(const UpdArgs& a, const int q1) {
                 double h[12]; double z = 0.0; float ar = 0.f;
                 bool contrib = false;
                 if (owner || searched)
-                    contrib = measure_fused<EXTR, PAIR>(a.m, a.sc, q, q < q1, s, searched, a.search_only != 0, Wk.walks, walk_phase, stage, h, z, ar);
+                    contrib = measure_fused<EXTR, PAIR, DET>(a.m, a.sc, q, q < q1, s, searched, a.search_only != 0, Wk.walks, walk_phase, stage, h, z, ar);
                 if (owner && !a.search_only) warp_accumulate<EXTR>(contrib, h, z, ar, acc, lane, stage);
             }
             if (a.search_only) return;
@@ -834,8 +839,8 @@ __global__ void __launch_bounds__(UPD_THREADS * PAIR, 3 - PAIR) k_update_n(UpdAr
 // values here rather than kernel parameters, so ptxas spills a little more (sm_90a, nvcc 12.9: stack 336 / 392 bytes against
 // 288 for EXTR false / true, spill stores + loads 508 / 716 bytes against 352 / 496).
 constexpr int BATCH_PUB_WORDS = 32;      // 256 bytes per slot
-template <bool EXTR>
-__global__ void __launch_bounds__(UPD_THREADS, 2) k_update_batch(UpdArgs a, int log_stride) {
+template <bool EXTR, bool DET = false>
+__device__ __forceinline__ void update_batch_body(UpdArgs& a, int log_stride) {
     const int s = (int)blockIdx.y;
     const size_t rows = (size_t)s * (size_t)a.sc.Q;
     a.ctl += s;
@@ -847,7 +852,11 @@ __global__ void __launch_bounds__(UPD_THREADS, 2) k_update_batch(UpdArgs a, int 
     a.sc.selected += rows;
     a.sc.plane += rows;
     a.sc.srange += rows;
-    update_body<EXTR, 1>(a, a.sc.q_end);
+    update_body<EXTR, 1, DET>(a, a.sc.q_end);
+}
+template <bool EXTR>
+__global__ void __launch_bounds__(UPD_THREADS, 2) k_update_batch(UpdArgs a, int log_stride) {
+    update_batch_body<EXTR>(a, log_stride);
 }
 
 // ============================================================================= one tile per worker block: k_update_wave
@@ -888,7 +897,7 @@ __device__ __forceinline__ bool row_current(ulonglong2 v, unsigned tag) { return
 __device__ __forceinline__ double row_value(ulonglong2 v) { return __longlong_as_double((long long)((v.y << 32) | (v.x & 0xffffffffull))); }
 
 // measure_fused<EXTR, 2> with the point's state in `pt` (slot threadIdx.x % 256); the same outputs in memory
-template <bool EXTR>
+template <bool EXTR, bool DET>
 __device__ __forceinline__ bool measure_wave(const MapView& m, const ScanView& sc, int q, bool active, const PoseS& s, bool searched,
                                              bool search_only, WalkPool& walks, int& phase, double* stage, WavePoint& pt, double* h,
                                              double& z, float& absres) {
@@ -903,7 +912,7 @@ __device__ __forceinline__ bool measure_wave(const MapView& m, const ScanView& s
     bool sel = false;
     float pabcd[4] = {0.f, 0.f, 0.f, 0.f};
     if (searched) {
-        TBest kb;
+        TBestT<DET> kb;
         knn_block_pair(m, active, wx, wy, wz, kb, walks, phase, stage);
         if (threadIdx.x >= UPD_THREADS) return false;
         if (active) {
@@ -1008,7 +1017,7 @@ __device__ void sol_gather(SolverSm& S, FilterCtl* ctl, const unsigned long long
 
 // update_body<EXTR, 2> for mode 0 with one tile per worker block (gridDim.x - 1 >= the tiles of [q_begin, q1)); rows: the
 // partial rows as tagged words, [worker block][PSTRIDE][2]
-template <bool EXTR>
+template <bool EXTR, bool DET = false>
 __device__ __forceinline__ void update_wave_body(const UpdArgs& a, unsigned long long* __restrict__ rows, const int q1) {
     static_assert(sizeof(PairXch) <= sizeof(double) * WorkerSm<EXTR>::STAGE, "the partner's list fits the owner warp's stage slice");
     __shared__ __align__(16) unsigned char smem_raw[sizeof(SolverSm) > sizeof(WorkerSm<EXTR>) ? sizeof(SolverSm) : sizeof(WorkerSm<EXTR>)];
@@ -1080,7 +1089,7 @@ __device__ __forceinline__ void update_wave_body(const UpdArgs& a, unsigned long
             double h[12]; double z = 0.0; float ar = 0.f;
             bool contrib = false;
             if (owner || searched)
-                contrib = measure_wave<EXTR>(a.m, a.sc, q, active, s, searched, a.search_only != 0, Wk.walks, walk_phase, stage, pt, h, z, ar);
+                contrib = measure_wave<EXTR, DET>(a.m, a.sc, q, active, s, searched, a.search_only != 0, Wk.walks, walk_phase, stage, pt, h, z, ar);
             if (owner && !a.search_only) warp_accumulate<EXTR>(contrib, h, z, ar, acc, lane, stage);
             if (a.search_only) return;
             if (owner) {
@@ -1147,6 +1156,30 @@ __global__ void __launch_bounds__(2 * UPD_THREADS, 1) k_update_wave(UpdArgs a, u
 template <bool EXTR>
 __global__ void __launch_bounds__(2 * UPD_THREADS, 1) k_update_n_wave(UpdArgs a, const int* __restrict__ n, unsigned long long* rows) {
     update_wave_body<EXTR>(a, rows, min(*n, a.sc.q_end));
+}
+
+// ============================================================================= the keyed tie rule (fl_map_set_deterministic)
+// Every update kernel above again, searching the map under the keyed order (map.cuh, "tie rules"): same bounds, same shared
+// memory, same tiles and sums, so the launch plan's grids hold for them.  Kernels of their own, so the default ones keep their code.
+template <bool EXTR, int PAIR>
+__global__ void __launch_bounds__(UPD_THREADS * PAIR, 3 - PAIR) k_update_det(UpdArgs a) {
+    update_body<EXTR, PAIR, true>(a, a.sc.q_end);
+}
+template <bool EXTR, int PAIR>
+__global__ void __launch_bounds__(UPD_THREADS * PAIR, 3 - PAIR) k_update_n_det(UpdArgs a, const int* __restrict__ n) {
+    update_body<EXTR, PAIR, true>(a, min(*n, a.sc.q_end));
+}
+template <bool EXTR>
+__global__ void __launch_bounds__(UPD_THREADS, 2) k_update_batch_det(UpdArgs a, int log_stride) {
+    update_batch_body<EXTR, true>(a, log_stride);
+}
+template <bool EXTR>
+__global__ void __launch_bounds__(2 * UPD_THREADS, 1) k_update_wave_det(UpdArgs a, unsigned long long* rows) {
+    update_wave_body<EXTR, true>(a, rows, a.sc.q_end);
+}
+template <bool EXTR>
+__global__ void __launch_bounds__(2 * UPD_THREADS, 1) k_update_n_wave_det(UpdArgs a, const int* __restrict__ n, unsigned long long* rows) {
+    update_wave_body<EXTR, true>(a, rows, min(*n, a.sc.q_end));
 }
 
 }  // namespace fl

@@ -216,6 +216,32 @@ int fl_map_stats(fl_map_t* m, int* out4);
  * those of KD_TREE::Nearest_Search either way).  on = 0 answers every query through the BVH walk; cell_size <= 0 picks
  * 2 x downsample_size.  Takes effect immediately (the directory is re-listed). */
 int fl_map_set_cell_directory(fl_map_t* m, int on, float cell_size);
+/* Deterministic mode (off by default; no reference counterpart).  With it on, every answer that reaches the caller or the
+ * filter's state is a function of the SET of valid points -- compared as (x, y, z, intensity) bits -- not of the slots they
+ * occupy, which racing inserts, deletes and re-lists make differ from run to run.  For maps holding the same valid points,
+ * whatever the history of Build / Add_Points / Delete_Point_Boxes / Add_Point_Boxes / maintenance that produced them:
+ *   - k-NN (fl_map_knn, fl_map_nearest_search and its _device form, every k and max_dist, and the neighbours every update
+ *     kernel finds): the returned set is the k smallest under the total order (d2, x, y, z, intensity), d2 the float32 the
+ *     kernels compute and the other keys breaking its bit-equal ties, each compared as an order-preserving integer of its bits
+ *     (-0 below +0).  The order is the usual one: ascending d2, candidates within 1e-10 by x (PointType_CMP), and entries equal
+ *     on both by (y, z, intensity).  The output bytes are equal across such maps.
+ *   - Add_Points with down-sampling: of the valid points of a voxel at equal distance from its centre, the one with the
+ *     smallest (x, y, z, intensity) counts as the nearest; batch points keep their input order.  The same prior point set and
+ *     batch give the same resulting point set and return value.
+ *   - Updates (fl_filter_update, its _device, _scan_device and _batch_device forms, map_incremental in both forms) read the
+ *     map only through these two rules, so x, P, pass logs, Nearest_Points and selected are equal bit for bit across such
+ *     maps and from run to run.  The update runs the fused kernels only: a filter on solver mode 0 or the two-kernels-per-pass
+ *     chain (fl_filter_set_fused 0) fails with FL_ERR_STATE.
+ *   - fl_map_flatten returns its rows sorted by (x, y, z, intensity) bits, so a map written to disk is byte-stable.
+ * Not covered: the row order of Box_Search / Radius_Search (their sets are already equal), the order of
+ * fl_map_acquire_removed, slot layout, fl_map_size (it counts lazily deleted slots) and sharded filters beyond what the
+ * same rules give them.  The mode differs from the reference only where the reference itself is arbitrary: bit-equal d2 and x
+ * at the k-th place, and equal distances to a voxel centre.
+ * The setter waits for the handle's stream, then switches; it takes no stream, so it cannot be called from inside a capture.
+ * Filters and scans created on the map follow its mode at every launch; a captured graph keeps the kernels of capture time,
+ * so capture again after switching (as after fl_filter_set_params).  A null handle (or output) is FL_ERR_ARG. */
+int fl_map_set_deterministic(fl_map_t* m, int on);
+int fl_map_get_deterministic(fl_map_t* m, int* on);
 /* [0] cells [1] external buckets [2] crowded cells (queries touching them use the BVH walk) [3] table capacity
  * [4] directory re-lists triggered by inserts [5] queries answered by the BVH walk since the last call (-1: directory off) */
 int fl_map_dir_stats(fl_map_t* m, int* out6);

@@ -33,6 +33,9 @@
 //   acquire_removed_points(PointVector&)     fl_map_acquire_removed: the points removed by Delete_Point_Boxes since the last call
 //                                            (the reference hands them over when it rebuilds the subtree; here at once)
 //   Root_Node                                non-null once built (laserMapping.cpp:909 tests it)
+//   (extension) set_deterministic(bool)      fl_map_set_deterministic: k-NN answers, the down-sampling survivor and the
+//                                            update depend only on the map's point set; FASTLIO_B200_DETERMINISTIC=1 turns
+//                                            it on at construction
 //
 // Limits and failure reporting (the reference's members return void / int and cannot fail):
 //   * k_nearest <= 5 (NUM_MATCH_POINTS, include/common_lib.h:26 -- the only k FAST-LIO uses).  A larger k is an error:
@@ -78,7 +81,15 @@ public:
             fprintf(stderr, "KD_TREE(H100): cannot create the device map on CUDA device %d: %s\n", dev, fl_last_error());
             map_ = nullptr;
             failed_ = true;
+        } else if (const char* d = getenv("FASTLIO_B200_DETERMINISTIC")) {
+            if (d[0] == '1') set_deterministic(true);
         }
+    }
+    // extension: the deterministic mode (fl_map_set_deterministic); FASTLIO_B200_DETERMINISTIC=1 turns it on at construction
+    void set_deterministic(bool on) { if (map_) check(fl_map_set_deterministic(map_, on ? 1 : 0), "set_deterministic"); }
+    bool deterministic() const {
+        int on = 0;
+        return map_ && fl_map_get_deterministic(map_, &on) == FL_OK && on;
     }
     // extension: device selection and failure reporting (see the header comment)
     static void set_default_device(int device) { default_device() = device; }
