@@ -45,6 +45,34 @@ def decode_pass_logs(raw, passes: int) -> list:
     return [_log_dict(PassLog.from_buffer_copy(buf[i].tobytes())) for i in range(passes)]
 
 
+class RelocGrid(C.Structure):
+    """fl_reloc_grid_t: grid counts and steps on x, y, z (m) and yaw (rad)"""
+    _fields_ = [("n", C.c_int * 4), ("step", C.c_double * 4)]
+
+
+class RelocParams(C.Structure):
+    """fl_reloc_params_t"""
+    _fields_ = [("keep", C.c_int), ("stride", C.c_int), ("r_inlier", C.c_float), ("min_effct", C.c_int)]
+
+
+class RelocRow(C.Structure):
+    """fl_reloc_row_t: one survivor of a relocalisation's screen"""
+    _fields_ = [("hyp", C.c_int), ("inliers", C.c_int), ("status", C.c_int), ("passes", C.c_int), ("effct", C.c_int),
+                ("pad", C.c_int), ("res_sum", C.c_double)]
+
+
+RELOC_ROW = np.dtype({"names": ["hyp", "inliers", "status", "passes", "effct", "res_sum"],
+                      "formats": ["<i4"] * 5 + ["<f8"], "offsets": [0, 4, 8, 12, 16, 24], "itemsize": 32})
+
+
+def decode_reloc_rows(raw) -> np.ndarray:
+    """The rows of Esekf.relocalize_device (a (keep, sizeof(fl_reloc_row_t)) uint8 array or tensor) as a structured array with the
+    fields hyp, inliers, status, passes, effct and res_sum."""
+    if hasattr(raw, "cpu"):
+        raw = raw.cpu().numpy()
+    return np.ascontiguousarray(raw, dtype=np.uint8).reshape(-1).view(RELOC_ROW).copy()
+
+
 class FastLioError(RuntimeError):
     pass
 
@@ -112,6 +140,7 @@ SYMBOLS = [
     "fl_scan_reserve", "fl_scan_upload_device", "fl_scan_undistort_device", "fl_scan_voxel_downsample_device",
     "fl_filter_update_scan_device", "fl_map_delete_boxes_async", "fl_localmap_segment_device",
     "fl_filter_reserve_batch", "fl_filter_batch_plan", "fl_filter_update_batch_device",
+    "fl_reloc_expand_grid_device", "fl_filter_reserve_reloc", "fl_filter_relocalize_device",
     "fl_preprocess_create", "fl_preprocess_destroy", "fl_preprocess_device", "fl_preprocess",
     "fl_scan_frame", "fl_scan_frame_device",
 ]
@@ -173,6 +202,10 @@ def load():
     L.fl_filter_reserve_batch.argtypes = [_vp, C.c_int]
     L.fl_filter_batch_plan.argtypes = [_vp, C.c_int, C.c_int, _i32p]
     L.fl_filter_update_batch_device.argtypes = [_vp, _vp, C.c_int, C.c_int, _vp, _vp, C.c_double, _vp, _vp, _vp]
+    L.fl_reloc_expand_grid_device.argtypes = [_vp, C.POINTER(RelocGrid), _vp, _vp]
+    L.fl_filter_reserve_reloc.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
+    L.fl_filter_relocalize_device.argtypes = [_vp, _vp, C.c_int, C.c_int, _vp, _vp, C.c_double, C.POINTER(RelocParams), _vp, _vp,
+                                              _vp, _vp, _vp, _vp]
     L.fl_filter_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int]
     L.fl_filter_destroy.argtypes = [C.c_void_p]
     L.fl_filter_set_params.argtypes = [C.c_void_p, C.c_int, _f64p, C.c_int]
@@ -641,6 +674,41 @@ class Esekf:
                                                      lg.data_ptr() if (logs and H) else None, t._stream()))
         return (status, lg) if logs else status
 
+    # ---- relocalisation: screen many hypotheses by inliers, update from the best, choose one (fl_filter_relocalize_device)
+    def reserve_reloc(self, nq_max: int, n_hyp_max: int, keep_max: int):
+        """fl_filter_reserve_reloc: size the relocalisation's buffers (and the batch's, for nq_max points); synchronous, grow-only."""
+        _check(self._L.fl_filter_reserve_reloc(self.h, int(nq_max), int(n_hyp_max), int(keep_max)))
+
+    def relocalize_device(self, scan, x_hyp, P, keep: int, r_inlier: float, min_effct: int, stride: int = 1, R: float = 0.001,
+                          x_out=None, P_out=None):
+        """fl_filter_relocalize_device on the current stream: scan (nq, 4) float32, x_hyp (H, 26) and P (23, 23) float64.  Returns
+        (x, P, status4, rows, inliers): the winner's updated state and covariance (x_out / P_out when given, left as they were when
+        no survivor qualifies), status4 int32 (4,) = (FL_OK or FL_ERR_STATE, h or -1, effct, inliers), rows a (min(keep, H),
+        sizeof(fl_reloc_row_t)) uint8 tensor (decode_reloc_rows reads it) and inliers int32 (H,).  Nothing synchronises, so the call
+        can be captured into a CUDA graph."""
+        import torch
+        t = self.tree
+        scan = t._tensor(scan, "scan", 4)
+        x_hyp = t._tensor(x_hyp, "x_hyp", 26, torch.float64)
+        P = t._tensor(P, "P", None, torch.float64, (23, 23))
+        H, dev_ = x_hyp.shape[0], x_hyp.device
+        if x_out is None:
+            x_out = torch.zeros(26, dtype=torch.float64, device=dev_)
+        if P_out is None:
+            P_out = torch.zeros((23, 23), dtype=torch.float64, device=dev_)
+        x_out = t._tensor(x_out, "x_out", None, torch.float64, (26,))
+        P_out = t._tensor(P_out, "P_out", None, torch.float64, (23, 23))
+        status4 = torch.empty(4, dtype=torch.int32, device=dev_)
+        inliers = torch.empty(max(H, 1), dtype=torch.int32, device=dev_)[:H]
+        rows = torch.empty((max(min(int(keep), H), 1), C.sizeof(RelocRow)), dtype=torch.uint8, device=dev_)[:max(min(int(keep), H), 0)]
+        prm = RelocParams(int(keep), int(stride), float(r_inlier), int(min_effct))
+        nq = scan.shape[0]
+        _check(self._L.fl_filter_relocalize_device(self.h, scan.data_ptr() if nq else None, nq, H, x_hyp.data_ptr() if H else None,
+                                                   P.data_ptr(), R, C.byref(prm), x_out.data_ptr(), P_out.data_ptr(),
+                                                   inliers.data_ptr() if H else None, rows.data_ptr() if rows.numel() else None,
+                                                   status4.data_ptr(), t._stream()))
+        return x_out, P_out, status4, rows, inliers
+
     def map_incremental_device(self, filter_size_map_min: float = 0.5, flg_EKF_inited: bool = True, out4=None):
         """fl_filter_map_incremental_device on the current stream.  Returns out4, an int32 tensor (4,) = (|PointToAdd|,
         |PointNoNeedDownsample|, Add_Points return, status), written without a host synchronisation (capturable)."""
@@ -1006,6 +1074,21 @@ class Preprocess:
                                             xyzi.data_ptr() if n_max else None, offset_ms.data_ptr() if n_max else None,
                                             out2.data_ptr(), last_ms.data_ptr(), stream))
         return xyzi, offset_ms, out2, last_ms
+
+
+def reloc_grid_device(x_prior, n, step):
+    """fl_reloc_expand_grid_device on the current stream: the (n0 n1 n2 n3, 26) float64 hypotheses of the grid n (4 counts) x step
+    (x, y, z in m, yaw in rad) around x_prior, a (26,) float64 CUDA tensor.  Hypothesis h = ((i_yaw n2 + i_z) n1 + i_y) n0 + i_x."""
+    import torch
+    if not isinstance(x_prior, torch.Tensor) or x_prior.device.type != "cuda" or x_prior.dtype != torch.float64 \
+            or tuple(x_prior.shape) != (26,) or not x_prior.is_contiguous():
+        raise TypeError("x_prior: expected a contiguous (26,) float64 CUDA tensor")
+    g = RelocGrid((C.c_int * 4)(*[int(v) for v in n]), (C.c_double * 4)(*[float(v) for v in step]))
+    H = int(np.prod([max(int(v), 0) for v in n]))
+    out = torch.empty((max(H, 1), 26), dtype=torch.float64, device=x_prior.device)[:H]
+    _check(load().fl_reloc_expand_grid_device(x_prior.data_ptr(), C.byref(g), out.data_ptr(),
+                                              C.c_void_p(torch.cuda.current_stream(x_prior.device).cuda_stream)))
+    return out
 
 
 def host_register(arr: np.ndarray):

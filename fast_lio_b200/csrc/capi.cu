@@ -329,6 +329,21 @@ int fl_filter_update_batch_device(fl_filter_t* f, const float* body_xyzi_device,
     return f->impl->update_batch_on_stream(body_xyzi_device, nq, n_hyp, x26_device, P_device, R, status2_device,
                                            reinterpret_cast<fl::PassLog*>(logs_device), static_cast<cudaStream_t>(stream));
 }
+int fl_reloc_expand_grid_device(const double* x26_prior_device, const fl_reloc_grid_t* grid, double* x26_hyp_device, void* stream) {
+    return fl::reloc_expand_grid(x26_prior_device, grid, x26_hyp_device, static_cast<cudaStream_t>(stream));
+}
+int fl_filter_reserve_reloc(fl_filter_t* f, int nq_max, int n_hyp_max, int keep_max) {
+    FILTER_GUARD(f);
+    return f->impl->reserve_reloc(nq_max, n_hyp_max, keep_max);
+}
+int fl_filter_relocalize_device(fl_filter_t* f, const float* body_xyzi_device, int nq, int n_hyp, const double* x26_hyp_device,
+                                const double* P_device, double R, const fl_reloc_params_t* params, double* x26_out_device,
+                                double* P_out_device, int* inliers_device, fl_reloc_row_t* rows_device, int* status4_device,
+                                void* stream) {
+    FILTER_GUARD(f);
+    return f->impl->relocalize_on_stream(body_xyzi_device, nq, n_hyp, x26_hyp_device, P_device, R, params, x26_out_device, P_out_device,
+                                         inliers_device, rows_device, status4_device, static_cast<cudaStream_t>(stream));
+}
 int fl_filter_get_nearest_device(fl_filter_t* f, float* out_pts_device, int* out_cnt_device, int nq, void* stream) {
     FILTER_GUARD(f);
     return f->impl->get_nearest_on_stream(out_pts_device, out_cnt_device, nq, static_cast<cudaStream_t>(stream));

@@ -1020,6 +1020,7 @@ Filter::~Filter() {
     d_bind_.release();
     b_body_.release(); b_ctl_.release(); b_pub_.release(); b_partials_.release();
     b_nearest_.release(); b_nearest_cnt_.release(); b_selected_.release(); b_plane_.release(); b_srange_.release();
+    r_keys_.release(); r_temp_.release(); r_inl_.release(); r_x_.release(); r_P_.release(); r_status_.release(); r_logs_.release();
     if (h_ctl_) cudaFreeHost(h_ctl_);
     if (ev0_) cudaEventDestroy(ev0_);
     if (ev1_) cudaEventDestroy(ev1_);

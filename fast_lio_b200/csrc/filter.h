@@ -116,6 +116,13 @@ public:
     int batch_plan(int nq, int n_hyp, int* workers, int* slots, int* waves) const;
     int update_batch_on_stream(const float* d_body, int nq, int n_hyp, double* d_x26, double* d_P, double R, int* d_status2,
                                PassLog* d_logs, cudaStream_t st);
+    // Relocalisation (fl_filter_relocalize_device, reloc.cu): screen n_hyp states by inliers (k_reloc_screen), rank them (cub radix
+    // sort), run update_batch_on_stream from the first `keep` and choose one (k_reloc_rank).  Its own buffers (r_*) hold the
+    // counts, the keys and the survivors' x, P, status and logs; reserve_reloc sizes them and calls reserve_batch (grow-only).
+    int reserve_reloc(int nq_max, int n_hyp_max, int keep_max);
+    int relocalize_on_stream(const float* d_body, int nq, int n_hyp, const double* d_x26_hyp, const double* d_P, double R,
+                             const fl_reloc_params_t* prm, double* d_x_out, double* d_P_out, int* d_inliers, fl_reloc_row_t* d_rows,
+                             int* d_status4, cudaStream_t st);
 
     // map_incremental (laserMapping.cpp:427-474) on the device: classify every scan point with the final
     // state and its cached neighbours, then Add_Points(PointToAdd, true) + Add_Points(PointNoNeedDownsample, false)
@@ -199,6 +206,8 @@ private:
     int read_binding();
     int batch_nq_max_ = -1;            // the nq_max reserve_batch sized the batch buffers for (-1: not yet)
     DeviceBuffer b_body_, b_ctl_, b_pub_, b_partials_, b_nearest_, b_nearest_cnt_, b_selected_, b_plane_, b_srange_;
+    int reloc_nq_max_ = -1, reloc_hyp_max_ = 0, reloc_keep_max_ = 0;     // what reserve_reloc sized (-1: not yet)
+    DeviceBuffer r_keys_, r_temp_, r_inl_, r_x_, r_P_, r_status_, r_logs_;
     int launches_ = 0;
     long long host_ns_[4] = {0, 0, 0, 0};
     bool shard_set_ = false;
@@ -211,5 +220,8 @@ private:
     void* peer_ptr_[P2P_MAX_RANKS] = {nullptr};
     bool p2p_on_ = false;
 };
+
+// fl_reloc_expand_grid_device (reloc.cu): the grid's hypotheses around d_prior, on the device that holds it
+int reloc_expand_grid(const double* d_prior, const fl_reloc_grid_t* g, double* d_hyp, cudaStream_t st);
 
 }  // namespace fl

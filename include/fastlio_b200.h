@@ -359,6 +359,63 @@ int fl_filter_batch_plan(fl_filter_t* f, int nq, int n_hyp, int* out3);
 int fl_filter_update_batch_device(fl_filter_t* f, const float* body_xyzi_device, int nq, int n_hyp, double* x26_device,
                                   double* P_device, double R, int* status2_device, fl_pass_log_t* logs_device, void* stream);
 
+/* ---- relocalisation: recover the pose of one scan on the map from many hypotheses
+ * Three stages on the caller's stream, none of which synchronises the host or sizes a launch from a device value, so a whole
+ * relocalisation can be captured into a CUDA graph and replayed.
+ *
+ * fl_reloc_expand_grid_device: hypotheses from a grid around a prior.  x26_prior_device is one state (26 doubles), x26_hyp_device
+ * receives H = n[0] n[1] n[2] n[3] states [H][26], hypothesis h = ((i_yaw n[2] + i_z) n[1] + i_y) n[0] + i_x.  The offset on axis
+ * a is (i_a - (n[a] - 1) / 2.0) step[a]: axes 0-2 add it to pos in the world frame (m), axis 3 turns rot by that yaw (rad) about
+ * u = -grav / |grav| of the prior, rot = q_yaw * rot_prior (the world z axis is not the gravity axis in general).  Every other
+ * component is the prior's.  The kernel runs on the device that holds x26_prior_device.  Each count must be >= 1 and each step
+ * finite and >= 0, else FL_ERR_ARG (so are a null grid, host, null or misaligned (8-byte) pointers, and x26_hyp_device on another
+ * device); H above INT_MAX is FL_ERR_CAPACITY.  Nothing is enqueued on a refusal.  Callers with hypotheses of their own (GNSS,
+ * place recognition) skip this stage. */
+typedef struct fl_reloc_grid {
+    int n[4];            /* x, y, z, yaw */
+    double step[4];      /* m, m, m, rad */
+} fl_reloc_grid_t;
+int fl_reloc_expand_grid_device(const double* x26_prior_device, const fl_reloc_grid_t* grid, double* x26_hyp_device, void* stream);
+
+/* fl_filter_relocalize_device: screen, refine and choose.
+ *   1. Screen (k_reloc_screen): every scan point i with i % stride == 0 is taken to the world by hypothesis h with the update's
+ *      FP64 transform and rounded to float32, exactly as the update's search queries; it is an inlier when the map holds a point
+ *      within r_inlier of it (d2 <= r_inlier * r_inlier in float32: the answer of fl_map_nearest_search with k = 1 and
+ *      max_dist = r_inlier).  inliers[h] counts them; the counts are integers, the same in both modes of the map.
+ *   2. The hypotheses are ranked by the 64-bit key ((screened - inliers[h]) << 32) | h, ascending: most inliers first, ties to
+ *      the lowest h.  The first min(keep, n_hyp) survive.
+ *   3. Refine: fl_filter_update_batch_device runs the scan from each survivor's state, in rank order, all with the one P_device
+ *      and R; a survivor qualifies when its status is FL_OK and the last pass's effct is >= min_effct.  The winner is the
+ *      qualifying survivor with the largest last-pass effct, then the smallest res_sum / effct, then the earliest rank.
+ * x26_out_device and P_out_device receive the winner's updated x and P, the bytes fl_filter_update_device gives from the winner's
+ * state with P_device; when none qualifies they are left as they were.  status4_device = (FL_OK, or FL_ERR_STATE when none
+ * qualifies; the winning h or -1; its last-pass effct or 0; its inliers or 0).  inliers_device [n_hyp] and rows_device
+ * [min(keep, n_hyp)] may be NULL; row s is survivor s: its h, inliers, batch status and passes, and the effct and res_sum of its
+ * last pass (0 when it ran none).
+ * fl_filter_reserve_reloc sizes the buffers of the call for scans of up to nq_max points, n_hyp_max hypotheses and keep_max
+ * survivors (it calls fl_filter_reserve_batch(nq_max)); synchronous and grow-only, a grow moves the buffers (capture again).
+ * Refusals enqueue nothing, also on a capturing stream.  FL_ERR_ARG: nq or n_hyp < 1, keep < 1, stride < 1, r_inlier not > 0,
+ * a null params, or a host, wrong-device, null or misaligned pointer (scan 16 bytes; hypotheses, P, x_out, P_out and rows 8;
+ * inliers and status 4; inliers and rows may be NULL).  FL_ERR_STATE: no fl_filter_reserve_reloc yet, or a sharded, solver-0 or fused-0 filter.  FL_ERR_CAPACITY:
+ * nq, n_hyp or keep above what was reserved.  The conventions, ordering and capture rules of fl_filter_update_batch_device; like
+ * the batch, the call leaves the filter's own results (getters, map_incremental) as they were: to go on mapping from the winner,
+ * run fl_filter_update_device from x26_out_device, then map_incremental. */
+typedef struct fl_reloc_params {
+    int keep;            /* survivors of the screen that run the update */
+    int stride;          /* screen every stride-th scan point */
+    float r_inlier;      /* m */
+    int min_effct;       /* effective points a survivor's last pass needs to qualify */
+} fl_reloc_params_t;
+typedef struct fl_reloc_row {
+    int hyp, inliers, status, passes, effct, pad;
+    double res_sum;
+} fl_reloc_row_t;
+int fl_filter_reserve_reloc(fl_filter_t* f, int nq_max, int n_hyp_max, int keep_max);
+int fl_filter_relocalize_device(fl_filter_t* f, const float* body_xyzi_device, int nq, int n_hyp, const double* x26_hyp_device,
+                                const double* P_device, double R, const fl_reloc_params_t* params, double* x26_out_device,
+                                double* P_out_device, int* inliers_device, fl_reloc_row_t* rows_device, int* status4_device,
+                                void* stream);
+
 /* ------------------------------------------------------------------ scan front end (SURVEY.md §8f rows 3-4)
  * The two steps that produce feats_down_body, kept in HBM on the map's device and stream so that a scan goes
  * raw -> de-skewed -> down-sampled -> update -> map_incremental with one upload. */
