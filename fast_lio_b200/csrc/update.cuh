@@ -896,7 +896,12 @@ __device__ __forceinline__ ulonglong2 row_load(const unsigned long long* p) {
 __device__ __forceinline__ bool row_current(ulonglong2 v, unsigned tag) { return (unsigned)(v.x >> 32) == tag && (unsigned)(v.y >> 32) == tag; }
 __device__ __forceinline__ double row_value(ulonglong2 v) { return __longlong_as_double((long long)((v.y << 32) | (v.x & 0xffffffffull))); }
 
-// measure_fused<EXTR, 2> with the point's state in `pt` (slot threadIdx.x % 256); the same outputs in memory
+}  // namespace fl
+#include "wave_search.cuh"
+namespace fl {
+
+// measure_fused<EXTR, 2> with the point's state in `pt` (slot threadIdx.x % 256) and the search of knn_block_wave; the same
+// outputs in memory
 template <bool EXTR, bool DET>
 __device__ __forceinline__ bool measure_wave(const MapView& m, const ScanView& sc, int q, bool active, const PoseS& s, bool searched,
                                              bool search_only, WalkPool& walks, int& phase, double* stage, WavePoint& pt, double* h,
@@ -913,7 +918,7 @@ __device__ __forceinline__ bool measure_wave(const MapView& m, const ScanView& s
     float pabcd[4] = {0.f, 0.f, 0.f, 0.f};
     if (searched) {
         TBestT<DET> kb;
-        knn_block_pair(m, active, wx, wy, wz, kb, walks, phase, stage);
+        knn_block_wave(m, active, wx, wy, wz, kb, walks, phase, stage);
         if (threadIdx.x >= UPD_THREADS) return false;
         if (active) {
             float4 p[KNN_K];
