@@ -73,6 +73,42 @@ def decode_reloc_rows(raw) -> np.ndarray:
     return np.ascontiguousarray(raw, dtype=np.uint8).reshape(-1).view(RELOC_ROW).copy()
 
 
+class ScanRef(C.Structure):
+    """fl_scan_ref_t: a scan's rows and its row count, both in device memory"""
+    _fields_ = [("body_xyzi", C.c_void_p), ("n", C.c_void_p)]
+
+
+def scan_refs(pairs, device=None):
+    """The device table of fl_filter_update_scans_device: an (S, 2) int64 CUDA tensor of fl_scan_ref_t rows.  Each entry is a
+    `Scan` (Scan.ref(): its device forms' feats_down_body and feats_down_size) or a (rows, n) pair: rows an (m, 4) float32 CUDA
+    tensor and n a one-element int32 CUDA tensor, or either one a raw device address (an int, 0 for null).  The table is copied
+    from the host, so build it outside stream capture; what it points at must outlive the calls that read it."""
+    import torch
+
+    def addr(v, name):
+        if isinstance(v, torch.Tensor):
+            if not v.is_cuda or not v.is_contiguous():
+                raise ValueError(f"scan_refs: {name} must be a contiguous CUDA tensor")
+            return v.data_ptr()
+        return int(v or 0)
+
+    rows = []
+    for p in pairs:
+        if isinstance(p, Scan):
+            b, n, _ = p.ref()
+        else:
+            body, n = p
+            if isinstance(body, torch.Tensor) and (body.dtype != torch.float32 or body.dim() != 2 or body.shape[1] != 4):
+                raise ValueError("scan_refs: rows must be an (m, 4) float32 tensor")
+            if isinstance(n, torch.Tensor) and n.dtype != torch.int32:
+                raise ValueError("scan_refs: n must be an int32 tensor")
+            b, n = addr(body, "rows"), addr(n, "n")
+        rows.append((b, n))
+    if device is None:
+        device = torch.device("cuda", torch.cuda.current_device())
+    return torch.tensor(rows, dtype=torch.int64).reshape(-1, 2).to(device)
+
+
 class FastLioError(RuntimeError):
     pass
 
@@ -143,6 +179,7 @@ SYMBOLS = [
     "fl_reloc_expand_grid_device", "fl_filter_reserve_reloc", "fl_filter_relocalize_device",
     "fl_preprocess_create", "fl_preprocess_destroy", "fl_preprocess_device", "fl_preprocess",
     "fl_scan_frame", "fl_scan_frame_device",
+    "fl_scan_get_ref", "fl_filter_update_scans_device",
 ]
 
 
@@ -202,6 +239,8 @@ def load():
     L.fl_filter_reserve_batch.argtypes = [_vp, C.c_int]
     L.fl_filter_batch_plan.argtypes = [_vp, C.c_int, C.c_int, _i32p]
     L.fl_filter_update_batch_device.argtypes = [_vp, _vp, C.c_int, C.c_int, _vp, _vp, C.c_double, _vp, _vp, _vp]
+    L.fl_filter_update_scans_device.argtypes = [_vp, _vp, C.c_int, C.c_int, _vp, _vp, C.c_double, _vp, _vp, _vp]
+    L.fl_scan_get_ref.argtypes = [_vp, C.POINTER(ScanRef), C.POINTER(C.c_int)]
     L.fl_reloc_expand_grid_device.argtypes = [_vp, C.POINTER(RelocGrid), _vp, _vp]
     L.fl_filter_reserve_reloc.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
     L.fl_filter_relocalize_device.argtypes = [_vp, _vp, C.c_int, C.c_int, _vp, _vp, C.c_double, C.POINTER(RelocParams), _vp, _vp,
@@ -674,6 +713,30 @@ class Esekf:
                                                      lg.data_ptr() if (logs and H) else None, t._stream()))
         return (status, lg) if logs else status
 
+    # ---- batched form over many scans: a scan and a prior per slot, one shared map (fl_filter_update_scans_device)
+    def update_scans_device(self, refs, x, P, nq_max: int, R: float = 0.001, status=None, logs: bool = False):
+        """fl_filter_update_scans_device on the current stream: refs the (S, 2) int64 table of scan_refs, x (S, 26) and P (S, 23,
+        23) float64, updated in place per slot (only where it succeeds).  Slot s runs rows [0, *n) of its scan, read on the device;
+        counts above nq_max are refused.  Returns status, an (S, 2) int32 tensor of (FL_OK, FL_ERR_STATE, or FL_ERR_ARG /
+        FL_ERR_CAPACITY for a refused slot, passes run); with logs=True also the pass logs as an (S, max_iter + 1,
+        sizeof(fl_pass_log_t)) uint8 tensor (decode_pass_logs reads them).  Nothing synchronises, so the call can be captured into
+        a CUDA graph."""
+        import torch
+        t = self.tree
+        x = t._tensor(x, "x", 26, torch.float64)
+        S = x.shape[0]
+        refs = t._tensor(refs, "refs", None, torch.int64, (S, 2))
+        P = t._tensor(P, "P", None, torch.float64, (S, 23, 23))
+        if status is None:
+            status = torch.empty((S, 2), dtype=torch.int32, device=x.device)
+        status = t._tensor(status, "status", None, torch.int32, (S, 2))
+        lg = torch.zeros((S, self.max_iter + 1, C.sizeof(PassLog)), dtype=torch.uint8, device=x.device) if logs else None
+        _check(self._L.fl_filter_update_scans_device(self.h, refs.data_ptr() if S else None, S, int(nq_max),
+                                                     x.data_ptr() if S else None, P.data_ptr() if S else None, R,
+                                                     status.data_ptr() if S else None, lg.data_ptr() if (logs and S) else None,
+                                                     t._stream()))
+        return (status, lg) if logs else status
+
     # ---- relocalisation: screen many hypotheses by inliers, update from the best, choose one (fl_filter_relocalize_device)
     def reserve_reloc(self, nq_max: int, n_hyp_max: int, keep_max: int):
         """fl_filter_reserve_reloc: size the relocalisation's buffers (and the batch's, for nq_max points); synchronous, grow-only."""
@@ -898,6 +961,14 @@ class Scan:
         out = t._tensor(out, "out", None, torch.int32, (1,))
         _check(self._L.fl_scan_voxel_downsample_device(self.h, leaf, out.data_ptr(), t._stream()))
         return out
+
+    def ref(self):
+        """fl_scan_get_ref: (body_ptr, n_ptr, n_max), the device forms' feats_down_body, the device address of feats_down_size and
+        the rows fl_scan_reserve sized; valid until a reserve that grows the scan."""
+        r = ScanRef()
+        m = C.c_int(0)
+        _check(self._L.fl_scan_get_ref(self.h, C.byref(r), C.byref(m)))
+        return int(r.body_xyzi or 0), int(r.n or 0), int(m.value)
 
     def update_device(self, filt: "Esekf", x, P, R: float = 0.001, status=None):
         """fl_filter_update_scan_device: x (26,) and P (23, 23) float64 tensors updated in place on success; returns status, an

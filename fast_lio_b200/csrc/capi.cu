@@ -534,6 +534,23 @@ int fl_filter_update_scan_device(fl_filter_t* f, fl_scan_t* s, double* x26_devic
     return f->impl->update_scan_on_stream(s->impl->down_dev(), s->impl->down_count_dev(), s->impl->dev_n_max(), x26_device, P_device, R,
                                           status2_device, static_cast<cudaStream_t>(stream));
 }
+static_assert(sizeof(fl_scan_ref_t) == 16, "fl_scan_ref_t is two device pointers");
+int fl_scan_get_ref(fl_scan_t* s, fl_scan_ref_t* out, int* n_max) {
+    SCAN_GUARD(s);
+    if (!out) { fl::set_last_error("fl_scan_get_ref: null out"); return FL_ERR_ARG; }
+    const int m = s->impl->reserved_n_max();
+    if (m < 0) { fl::set_last_error("fl_scan_get_ref: call fl_scan_reserve first"); return FL_ERR_STATE; }
+    out->body_xyzi = reinterpret_cast<const float*>(s->impl->down_dev());
+    out->n = s->impl->down_count_dev();
+    if (n_max) *n_max = m;
+    return FL_OK;
+}
+int fl_filter_update_scans_device(fl_filter_t* f, const fl_scan_ref_t* scans_device, int n_scans, int nq_max, double* x26_device,
+                                  double* P_device, double R, int* status2_device, fl_pass_log_t* logs_device, void* stream) {
+    FILTER_GUARD(f);
+    return f->impl->update_scans_on_stream(scans_device, n_scans, nq_max, x26_device, P_device, R, status2_device,
+                                           reinterpret_cast<fl::PassLog*>(logs_device), static_cast<cudaStream_t>(stream));
+}
 // publish_frame_world / publish_frame_body / pointBodyToWorld                     laserMapping.cpp:177-220, :478-549, :909-921
 int fl_scan_frame(fl_scan_t* s, int which, int frame, const double* x26, float* out_xyzi, int cap) {
     SCAN_HOST_GUARD(s);

@@ -960,6 +960,41 @@ __global__ void __launch_bounds__(STATE_THREADS) k_batch_state_out(const FilterC
     state_out(ctl + b, x26 + (size_t)b * XLEN, P + (size_t)b * NDOF * NDOF, status2 + 2 * b);
 }
 
+// fl_filter_update_scans_device: block b validates table entry b of a wave (the wave's first) and its count, writes slot b of the
+// ScanSlot table k_update_scans reads, and sets the slot up from prior b as k_batch_state_in does.  A refused slot's prior is
+// not read and its control block is not set up.
+__global__ void __launch_bounds__(STATE_THREADS) k_scans_state_in(FilterCtl* ctl, unsigned long long* pub, const fl_scan_ref_t* refs,
+                                                                  int nq_max, const double* __restrict__ x26,
+                                                                  const double* __restrict__ P, StateIn s, ScanSlot* slots) {
+    pdl_launch();           // as k_state_in: k_update_scans reads the table after its pdl_wait()
+    const int b = (int)blockIdx.x;
+    const fl_scan_ref_t r = refs[b];
+    const float4* body = reinterpret_cast<const float4*>(r.body_xyzi);
+    int c = 0, status = FL_ERR_ARG;
+    if (r.n && ((uintptr_t)r.n & 3) == 0) {
+        c = *r.n;
+        if (c < 0 || (c > 0 && (!body || ((uintptr_t)body & 15)))) status = FL_ERR_ARG;
+        else status = c > nq_max ? FL_ERR_CAPACITY : FL_OK;
+    }
+    if (threadIdx.x == 0) {
+        ScanSlot sl;
+        sl.body = body; sl.n = status == FL_OK ? c : 0; sl.status = status;
+        slots[b] = sl;
+    }
+    if (status == FL_OK) state_in(ctl + b, pub + (size_t)b * BATCH_PUB_WORDS, x26 + (size_t)b * XLEN, P + (size_t)b * NDOF * NDOF, s);
+}
+// block b: slot b into prior b of x26 / P / status2 (the wave's first); a refused slot writes (its status, 0) and nothing else
+__global__ void __launch_bounds__(STATE_THREADS) k_scans_state_out(const FilterCtl* __restrict__ ctl, const ScanSlot* __restrict__ slots,
+                                                                   double* __restrict__ x26, double* __restrict__ P, int* __restrict__ status2) {
+    const int b = (int)blockIdx.x;
+    const int status = slots[b].status;
+    if (status != FL_OK) {
+        if (threadIdx.x == 0) { status2[2 * b] = status; status2[2 * b + 1] = 0; }
+        return;
+    }
+    state_out(ctl + b, x26 + (size_t)b * XLEN, P + (size_t)b * NDOF * NDOF, status2 + 2 * b);
+}
+
 // map_incremental over n_max rows with the count in device memory: rows [*n, n_max) are neither PointToAdd nor PointNoNeedDownsample
 __global__ void k_flags_clear(unsigned char* __restrict__ flag_add, unsigned char* __restrict__ flag_no, const int* __restrict__ n, int n_max) {
     const int q = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1019,7 +1054,7 @@ Filter::~Filter() {
     mi_world_.release(); mi_flag_add_.release(); mi_flag_no_.release(); mi_list_add_.release(); mi_list_no_.release(); mi_tmp_.release(); mi_counts_.release();
     d_bind_.release();
     b_body_.release(); b_ctl_.release(); b_pub_.release(); b_partials_.release();
-    b_nearest_.release(); b_nearest_cnt_.release(); b_selected_.release(); b_plane_.release(); b_srange_.release();
+    b_nearest_.release(); b_nearest_cnt_.release(); b_selected_.release(); b_plane_.release(); b_srange_.release(); b_slots_.release();
     r_keys_.release(); r_temp_.release(); r_inl_.release(); r_x_.release(); r_P_.release(); r_status_.release(); r_logs_.release();
     if (h_ctl_) cudaFreeHost(h_ctl_);
     if (ev0_) cudaEventDestroy(ev0_);
@@ -1080,6 +1115,18 @@ int Filter::init() {
             const int host = k == UK_N1 ? UK_UPDATE1 : k == UK_N2 ? UK_UPDATE2 : k == UK_N_WAVE ? UK_WAVE : -1;
             if (host >= 0) cap = std::min(cap, upd_caps_.blocks[host][e]);
         }
+    // k_update_scans runs UK_BATCH's plan; it has k_update_batch's registers and shared memory (tests/test_update_scans_build.py),
+    // and should the two co-resident counts ever differ, it plans with the smaller
+    scans_caps_ = upd_caps_;
+    {
+        const void* const scans_fn[2][2] = {{(const void*)k_update_scans<false>, (const void*)k_update_scans<true>},
+                                            {(const void*)k_update_scans_det<false>, (const void*)k_update_scans_det<true>}};
+        for (int e = 0; e < 2; e++)
+            for (int d = 0; d < 2; d++) {
+                FL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, scans_fn[d][e], UPD_THREADS, 0));
+                scans_caps_.blocks[UK_BATCH][e] = std::min(scans_caps_.blocks[UK_BATCH][e], sms_ * occ);
+            }
+    }
     {
         const int* wave = upd_caps_.blocks[UK_WAVE];
         const size_t bytes = sizeof(unsigned long long) * 2 * PSTRIDE * (size_t)std::max(1, std::max(wave[0], wave[1]));
@@ -1301,8 +1348,14 @@ UpdPlan Filter::plan(UpdRoute r, int rows, int n_hyp) const {
 }
 
 template <bool E>
-static cudaError_t launch_upd_kernel(const UpdPlan& p, bool pdl, cudaStream_t st, const UpdArgs& a, const int* n, unsigned long long* rows, int log_stride) {
+static cudaError_t launch_upd_kernel(const UpdPlan& p, bool pdl, cudaStream_t st, const UpdArgs& a, const int* n, unsigned long long* rows, int log_stride,
+                                     const ScanSlot* slots) {
     const dim3 grid((unsigned)p.grid_x, (unsigned)p.slots);
+    if (p.scans) {                           // UK_BATCH with a scan per slot
+        if (p.kernel != UK_BATCH) return cudaErrorInvalidValue;
+        return p.det ? launch_pdl(k_update_scans_det<E>, grid, p.block, st, pdl, a, log_stride, slots)
+                     : launch_pdl(k_update_scans<E>, grid, p.block, st, pdl, a, log_stride, slots);
+    }
     if (p.det) switch (p.kernel) {           // the keyed tie rule (fl_map_set_deterministic)
     case UK_UPDATE1: return launch_pdl(k_update_det<E, 1>, grid, p.block, st, pdl, a);
     case UK_UPDATE2: return launch_pdl(k_update_det<E, 2>, grid, p.block, st, pdl, a);
@@ -1324,8 +1377,9 @@ static cudaError_t launch_upd_kernel(const UpdPlan& p, bool pdl, cudaStream_t st
     default: return cudaErrorInvalidValue;
     }
 }
-cudaError_t Filter::launch_plan(const UpdPlan& p, const UpdArgs& a, cudaStream_t st, const int* n, int log_stride) {
-    return (extrinsic_est_ ? launch_upd_kernel<true> : launch_upd_kernel<false>)(p, pdl_ && p.pdl, st, a, n, rows_.as<unsigned long long>(), log_stride);
+cudaError_t Filter::launch_plan(const UpdPlan& p, const UpdArgs& a, cudaStream_t st, const int* n, int log_stride, const ScanSlot* slots) {
+    return (extrinsic_est_ ? launch_upd_kernel<true> : launch_upd_kernel<false>)(p, pdl_ && p.pdl, st, a, n, rows_.as<unsigned long long>(), log_stride,
+                                                                                 slots);
 }
 
 int Filter::launch_search_only() {
@@ -1570,6 +1624,7 @@ int Filter::reserve_batch(int nq_max) {
     FL_CHECK(b_selected_.reserve(rows));
     FL_CHECK(b_plane_.reserve(sizeof(float4) * rows));
     FL_CHECK(b_srange_.reserve(sizeof(double) * rows));
+    FL_CHECK(b_slots_.reserve(sizeof(ScanSlot) * (size_t)cap));
     FL_CUDA(cudaMemsetAsync(b_ctl_.ptr, 0, b_ctl_.bytes, stream()));
     FL_CUDA(cudaMemsetAsync(b_pub_.ptr, 0, b_pub_.bytes, stream()));
     FL_CUDA(cudaStreamSynchronize(stream()));
@@ -1623,6 +1678,63 @@ int Filter::update_batch_on_stream(const float* d_body, int nq, int n_hyp, doubl
         p.slots = n;                                  // grid.y: the hypotheses of this wave (the last may be partial)
         FL_CUDA(launch_plan(p, a, st, nullptr, log_stride));
         k_batch_state_out<<<n, STATE_THREADS, 0, st>>>(ctl, x, P, d_status2 + 2 * (size_t)h0);
+        FL_CUDA(cudaGetLastError());
+    }
+    return map_->query_end(st, joined);
+}
+
+// Slot s at count c gets the workers of the single form at nq_max rows; with the blocks beyond its tiles writing +0.0 rows, that is
+// the single form at c (update.cuh, k_update_scans).  Waves as update_batch_on_stream, planned at nq_max.
+int Filter::update_scans_on_stream(const fl_scan_ref_t* d_refs, int n_scans, int nq_max, double* d_x26, double* d_P, double R,
+                                   int* d_status2, PassLog* d_logs, cudaStream_t st) {
+    const int dev = map_->device();
+    if (n_scans < 0 || nq_max < 0 ||
+        (n_scans > 0 && (!device_ptr(d_refs, dev, 8) || !device_ptr(d_x26, dev, 8) || !device_ptr(d_P, dev, 8) ||
+                         !device_ptr(d_status2, dev, 4) || (d_logs && !device_ptr(d_logs, dev, 8))))) {
+        set_last_error("update_scans_device: n_scans or nq_max < 0, or a buffer is not device memory on device %d (table, x, P and "
+                       "logs 8-byte, status 4-byte aligned)", dev);
+        return FL_ERR_ARG;
+    }
+    FL_CHECK(device_form_scope("update_scans_device", true));
+    if (batch_nq_max_ < 0) { set_last_error("update_scans_device: call fl_filter_reserve_batch first"); return FL_ERR_STATE; }
+    if (nq_max > batch_nq_max_) {
+        set_last_error("update_scans_device: nq_max = %d exceeds the %d fl_filter_reserve_batch sized", nq_max, batch_nq_max_);
+        return FL_ERR_CAPACITY;
+    }
+    UpdPlan p = plan_update(scans_caps_, UR_BATCH, nq_max, extrinsic_est_, false, n_scans, map_->deterministic());
+    p.scans = true;
+    if (!p.slots) {
+        set_last_error("update_scans_device: a slot takes %d blocks, %d k_update_scans blocks are co-resident", p.grid_x,
+                       scans_caps_.blocks[UK_BATCH][extrinsic_est_ ? 1 : 0]);
+        return FL_ERR_CAPACITY;
+    }
+    if (n_scans == 0) return FL_OK;
+    FL_CUDA(cudaSetDevice(dev));
+    bool joined = false;
+    FL_CHECK(map_->query_begin(st, &joined));
+    ScanView sc;
+    memset(&sc, 0, sizeof(sc));                       // body and q_end are the slot's (k_update_scans)
+    sc.nearest = b_nearest_.as<float4>(); sc.nearest_cnt = b_nearest_cnt_.as<int>(); sc.selected = b_selected_.as<unsigned char>();
+    sc.plane = b_plane_.as<float4>(); sc.srange = b_srange_.as<double>();
+    sc.q_begin = 0; sc.q_end = sc.Q = nq_max;
+    const StateIn s = state_in_args(R);
+    const int log_stride = max_iter_ + 1;
+    FilterCtl* ctl = b_ctl_.as<FilterCtl>();
+    unsigned long long* pub = b_pub_.as<unsigned long long>();
+    ScanSlot* slots = b_slots_.as<ScanSlot>();
+    for (int w = 0; w < p.waves; w++) {
+        const int h0 = w * p.slots, n = std::min(p.slots, n_scans - h0);
+        double* x = d_x26 + (size_t)h0 * XLEN;
+        double* P = d_P + (size_t)h0 * NDOF * NDOF;
+        k_scans_state_in<<<n, STATE_THREADS, 0, st>>>(ctl, pub, d_refs + h0, nq_max, x, P, s, slots);
+        FL_CUDA(cudaGetLastError());
+        UpdArgs a = upd_args(max_iter_ + 1, 0, 0);    // the map view, the search A/B switch and a fresh nonce, as the single form
+        a.sc = sc; a.ctl = ctl; a.partials = b_partials_.as<double>(); a.pub = pub;
+        a.logs = d_logs ? d_logs + (size_t)h0 * log_stride : nullptr;
+        UpdPlan pw = p;
+        pw.slots = n;                                 // grid.y: the slots of this wave (the last may be partial)
+        FL_CUDA(launch_plan(pw, a, st, nullptr, log_stride, slots));
+        k_scans_state_out<<<n, STATE_THREADS, 0, st>>>(ctl, slots, x, P, d_status2 + 2 * (size_t)h0);
         FL_CUDA(cudaGetLastError());
     }
     return map_->query_end(st, joined);

@@ -57,6 +57,7 @@ struct ScanView {
 struct NcclApi;
 struct UpdArgs;
 struct StateIn;
+struct ScanSlot;
 
 // Peer-memory exchange of the per-pass sums (fused into k_residual's solver block): every rank owns a
 // mailbox [2 epoch parities][nranks][96] values, each two epoch-tagged 8-byte words; peers store into it over NVLink.
@@ -116,6 +117,10 @@ public:
     int batch_plan(int nq, int n_hyp, int* workers, int* slots, int* waves) const;
     int update_batch_on_stream(const float* d_body, int nq, int n_hyp, double* d_x26, double* d_P, double R, int* d_status2,
                                PassLog* d_logs, cudaStream_t st);
+    // The batch with a scan per slot (fl_filter_update_scans_device): slot s runs the table entry d_refs[s] in place, on the batch's
+    // buffers, in waves planned at nq_max (UR_BATCH on scans_caps_); k_scans_state_in validates each entry and count on the device.
+    int update_scans_on_stream(const fl_scan_ref_t* d_refs, int n_scans, int nq_max, double* d_x26, double* d_P, double R,
+                               int* d_status2, PassLog* d_logs, cudaStream_t st);
     // Relocalisation (fl_filter_relocalize_device, reloc.cu): screen n_hyp states by inliers (k_reloc_screen), rank them (cub radix
     // sort), run update_batch_on_stream from the first `keep` and choose one (k_reloc_rank).  Its own buffers (r_*) hold the
     // counts, the keys and the survivors' x, P, status and logs; reserve_reloc sizes them and calls reserve_batch (grow-only).
@@ -181,11 +186,14 @@ private:
     DeviceBuffer pub_;                 // k_update's publication block
     unsigned launch_nonce_ = 0;
     UpdCaps upd_caps_ = {};                      // co-resident blocks of every update kernel on this device (init)
+    UpdCaps scans_caps_ = {};                    // upd_caps_ with UK_BATCH's count lowered to k_update_scans' if that is smaller
     int launch_update(int max_passes, int mode, int search_only) { return launch_update(max_passes, mode, search_only, stream()); }
     int launch_update(int max_passes, int mode, int search_only, cudaStream_t st);
     UpdPlan plan(UpdRoute r, int rows, int n_hyp = 0) const;       // plan_update here, FASTLIO_B200_PAIR read at every plan
-    // the only launch of an update kernel: n is the count of the _n forms, log_stride k_update_batch's, grid.y = p.slots
-    cudaError_t launch_plan(const UpdPlan& p, const UpdArgs& a, cudaStream_t st, const int* n = nullptr, int log_stride = 0);
+    // the only launch of an update kernel: n is the count of the _n forms, log_stride k_update_batch's, grid.y = p.slots,
+    // slots k_update_scans' table (p.scans)
+    cudaError_t launch_plan(const UpdPlan& p, const UpdArgs& a, cudaStream_t st, const int* n = nullptr, int log_stride = 0,
+                            const ScanSlot* slots = nullptr);
     StateIn state_in_args(double R) const;       // k_state_in / k_batch_state_in's setup besides the caller's x26 / P
     // the device forms cover a single-rank filter (and the update a fused, solver-1 one); FL_ERR_STATE otherwise
     int device_form_scope(const char* what, bool update) const;
@@ -206,6 +214,7 @@ private:
     int read_binding();
     int batch_nq_max_ = -1;            // the nq_max reserve_batch sized the batch buffers for (-1: not yet)
     DeviceBuffer b_body_, b_ctl_, b_pub_, b_partials_, b_nearest_, b_nearest_cnt_, b_selected_, b_plane_, b_srange_;
+    DeviceBuffer b_slots_;             // update_scans_on_stream: one wave's ScanSlot table (k_scans_state_in)
     int reloc_nq_max_ = -1, reloc_hyp_max_ = 0, reloc_keep_max_ = 0;     // what reserve_reloc sized (-1: not yet)
     DeviceBuffer r_keys_, r_temp_, r_inl_, r_x_, r_P_, r_status_, r_logs_;
     int launches_ = 0;

@@ -47,6 +47,7 @@ public:
     const int* down_count_dev() const;
     int dev_n_max() const { return dev_n_max_; }
     bool dev_down_ready() const { return dev_down_; }      // a device-form down-sample ran since the last upload
+    int reserved_n_max() const { return dev_used_ ? res_n_max_ : -1; }      // the rows reserve_device sized (-1: not yet)
 
 private:
     static constexpr size_t UNDISTORT_SMEM_MAX = 200 * 1024;     // IMU poses in k_undistort's shared memory

@@ -26,6 +26,7 @@ struct UpdPlan {
     int block, smem;           // threads per block, dynamic shared memory bytes
     bool pdl;                  // may overlap its predecessor (programmatic dependent launch, when the filter has it on)
     bool det;                  // the keyed-tie-rule instantiation of `kernel` (the map's deterministic mode)
+    bool scans;                // UK_BATCH with a scan per slot (k_update_scans): never set here, the filter sets it
 };
 
 // Every co-resident block works (a searching pass wants many warps in flight), one thread per point in full warps.  Two threads

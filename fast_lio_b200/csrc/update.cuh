@@ -1187,4 +1187,33 @@ __global__ void __launch_bounds__(2 * UPD_THREADS, 1) k_update_n_wave_det(UpdArg
     update_wave_body<EXTR, true>(a, rows, min(*n, a.sc.q_end));
 }
 
+// ============================================================================= a scan per slot (fl_filter_update_scans_device)
+// k_update_batch's slots, each on a scan of its own.  The grid is sized at nq_max (sc.Q, the row stride of the slot's caches)
+// and slot s runs rows [0, c) of its body, c its validated count: q1 = c as k_update_n's count, so tile t goes to block t + 1
+// exactly as in the single form at c rows, and the blocks beyond write +0.0 partial rows, which leave the fixed-order sums
+// unchanged.  When the tiles of nq_max exceed the co-resident workers both forms have the same cap - 1 workers.
+// k_scans_state_in writes the slot table (body, count, status) as the kernel ahead of this one, so it is read after pdl_wait()
+// (update_body's own pdl_wait() then returns at once).  A refused slot's blocks return without touching anything.
+struct ScanSlot {
+    const float4* body;
+    int n, status;          // status FL_OK: run rows [0, n); otherwise refused
+};
+template <bool EXTR, bool DET>
+__device__ __forceinline__ void update_scans_body(UpdArgs& a, int log_stride, const ScanSlot* slots) {
+    pdl_wait();
+    const ScanSlot sl = slots[blockIdx.y];
+    if (sl.status != FL_OK) return;
+    a.sc.body = sl.body;
+    a.sc.q_end = sl.n;      // <= nq_max = sc.Q (k_scans_state_in refuses more)
+    update_batch_body<EXTR, DET>(a, log_stride);
+}
+template <bool EXTR>
+__global__ void __launch_bounds__(UPD_THREADS, 2) k_update_scans(UpdArgs a, int log_stride, const ScanSlot* slots) {
+    update_scans_body<EXTR, false>(a, log_stride, slots);
+}
+template <bool EXTR>
+__global__ void __launch_bounds__(UPD_THREADS, 2) k_update_scans_det(UpdArgs a, int log_stride, const ScanSlot* slots) {
+    update_scans_body<EXTR, true>(a, log_stride, slots);
+}
+
 }  // namespace fl

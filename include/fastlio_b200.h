@@ -490,6 +490,41 @@ int fl_scan_voxel_downsample_device(fl_scan_t* s, float leaf_size, int* n_out_de
 int fl_filter_update_scan_device(fl_filter_t* f, fl_scan_t* s, double* x26_device, double* P_device, double R, int* status2_device,
                                  void* stream);
 
+/* ---- batched form of the update over many scans: each slot its own scan and prior, one shared map (a fleet localising on a
+ * prior map, offline re-registration of a recorded sequence)
+ * esekf::update_iterated_dyn_share_modified run for n_scans (scan, prior) pairs    esekfom.hpp:1619-1931, laserMapping.cpp:638-754
+ * scans_device is a device table of n_scans fl_scan_ref_t.  For slot s the count c = *scans_device[s].n is read when `stream`
+ * reaches the call.  Per slot: if 0 <= c <= nq_max and the body is non-null and 16-byte aligned (null is allowed when c = 0),
+ * x26_device[s], P_device[s], status2_device[s] and logs_device[s][0, passes) receive exactly the bytes fl_filter_update_device
+ * gives for rows [0, c) of that body from the prior (x26_device[s], P_device[s]) on the same map, R and parameters; log entries
+ * from `passes` on are not written.  A refused slot: c < 0, a null or misaligned body with c > 0, or a null or misaligned
+ * (4-byte) count pointer gives status2_device[s] = (FL_ERR_ARG, 0); c > nq_max gives (FL_ERR_CAPACITY, 0).  Its x, P and logs
+ * are not touched, and no other slot's result depends on it.  x26_device is [n_scans][26], P_device [n_scans][23 * 23],
+ * status2_device [n_scans][2], logs_device (may be NULL) [n_scans][max_iter + 1].
+ * The slots run in waves planned at nq_max: fl_filter_batch_plan(f, nq_max, n_scans, out3) gives (workers per slot, slots per
+ * wave, waves), and a wave lasts as long as its slowest slot.  The call uses the buffers of fl_filter_reserve_batch(f, >= nq_max)
+ * and, like fl_filter_update_batch_device, leaves the filter's own results as they were: the getters, map_incremental (both
+ * forms) and the next single update.  Calls that use the batch's buffers of one filter must be ordered on one stream.
+ * The scans are read in place, not copied: their rows and counts must stay as they are until `stream` has passed the call.
+ * Several slots may reference the same or overlapping rows.
+ * The conventions, ordering and capture rules of fl_filter_update_batch_device; the map's deterministic mode is followed.
+ * n_scans = 0 returns FL_OK and enqueues nothing.  Refusals enqueue nothing, also on a capturing stream.  FL_ERR_ARG: n_scans or
+ * nq_max < 0; a host, wrong-device, null or misaligned pointer (table 8 bytes, x and P 8, status 4, logs 8).  FL_ERR_STATE: no
+ * fl_filter_reserve_batch yet, or a sharded, solver-0 or fused-0 filter.  FL_ERR_CAPACITY: nq_max above the reserved nq_max,
+ * or one slot does not fit the co-resident grid.
+ * fl_scan_get_ref writes the device forms' feats_down_body and feats_down_size of a scan front end as a table entry, and *n_max
+ * (may be NULL) the rows fl_scan_reserve sized.  The entry is valid until an fl_scan_reserve that grows the scan (capture
+ * again after it).  FL_ERR_STATE before fl_scan_reserve; a null out is FL_ERR_ARG.  Per robot, fl_scan_upload_device ->
+ * undistort_device -> voxel_downsample_device, then one fl_filter_update_scans_device over every robot's entry, can be captured
+ * into one graph. */
+typedef struct fl_scan_ref {
+    const float* body_xyzi;   /* device: the scan's rows (x, y, z, intensity), 16-byte aligned */
+    const int* n;             /* device: its row count, read when the stream reaches the call */
+} fl_scan_ref_t;              /* 16 bytes */
+int fl_scan_get_ref(fl_scan_t* s, fl_scan_ref_t* out, int* n_max);
+int fl_filter_update_scans_device(fl_filter_t* f, const fl_scan_ref_t* scans_device, int n_scans, int nq_max, double* x26_device,
+                                  double* P_device, double R, int* status2_device, fl_pass_log_t* logs_device, void* stream);
+
 /* ---- the scan's clouds in a frame: the clouds a FAST-LIO user consumes after map_incremental (laserMapping.cpp:980-982)
  * which (as in fl_scan_download): 0 feats_undistort (de-skewed, or as uploaded), 1 feats_down_body.  Per row, float (x, y, z,
  * intensity), the intensity passed through; the coordinates in FP64 with Eigen's _transformVector order, then rounded to float:
