@@ -874,7 +874,7 @@ __global__ void __launch_bounds__(UPD_THREADS, 2) k_update_batch(UpdArgs a, int 
 // Stamps in ctl->prof besides k_update's clock64 ones, in %globaltimer ns so they compare across SMs, for the pass that ends
 // the update: [11] the solver has summed every partial row, [2] its publication is visible on the solver's SM (an otherwise
 // idle thread of block 0 polls for it), [3] the last worker block has picked it up.  Each is read by a thread nothing waits
-// for: a %globaltimer read costs several hundred cycles on H100.
+// for: a %globaltimer read costs several hundred cycles on H100.  The solver pass is sol_pass_wave (wave_solver.cuh).
 struct WavePoint {                 // dynamic shared memory of a worker block: its tile's points
     float4 body[UPD_THREADS];
     float4 plane[UPD_THREADS];
@@ -898,6 +898,7 @@ __device__ __forceinline__ double row_value(ulonglong2 v) { return __longlong_as
 
 }  // namespace fl
 #include "wave_search.cuh"
+#include "wave_solver.cuh"
 namespace fl {
 
 // measure_fused<EXTR, 2> with the point's state in `pt` (slot threadIdx.x % 256) and the search of knn_block_wave; the same
@@ -958,7 +959,8 @@ __device__ __forceinline__ bool measure_wave(const MapView& m, const ScanView& s
 
 // sol_reduce over tagged rows: warp w takes the rows w, w + 8, ... of pass `tag` GATHER_ROWS at a time, spins until each of them
 // is current (every poll reloads all the stale words of the batch at once: one round trip) and sums them in ascending order from
-// +0.0 (sol_reduce's order; the +0.0 rows it adds past nwork change no sum)
+// +0.0 (sol_reduce's order; the +0.0 rows it adds past nwork change no sum).  Ends with the warps' sums in S.wred after one
+// barrier: sol_pass_wave adds them up.
 constexpr int GATHER_ROWS = 8;
 __device__ void sol_gather(SolverSm& S, FilterCtl* ctl, const unsigned long long* __restrict__ rows, int nwork, unsigned tag) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -1004,19 +1006,18 @@ __device__ void sol_gather(SolverSm& S, FilterCtl* ctl, const unsigned long long
     if (late) S.late = 2;
     sol_sync();
     if (tid == 0) ctl->prof[9] = clock64();
-    if (tid < PSTRIDE) {
+    // warp 0 adds the warps' sums itself and stores S.red (sol_pass_wave); warps 1..3 expand H^T H for the log from the same
+    // sums in the same order
+    if (tid >= 32 && tid < 32 + 78) {
+        const int o = tid - 32;
         double v = 0.0;
 #pragma unroll
-        for (int w = 0; w < UPD_WARPS; w++) v += S.wred[w][tid];
-        S.red[tid] = v;
-        if (tid < 78) {
-            int a = 0, rem = tid;
-            while (rem >= 12 - a) { rem -= 12 - a; a++; }
-            const int b = a + rem;
-            S.HTH[a * 12 + b] = v; S.HTH[b * 12 + a] = v;
-        }
+        for (int w = 0; w < UPD_WARPS; w++) v += S.wred[w][o];
+        int a = 0, rem = o;
+        while (rem >= 12 - a) { rem -= 12 - a; a++; }
+        const int b = a + rem;
+        S.HTH[a * 12 + b] = v; S.HTH[b * 12 + a] = v;
     }
-    sol_sync();
     if (tid == 128) ctl->prof[11] = (long long)globaltimer();         // a warp the gain does not wait for
 }
 
@@ -1141,7 +1142,7 @@ __device__ __forceinline__ void update_wave_body(const UpdArgs& a, unsigned long
         if (tid == 0) ctl->prof[8] = clock64();
         sol_gather(S, ctl, rows, nwork, row_tag(epoch, p));
         if (tid == 0) ctl->prof[1] = clock64();
-        sol_pass<EXTR>(S, ctl, a.logs, a.pub, pub_tag(a.nonce, p + 1));
+        sol_pass_wave<EXTR>(S, ctl, a.logs, a.pub, pub_tag(a.nonce, p + 1));
         if (tid == 0) ctl->prof[7] = clock64();
     }
     if (tid == 0) {
