@@ -109,6 +109,39 @@ def scan_refs(pairs, device=None):
     return torch.tensor(rows, dtype=torch.int64).reshape(-1, 2).to(device)
 
 
+class ScanRaw(C.Structure):
+    """fl_scan_raw_t: one slot's raw scan for fl_scan_batch_run_device, every pointer in device memory"""
+    _fields_ = [("xyzi", C.c_void_p), ("offset_ms", C.c_void_p), ("n", C.c_void_p), ("imu_pose22", C.c_void_p), ("n_pose", C.c_void_p),
+                ("x26_end", C.c_void_p)]
+
+
+def scan_raws(entries, device=None):
+    """The device table of fl_scan_batch_run_device: an (S, 6) int64 CUDA tensor of fl_scan_raw_t rows.  Each entry is a tuple
+    (xyzi, offset_ms, n, imu_pose22, n_pose, x26_end), or a dict with those keys (imu_pose22, n_pose and x26_end may be left out
+    when not de-skewing): xyzi an (m, 4) float32, offset_ms an (m,) float32, n and n_pose one-element int32, imu_pose22 an
+    (n_pose_max, 22) float64 and x26_end a (26,) float64 CUDA tensor, or any of them a raw device address (an int, 0 or None for
+    null).  The table is copied from the host, so build it outside stream capture; what it points at must stay alive until the
+    stream has passed the calls that read it."""
+    import torch
+    names = ("xyzi", "offset_ms", "n", "imu_pose22", "n_pose", "x26_end")
+    dtypes = (torch.float32, torch.float32, torch.int32, torch.float64, torch.int32, torch.float64)
+    rows = []
+    for e in entries:
+        vals = [e.get(k) for k in names] if isinstance(e, dict) else list(e) + [None] * (6 - len(e))
+        row = []
+        for v, name, dt in zip(vals, names, dtypes):
+            if isinstance(v, torch.Tensor):
+                if not v.is_cuda or not v.is_contiguous() or v.dtype != dt:
+                    raise ValueError(f"scan_raws: {name} must be a contiguous {dt} CUDA tensor")
+                row.append(v.data_ptr())
+            else:
+                row.append(int(v or 0))
+        rows.append(row)
+    if device is None:
+        device = torch.device("cuda", torch.cuda.current_device())
+    return torch.tensor(rows, dtype=torch.int64).reshape(-1, 6).to(device)
+
+
 class FastLioError(RuntimeError):
     pass
 
@@ -180,6 +213,8 @@ SYMBOLS = [
     "fl_preprocess_create", "fl_preprocess_destroy", "fl_preprocess_device", "fl_preprocess",
     "fl_scan_frame", "fl_scan_frame_device",
     "fl_scan_get_ref", "fl_filter_update_scans_device",
+    "fl_scan_batch_create", "fl_scan_batch_destroy", "fl_scan_batch_reserve", "fl_scan_batch_run_device", "fl_scan_batch_get_refs",
+    "fl_scan_batch_download",
 ]
 
 
@@ -241,6 +276,12 @@ def load():
     L.fl_filter_update_batch_device.argtypes = [_vp, _vp, C.c_int, C.c_int, _vp, _vp, C.c_double, _vp, _vp, _vp]
     L.fl_filter_update_scans_device.argtypes = [_vp, _vp, C.c_int, C.c_int, _vp, _vp, C.c_double, _vp, _vp, _vp]
     L.fl_scan_get_ref.argtypes = [_vp, C.POINTER(ScanRef), C.POINTER(C.c_int)]
+    L.fl_scan_batch_create.argtypes = [C.POINTER(C.c_void_p), _vp]
+    L.fl_scan_batch_destroy.argtypes = [_vp]
+    L.fl_scan_batch_reserve.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
+    L.fl_scan_batch_run_device.argtypes = [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, _vp, _vp]
+    L.fl_scan_batch_get_refs.argtypes = [_vp, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_int)]
+    L.fl_scan_batch_download.argtypes = [_vp, C.c_int, C.c_int, _f32p, C.c_int]
     L.fl_reloc_expand_grid_device.argtypes = [_vp, C.POINTER(RelocGrid), _vp, _vp]
     L.fl_filter_reserve_reloc.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
     L.fl_filter_relocalize_device.argtypes = [_vp, _vp, C.c_int, C.c_int, _vp, _vp, C.c_double, C.POINTER(RelocParams), _vp, _vp,
@@ -1010,6 +1051,79 @@ class Scan:
         _check(self._L.fl_scan_frame_device(self.h, which, frame, None if x is None else x.data_ptr(), out.data_ptr(),
                                             self._n_io.data_ptr(), out.shape[0], status.data_ptr(), t._stream()))
         return status
+
+
+class _DeviceTable:
+    """A view of device memory the batch owns, for torch.as_tensor (the __cuda_array_interface__ protocol); holds the batch."""
+
+    def __init__(self, owner, ptr: int, rows: int):
+        self.owner = owner
+        self.__cuda_array_interface__ = {"shape": (rows, 2), "typestr": "<i8", "data": (ptr, False), "version": 2}
+
+
+class ScanBatch:
+    """The scan front end of many scans in one call (fl_scan_batch_run_device): per slot UndistortPcl's sort and backward pass
+    (IMU_Processing.hpp:232-346) and the pcl::VoxelGrid down-sampling (laserMapping.cpp:904-905), each slot equal to a `Scan`'s
+    device forms on the same inputs, into the table Esekf.update_scans_device reads."""
+
+    def __init__(self, tree: KdTree):
+        self._L = load()
+        self.tree = tree
+        h = C.c_void_p()
+        _check(self._L.fl_scan_batch_create(C.byref(h), tree.h))
+        self.h = h
+
+    def close(self):
+        if getattr(self, "h", None):
+            self._L.fl_scan_batch_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def reserve(self, n_scans_max: int, n_max: int, n_pose_max: int):
+        """fl_scan_batch_reserve: buffers for up to n_scans_max slots of n_max rows and n_pose_max IMU poses (synchronous, grow-only;
+        a grow moves the buffers and the ref tables, so capture graphs again after one)."""
+        _check(self._L.fl_scan_batch_reserve(self.h, n_scans_max, n_max, n_pose_max))
+        self._slots_max = max(getattr(self, "_slots_max", 1), n_scans_max)
+
+    def run_device(self, raws, n_max: int, n_pose_max: int, leaf: float, undistort: bool = True, status=None):
+        """fl_scan_batch_run_device on the current stream: raws the (S, 6) int64 table of scan_raws.  Returns status, an (S, 2)
+        int32 tensor = (FL_OK, feats_down_size) or (refusal, 0) per slot, written on the current stream."""
+        import torch
+        t = self.tree
+        if not isinstance(raws, torch.Tensor) or raws.dtype != torch.int64 or raws.dim() != 2 or raws.shape[1] != 6:
+            raise TypeError("raws must be the (S, 6) int64 tensor of scan_raws")
+        S = raws.shape[0]
+        if S:
+            raws = t._tensor(raws, "raws", 6, torch.int64)
+        if status is None:
+            status = torch.empty((S, 2), dtype=torch.int32, device=f"cuda:{t.device}")
+        if S:
+            status = t._tensor(status, "status", None, torch.int32, (S, 2))
+        _check(self._L.fl_scan_batch_run_device(self.h, raws.data_ptr() if S else None, S, n_max, n_pose_max, 1 if undistort else 0,
+                                                leaf, status.data_ptr() if S else None, t._stream()))
+        return status
+
+    def refs(self, which: int = 1):
+        """fl_scan_batch_get_refs: the device table of n_scans_max fl_scan_ref_t entries (feats_undistort for which 0,
+        feats_down_body for 1) as an (n_scans_max, 2) int64 CUDA tensor over the batch's own memory, for Esekf.update_scans_device
+        (slice the first S rows), and the reserved n_max, its nq_max."""
+        import torch
+        p, m = C.c_void_p(), C.c_int(0)
+        _check(self._L.fl_scan_batch_get_refs(self.h, which, C.byref(p), C.byref(m)))
+        return torch.as_tensor(_DeviceTable(self, int(p.value), self._slots_max), device=f"cuda:{self.tree.device}"), int(m.value)
+
+    def download(self, which: int, slot: int) -> np.ndarray:
+        """fl_scan_batch_download: slot `slot`'s rows of the last call (which 0 feats_undistort, 1 feats_down_body) as an (n, 4)
+        float32 array; a refused slot has none."""
+        n = _check(self._L.fl_scan_batch_download(self.h, which, slot, np.zeros((1, 4), dtype=np.float32), 0))
+        out = np.zeros((max(n, 1), 4), dtype=np.float32)
+        _check(self._L.fl_scan_batch_download(self.h, which, slot, out, n))
+        return out[:n].copy()
 
 
 class LocalMap:

@@ -40,6 +40,10 @@ struct fl_scan {
     fl::ScanFrontEnd* impl;
     fl_map* map;
 };
+struct fl_scan_batch {
+    fl::ScanBatch* impl;
+    fl_map* map;
+};
 struct fl_localmap {
     fl::LocalMapCube cube;
     fl_map* map = nullptr;          // the map of the device form (retained), whose device holds the cube from then on
@@ -550,6 +554,52 @@ int fl_filter_update_scans_device(fl_filter_t* f, const fl_scan_ref_t* scans_dev
     FILTER_GUARD(f);
     return f->impl->update_scans_on_stream(scans_device, n_scans, nq_max, x26_device, P_device, R, status2_device,
                                            reinterpret_cast<fl::PassLog*>(logs_device), static_cast<cudaStream_t>(stream));
+}
+// ------------------------------------------------------------------------------------ scan front end of many scans
+static_assert(sizeof(fl_scan_raw_t) == 48, "fl_scan_raw_t is six device pointers");
+#define BATCH_GUARD(b)                                                                             \
+    if (!(b) || !(b)->impl) { fl::set_last_error("null scan batch handle"); return FL_ERR_ARG; }   \
+    std::lock_guard<std::mutex> _lk((b)->map->mu);                                                   \
+    (b)->map->impl->touch()
+int fl_scan_batch_create(fl_scan_batch_t** out, fl_map_t* map) {
+    if (!out) return FL_ERR_ARG;
+    *out = nullptr;
+    if (!map || !map->impl) { fl::set_last_error("fl_scan_batch_create: null map handle"); return FL_ERR_ARG; }
+    fl_scan_batch* b = new (std::nothrow) fl_scan_batch();
+    if (!b) return FL_ERR_CAPACITY;
+    b->map = map;
+    b->impl = new (std::nothrow) fl::ScanBatch(map->impl);
+    if (!b->impl) { delete b; return FL_ERR_CAPACITY; }
+    map_retain(map);
+    *out = b;
+    return FL_OK;
+}
+int fl_scan_batch_destroy(fl_scan_batch_t* b) {
+    if (!b) return FL_OK;
+    delete b->impl;
+    map_release(b->map);
+    delete b;
+    return FL_OK;
+}
+int fl_scan_batch_reserve(fl_scan_batch_t* b, int n_scans_max, int n_max, int n_pose_max) {
+    BATCH_GUARD(b);
+    return b->impl->reserve(n_scans_max, n_max, n_pose_max);
+}
+int fl_scan_batch_run_device(fl_scan_batch_t* b, const fl_scan_raw_t* raws_device, int n_scans, int n_max, int n_pose_max, int undistort,
+                             float leaf_size, int* status2_device, void* stream) {
+    BATCH_GUARD(b);
+    return b->impl->run_on_stream(raws_device, n_scans, n_max, n_pose_max, undistort, leaf_size, status2_device,
+                                  static_cast<cudaStream_t>(stream));
+}
+int fl_scan_batch_get_refs(fl_scan_batch_t* b, int which, const fl_scan_ref_t** refs_device, int* n_max) {
+    BATCH_GUARD(b);
+    return b->impl->refs(which, refs_device, n_max);
+}
+int fl_scan_batch_download(fl_scan_batch_t* b, int which, int slot, float* out_xyzi, int cap) {
+    BATCH_GUARD(b);
+    int n = 0;
+    const int rc = b->impl->download(which, slot, out_xyzi, cap, &n);
+    return rc == FL_OK ? n : rc;
 }
 // publish_frame_world / publish_frame_body / pointBodyToWorld                     laserMapping.cpp:177-220, :478-549, :909-921
 int fl_scan_frame(fl_scan_t* s, int which, int frame, const double* x26, float* out_xyzi, int cap) {

@@ -3,6 +3,7 @@
 #include <cfloat>
 #include <cmath>
 #include <cstring>
+#include <vector>
 
 #include <cub/cub.cuh>
 
@@ -78,12 +79,39 @@ __device__ __forceinline__ void compensate(float4& p, double t, const double* he
     p.x = float(out.x); p.y = float(out.y); p.z = float(out.z);
 }
 
+__device__ __forceinline__ EndState end_state(const double* x_end) {
+    EndState e;
+    e.pos = ld3(x_end);
+    e.rot_inv = qconj(ldq(x_end + 3));
+    e.offR = ldq(x_end + 7);
+    e.offR_inv = qconj(e.offR);
+    e.offT = ld3(x_end + 11);
+    return e;
+}
+
 // The reference sweeps points and IMU segments backwards together (:314-345).  For time-sorted points that
 // is: point i belongs to the LAST segment kp whose head is strictly older than the point; points older than
 // every head stay untouched.  One quirk is kept: the sweep `break`s on the first point and then re-tests
 // it against every earlier segment, so point 0 is compensated once per earlier segment that is older than it.
 // Device forms: n and n_pose are the row bounds, the counts are min(*n_dev, n) and *n_pose_dev clamped to [0, n_pose], and
 // the kernel marks the device forms' cloud as de-skewed and current (dc: null in the host form).
+// Row i of the sorted cloud, at time t (s), through the segments of the n_pose poses in s_pose; written back only when it moved.
+// k_batch_undistort's form of k_undistort's loop below, which keeps its own copy: calling this helper there flips one branch of
+// its SASS (tests/golden/sass_scan_kernels_sm90a.json pins it).
+__device__ __forceinline__ void undistort_row(float4* __restrict__ pts, int i, double t, const double* s_pose, int n_pose, const EndState& e) {
+    float4 p = pts[i];
+    bool touched = false;
+    for (int kp = n_pose - 1; kp >= 1; kp--) {
+        const double* head = s_pose + (kp - 1) * POSE_DOUBLES;
+        if (t > head[0]) {
+            compensate(p, t, head, head + POSE_DOUBLES, e);
+            touched = true;
+            if (i != 0) break;
+        }
+    }
+    if (touched) pts[i] = p;
+}
+
 __global__ void k_undistort(float4* __restrict__ pts, const float* __restrict__ t_ms, int n,
                             const double* __restrict__ poses, int n_pose, const double* __restrict__ x_end,
                             const int* __restrict__ n_dev, const int* __restrict__ n_pose_dev, ScanDevCtl* dc) {
@@ -139,11 +167,11 @@ __global__ void k_upload_n(const float4* __restrict__ xyzi, const float* __restr
     else time[i] = __int_as_float(0x7FFFFFFF);
 }
 
-// getMinMax3D (pcl/common/impl/common.hpp) over a dense cloud
-__global__ void k_vg_minmax(const float4* __restrict__ pts, int n, VgCtl* c, const int* __restrict__ n_dev) {
-    n = dev_count(n_dev, n);
+// getMinMax3D (pcl/common/impl/common.hpp) over a dense cloud: the block's rows i = block * blockDim.x + threadIdx.x, strided by
+// blocks * blockDim.x, into c's bounds
+__device__ __forceinline__ void vg_minmax_block(const float4* __restrict__ pts, int n, VgCtl* c, int block, int blocks) {
     float mn[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, mx[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    for (int i = block * blockDim.x + threadIdx.x; i < n; i += blocks * blockDim.x) {
         const float4 p = pts[i];
         mn[0] = fminf(mn[0], p.x); mx[0] = fmaxf(mx[0], p.x);
         mn[1] = fminf(mn[1], p.y); mx[1] = fmaxf(mx[1], p.y);
@@ -174,6 +202,10 @@ __global__ void k_vg_minmax(const float4* __restrict__ pts, int n, VgCtl* c, con
     }
 }
 
+__global__ void k_vg_minmax(const float4* __restrict__ pts, int n, VgCtl* c, const int* __restrict__ n_dev) {
+    vg_minmax_block(pts, dev_count(n_dev, n), c, blockIdx.x, gridDim.x);
+}
+
 struct VgGrid {
     float inv;
     int min_b[3], mul[3];
@@ -197,6 +229,15 @@ __device__ __forceinline__ VgGrid vg_grid(const VgCtl* c, float leaf) {
     return g;
 }
 
+// A real row's voxel key: its cell's index in the grid, or in passthrough mode its row index i, which makes the "cell" the point
+// itself and turns the rest of the pipeline into a copy
+__device__ __forceinline__ unsigned vg_key(const float4& p, const VgGrid& g, int i) {
+    const int i0 = int(__fsub_rn(floorf(__fmul_rn(p.x, g.inv)), float(g.min_b[0])));
+    const int i1 = int(__fsub_rn(floorf(__fmul_rn(p.y, g.inv)), float(g.min_b[1])));
+    const int i2 = int(__fsub_rn(floorf(__fmul_rn(p.z, g.inv)), float(g.min_b[2])));
+    return g.overflow ? unsigned(i) : unsigned(i0 * g.mul[0] + i1 * g.mul[1] + i2 * g.mul[2]);
+}
+
 // Padding rows (device forms) get the key 0xFFFFFFFF.  Real keys are below 2^31 (the overflow test bounds the grid, passthrough
 // keys are row indices), and a real key equal to it would still precede the padding rows in the stable sort.
 __global__ void k_vg_keys(const float4* __restrict__ pts, int n, float leaf, VgCtl* c, unsigned* __restrict__ keys, int* __restrict__ vals,
@@ -206,12 +247,7 @@ __global__ void k_vg_keys(const float4* __restrict__ pts, int n, float leaf, VgC
     if (i == 0) c->passthrough = g.overflow ? 1 : 0;
     if (i >= n) return;
     if (i >= dev_count(n_dev, n)) { keys[i] = 0xFFFFFFFFu; vals[i] = i; return; }
-    const float4 p = pts[i];
-    const int i0 = int(__fsub_rn(floorf(__fmul_rn(p.x, g.inv)), float(g.min_b[0])));
-    const int i1 = int(__fsub_rn(floorf(__fmul_rn(p.y, g.inv)), float(g.min_b[1])));
-    const int i2 = int(__fsub_rn(floorf(__fmul_rn(p.z, g.inv)), float(g.min_b[2])));
-    // in passthrough mode the "cell" is the point itself, which turns the rest of the pipeline into a copy
-    keys[i] = g.overflow ? unsigned(i) : unsigned(i0 * g.mul[0] + i1 * g.mul[1] + i2 * g.mul[2]);
+    keys[i] = vg_key(pts[i], g, i);
     vals[i] = i;
 }
 
@@ -222,16 +258,10 @@ __global__ void k_vg_heads(const unsigned* __restrict__ keys, int n, int* __rest
 }
 
 // CentroidPoint per occupied cell: float sums in ascending input index (the radix sort is stable), then / count.
-// One thread per cell walks its run; raw scans put a handful of points into a cell.
-__global__ void k_vg_centroid(const float4* __restrict__ pts, const unsigned* __restrict__ keys, const int* __restrict__ vals,
-                              const int* __restrict__ heads, const int* __restrict__ pos, int n, float4* __restrict__ out, VgCtl* c,
-                              const int* __restrict__ n_dev) {
-    n = dev_count(n_dev, n);
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    if (i == n - 1) c->total = pos[i] + heads[i];
-    if (!heads[i]) return;
-    const unsigned key = keys[i];
+// One thread per cell walks its run; raw scans put a handful of points into a cell.  The run of head row i among rows [0, n):
+template <class Key>
+__device__ __forceinline__ float4 vg_run(const float4* __restrict__ pts, const Key* __restrict__ keys, const int* __restrict__ vals, int i, int n) {
+    const Key key = keys[i];
     float sx = 0.f, sy = 0.f, sz = 0.f, si = 0.f;
     int j = i;
     do {
@@ -240,7 +270,18 @@ __global__ void k_vg_centroid(const float4* __restrict__ pts, const unsigned* __
         j++;
     } while (j < n && keys[j] == key);
     const float cnt = float(j - i);
-    out[pos[i]] = make_float4(__fdiv_rn(sx, cnt), __fdiv_rn(sy, cnt), __fdiv_rn(sz, cnt), __fdiv_rn(si, cnt));
+    return make_float4(__fdiv_rn(sx, cnt), __fdiv_rn(sy, cnt), __fdiv_rn(sz, cnt), __fdiv_rn(si, cnt));
+}
+
+__global__ void k_vg_centroid(const float4* __restrict__ pts, const unsigned* __restrict__ keys, const int* __restrict__ vals,
+                              const int* __restrict__ heads, const int* __restrict__ pos, int n, float4* __restrict__ out, VgCtl* c,
+                              const int* __restrict__ n_dev) {
+    n = dev_count(n_dev, n);
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    if (i == n - 1) c->total = pos[i] + heads[i];
+    if (!heads[i]) return;
+    out[pos[i]] = vg_run(pts, keys, vals, i, n);
 }
 
 // ------------------------------------------------------------------------------------------------ clouds in a frame
@@ -274,6 +315,142 @@ __global__ void k_frame_commit(const int* __restrict__ n_dev, int n_max, int* __
     if (st == FL_OK) *n_io = pos + n;
     status2[0] = st;
     status2[1] = n;
+}
+
+
+// ------------------------------------------------------------------------------------------------ many scans (ScanBatch)
+// Slot s owns rows [s * n_max, (s + 1) * n_max) of every packed buffer; the grids are (row blocks, slots), so blockIdx.y is the slot.
+struct BatchSlot {
+    VgCtl vg;           // the slot's voxel grid; vg.total: its feats_down_size
+    int n;              // its count c, 0 for a refused slot
+    int err;            // FL_OK or its refusal
+};
+
+// cub's radix key for a float (its RadixSortTwiddle): -0.0 folded onto +0.0, then the sign-dependent flip.  Below the slot index
+// in bits 32 and up, one sort orders every slot's rows by time as the single form's sort orders the scan's, stably.
+__device__ __forceinline__ unsigned twiddle_f32(float t) {
+    unsigned b = __float_as_uint(t);
+    if (b == 0x80000000u) b = 0u;
+    return b ^ ((b & 0x80000000u) ? 0xFFFFFFFFu : 0x80000000u);
+}
+// the float a sorted key stands for; -0.0 comes back as +0.0, which k_undistort's arithmetic cannot tell apart (the time only
+// enters through t > head[0], true for neither zero against any head, and t - head[0] of a point older than its head)
+__device__ __forceinline__ float untwiddle_f32(unsigned k) { return __uint_as_float(k ^ ((k & 0x80000000u) ? 0x80000000u : 0xFFFFFFFFu)); }
+
+__device__ __forceinline__ bool misaligned(const void* p, unsigned align) { return (reinterpret_cast<uintptr_t>(p) & (align - 1)) != 0; }
+
+// fl_scan_batch_run_device's first step, k_upload_n per slot: the slot's refusal is decided, its first c rows are copied into the
+// packed buffer and, when de-skewing, their time keys written, the padding rows carrying the padding time (0x7FFFFFFF, whose key
+// 0xFFFFFFFF sorts after every real row of the slot).  Thread 0 of each slot resets its voxel grid and writes its ref-table
+// entries; block (0, 0) also sets the counts of the slots [n_scans, n_scans_max) to -1.
+__global__ void k_batch_gather(const fl_scan_raw_t* __restrict__ raws, int n_scans, int n_scans_max, int n_max, int n_pose_max, int undistort,
+                               float4* __restrict__ raw, unsigned long long* __restrict__ keys, const float4* sraw, const float4* down,
+                               BatchSlot* __restrict__ slots, fl_scan_ref_t* __restrict__ refs, int* __restrict__ counts) {
+    const int s = blockIdx.y;
+    const fl_scan_raw_t r = raws[s];
+    int err = FL_OK, c = 0;
+    if (!r.n || misaligned(r.n, 4)) err = FL_ERR_ARG;
+    else {
+        c = *r.n;
+        if (c < 0) err = FL_ERR_ARG;
+        else if (c > n_max) err = FL_ERR_CAPACITY;
+        else if (c > 0 && (!r.xyzi || misaligned(r.xyzi, 16) || !r.offset_ms || misaligned(r.offset_ms, 4))) err = FL_ERR_ARG;
+        else if (undistort) {
+            if (!r.x26_end || misaligned(r.x26_end, 8) || misaligned(r.n_pose, 4)) err = FL_ERR_ARG;
+            else if (r.n_pose && min(max(*r.n_pose, 0), n_pose_max) >= 2 && (!r.imu_pose22 || misaligned(r.imu_pose22, 8))) err = FL_ERR_ARG;
+        }
+    }
+    if (err != FL_OK) c = 0;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const size_t row = (size_t)s * n_max + i;
+    if (i == 0) {
+        BatchSlot& b = slots[s];
+        for (int a = 0; a < 3; a++) { b.vg.mn[a] = FLT_MAX; b.vg.mx[a] = -FLT_MAX; }
+        b.vg.total = 0; b.vg.passthrough = 0;
+        b.n = c; b.err = err;
+        const size_t base = (size_t)s * n_max;
+        refs[s].body_xyzi = reinterpret_cast<const float*>((undistort ? sraw : raw) + base);
+        refs[s].n = counts + s;
+        refs[n_scans_max + s].body_xyzi = reinterpret_cast<const float*>(down + base);
+        refs[n_scans_max + s].n = counts + n_scans_max + s;
+        counts[s] = err == FL_OK ? c : -1;
+        counts[n_scans_max + s] = -1;                       // k_batch_commit writes feats_down_size
+    }
+    if (s == 0 && blockIdx.x == 0)
+        for (int t = n_scans + threadIdx.x; t < n_scans_max; t += blockDim.x) counts[t] = counts[n_scans_max + t] = -1;
+    if (i >= n_max) return;
+    if (i < c) raw[row] = reinterpret_cast<const float4*>(r.xyzi)[i];
+    if (undistort) keys[row] = ((unsigned long long)s << 32) | (i < c ? twiddle_f32(r.offset_ms[i]) : 0xFFFFFFFFu);
+}
+
+// k_undistort per slot over the time-sorted rows: each block belongs to one slot and loads that slot's poses into shared memory
+__global__ void k_batch_undistort(float4* __restrict__ pts, const unsigned long long* __restrict__ keys, int n_max,
+                                  const fl_scan_raw_t* __restrict__ raws, int n_pose_max, const BatchSlot* __restrict__ slots) {
+    extern __shared__ double s_pose[];
+    const int s = blockIdx.y;
+    if (slots[s].err != FL_OK) return;
+    const fl_scan_raw_t r = raws[s];
+    const int n_pose = r.n_pose ? min(max(*r.n_pose, 0), n_pose_max) : 0;
+    if (n_pose < 2) return;                                 // no segment: the points stay as sorted
+    const int n = slots[s].n;
+    for (int i = threadIdx.x; i < n_pose * POSE_DOUBLES; i += blockDim.x) s_pose[i] = r.imu_pose22[i];
+    __syncthreads();
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const EndState e = end_state(r.x26_end);
+    const size_t base = (size_t)s * n_max;
+    undistort_row(pts + base, i, double(untwiddle_f32(unsigned(keys[base + i]))) / double(1000), s_pose, n_pose, e);
+}
+
+__global__ void k_batch_minmax(const float4* __restrict__ pts, int n_max, BatchSlot* slots) {
+    const int s = blockIdx.y;
+    vg_minmax_block(pts + (size_t)s * n_max, slots[s].n, &slots[s].vg, blockIdx.x, gridDim.x);
+}
+
+// k_vg_keys per slot, the slot index above the 32-bit key; the values are global rows
+__global__ void k_batch_keys(const float4* __restrict__ pts, int n_max, float leaf, BatchSlot* slots, unsigned long long* __restrict__ keys,
+                             int* __restrict__ vals) {
+    const int s = blockIdx.y;
+    const VgGrid g = vg_grid(&slots[s].vg, leaf);
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i == 0) slots[s].vg.passthrough = g.overflow ? 1 : 0;
+    if (i >= n_max) return;
+    const size_t row = (size_t)s * n_max + i;
+    keys[row] = ((unsigned long long)s << 32) | (i < slots[s].n ? vg_key(pts[row], g, i) : 0xFFFFFFFFu);
+    vals[row] = (int)row;
+}
+
+// k_vg_heads per slot: the heads restart at each slot's first row, padding rows are none
+__global__ void k_batch_heads(const unsigned long long* __restrict__ keys, int n_max, const BatchSlot* __restrict__ slots, int* __restrict__ heads) {
+    const int s = blockIdx.y;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_max) return;
+    const size_t row = (size_t)s * n_max + i;
+    heads[row] = (i < slots[s].n && (i == 0 || keys[row] != keys[row - 1])) ? 1 : 0;
+}
+
+// k_vg_centroid per slot: positions of the one exclusive scan over every slot, less the slot's first; rows at s * n_max + position
+__global__ void k_batch_centroid(const float4* __restrict__ pts, const unsigned long long* __restrict__ keys, const int* __restrict__ vals,
+                                 const int* __restrict__ heads, const int* __restrict__ pos, int n_max, float4* __restrict__ out, BatchSlot* slots) {
+    const int s = blockIdx.y;
+    const int n = slots[s].n;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const size_t base = (size_t)s * n_max;
+    const int at = pos[base + i] - pos[base];
+    if (i == n - 1) slots[s].vg.total = at + heads[base + i];
+    if (!heads[base + i]) return;
+    out[base + at] = vg_run(pts, keys + base, vals + base, i, n);
+}
+
+// status2 = (FL_OK, feats_down_size) and the count of ref table 1, or (refusal, 0) and -1
+__global__ void k_batch_commit(const BatchSlot* __restrict__ slots, int n_scans, int n_scans_max, int* __restrict__ counts, int* __restrict__ status2) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n_scans) return;
+    const int err = slots[s].err, total = err == FL_OK ? slots[s].vg.total : 0;
+    counts[n_scans_max + s] = err == FL_OK ? total : -1;
+    status2[2 * s] = err;
+    status2[2 * s + 1] = total;
 }
 
 }  // namespace
@@ -629,6 +806,175 @@ int ScanFrontEnd::settle() {
         FL_CUDA(cudaMemcpyAsync(down_.ptr, d_down_.ptr, sizeof(float4) * (size_t)n_down_, cudaMemcpyDeviceToDevice, st));
     }
     FL_CUDA(cudaMemsetAsync(&d_ctl_.as<ScanDevCtl>()->src, 0, sizeof(int), st));
+    return FL_OK;
+}
+
+// ================================================================================================ ScanBatch
+ScanBatch::~ScanBatch() {
+    cudaSetDevice(map_->device());
+    DeviceBuffer* all[] = {&raw_, &sraw_, &down_, &keys_, &keys_alt_, &vals_, &vals_alt_, &heads_, &pos_, &cub_, &slots_, &refs_, &counts_};
+    for (DeviceBuffer* b : all) b->release();
+}
+
+namespace {
+// the bits the slot index takes above the 32-bit keys of n_scans slots
+int slot_bits(int n_scans) {
+    int b = 0;
+    while ((1ll << b) < (long long)n_scans) b++;
+    return b;
+}
+}  // namespace
+
+// cub's temporary storage for both sorts and the scan over `rows` packed rows, the sorts on bits [0, end_bit)
+int ScanBatch::cub_bytes(int rows, int end_bit, size_t* bytes) const {
+    using U64 = unsigned long long;
+    size_t t_time = 0, t_vg = 0, t_scan = 0;
+    FL_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t_time, (const U64*)nullptr, (U64*)nullptr, (const float4*)nullptr, (float4*)nullptr, rows, 0, end_bit));
+    FL_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t_vg, (const U64*)nullptr, (U64*)nullptr, (const int*)nullptr, (int*)nullptr, rows, 0, end_bit));
+    FL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, t_scan, (const int*)nullptr, (int*)nullptr, rows));
+    *bytes = std::max(t_time, std::max(t_vg, t_scan));
+    return FL_OK;
+}
+
+int ScanBatch::reserve(int n_scans_max, int n_max, int n_pose_max) {
+    if (n_scans_max < 0 || n_max < 0 || n_pose_max < 0) {
+        set_last_error("scan batch reserve: n_scans_max, n_max and n_pose_max must be >= 0");
+        return FL_ERR_ARG;
+    }
+    const int S = std::max(res_slots_, n_scans_max), m = std::max(res_n_max_, n_max), np = std::max(res_pose_max_, n_pose_max);
+    const size_t smem = sizeof(double) * POSE_DOUBLES * (size_t)np;
+    if (smem > UNDISTORT_SMEM_MAX || S > SLOTS_MAX || (long long)S * m > (long long)INT_MAX) {
+        set_last_error("scan batch reserve: %d IMU poses (shared memory holds %d), %d slots (at most %d) or %lld rows (at most INT_MAX)", np,
+                       (int)(UNDISTORT_SMEM_MAX / (sizeof(double) * POSE_DOUBLES)), S, SLOTS_MAX, (long long)S * m);
+        return FL_ERR_CAPACITY;
+    }
+    if (reserved_ && S == res_slots_ && m == res_n_max_ && np == res_pose_max_) return FL_OK;
+    FL_CUDA(cudaSetDevice(map_->device()));
+    FL_CUDA(cudaStreamSynchronize(map_->stream()));
+    const size_t rows = (size_t)std::max(1, S * m), slots = (size_t)std::max(1, S);
+    FL_CHECK(raw_.reserve(sizeof(float4) * rows));
+    FL_CHECK(sraw_.reserve(sizeof(float4) * rows));
+    FL_CHECK(down_.reserve(sizeof(float4) * rows));
+    FL_CHECK(keys_.reserve(sizeof(unsigned long long) * rows));
+    FL_CHECK(keys_alt_.reserve(sizeof(unsigned long long) * rows));
+    FL_CHECK(vals_.reserve(sizeof(int) * rows));
+    FL_CHECK(vals_alt_.reserve(sizeof(int) * rows));
+    FL_CHECK(heads_.reserve(sizeof(int) * rows));
+    FL_CHECK(pos_.reserve(sizeof(int) * rows));
+    size_t tmp = 0;
+    FL_CHECK(cub_bytes((int)rows, 32 + slot_bits(S), &tmp));
+    FL_CHECK(cub_.reserve(tmp));
+    FL_CHECK(slots_.reserve(sizeof(BatchSlot) * slots));
+    FL_CHECK(refs_.reserve(sizeof(fl_scan_ref_t) * 2 * slots));
+    FL_CHECK(counts_.reserve(sizeof(int) * 2 * slots));
+    // table 0 then table 1, n_scans_max entries each; every entry starts as a slot with no rows (count -1)
+    std::vector<fl_scan_ref_t> t(2 * slots);
+    for (size_t s = 0; s < slots; s++) {
+        t[s].body_xyzi = reinterpret_cast<const float*>(raw_.as<float4>() + s * m);
+        t[s].n = counts_.as<int>() + s;
+        t[slots + s].body_xyzi = reinterpret_cast<const float*>(down_.as<float4>() + s * m);
+        t[slots + s].n = counts_.as<int>() + slots + s;
+    }
+    FL_CUDA(cudaMemcpyAsync(refs_.ptr, t.data(), sizeof(fl_scan_ref_t) * 2 * slots, cudaMemcpyHostToDevice, map_->stream()));
+    FL_CUDA(cudaMemsetAsync(counts_.ptr, 0xFF, sizeof(int) * 2 * slots, map_->stream()));
+    if (smem > undistort_smem_) {
+        FL_CUDA(cudaFuncSetAttribute(k_batch_undistort, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        undistort_smem_ = smem;
+    }
+    FL_CUDA(cudaStreamSynchronize(map_->stream()));
+    res_slots_ = (int)slots;
+    res_n_max_ = m;
+    res_pose_max_ = np;
+    reserved_ = true;
+    return FL_OK;
+}
+
+int ScanBatch::run_on_stream(const fl_scan_raw_t* d_raws, int n_scans, int n_max, int n_pose_max, int undistort, float leaf, int* d_status2,
+                             cudaStream_t st) {
+    const int dev = map_->device();
+    if (n_scans < 0 || n_max < 0 || n_pose_max < 0 || !(leaf > 0.f) || (undistort != 0 && undistort != 1) ||
+        (n_scans > 0 && (!device_ptr(d_raws, dev, 8) || !device_ptr(d_status2, dev, 4)))) {
+        set_last_error("scan batch run_device: n_scans, n_max or n_pose_max < 0, leaf not > 0, undistort not 0 or 1, or a buffer is not "
+                       "device memory on device %d (table 8-byte, status 4-byte aligned)", dev);
+        return FL_ERR_ARG;
+    }
+    if (!reserved_) { set_last_error("scan batch run_device: call fl_scan_batch_reserve first"); return FL_ERR_STATE; }
+    const size_t smem = sizeof(double) * POSE_DOUBLES * (size_t)n_pose_max;
+    if (n_scans > res_slots_ || n_max > res_n_max_ || n_pose_max > res_pose_max_ || smem > UNDISTORT_SMEM_MAX ||
+        (long long)n_scans * n_max > (long long)INT_MAX) {
+        set_last_error("scan batch run_device: %d slots, %d rows or %d poses exceed the %d, %d and %d fl_scan_batch_reserve sized", n_scans,
+                       n_max, n_pose_max, res_slots_, res_n_max_, res_pose_max_);
+        return FL_ERR_CAPACITY;
+    }
+    if (n_scans == 0) return FL_OK;
+    const int rows = n_scans * n_max, end_bit = 32 + slot_bits(n_scans);
+    size_t need = 0;
+    FL_CHECK(cub_bytes(rows, end_bit, &need));
+    if (need > cub_.bytes) { set_last_error("scan batch run_device: %d rows exceed what fl_scan_batch_reserve sized", rows); return FL_ERR_CAPACITY; }
+    FL_CUDA(cudaSetDevice(dev));
+    bool joined = false;
+    FL_CHECK(map_->query_begin(st, &joined));
+    using U64 = unsigned long long;
+    BatchSlot* slots = slots_.as<BatchSlot>();
+    float4 *raw = raw_.as<float4>(), *sraw = sraw_.as<float4>(), *down = down_.as<float4>();
+    U64 *keys = keys_.as<U64>(), *keys_alt = keys_alt_.as<U64>();
+    int *vals = vals_.as<int>(), *vals_alt = vals_alt_.as<int>(), *heads = heads_.as<int>(), *pos = pos_.as<int>(), *counts = counts_.as<int>();
+    const int block = 256, gx = std::max(1, (n_max + block - 1) / block);
+    k_batch_gather<<<dim3(gx, n_scans), block, 0, st>>>(d_raws, n_scans, res_slots_, n_max, n_pose_max, undistort, raw, keys, sraw, down, slots,
+                                                        refs_.as<fl_scan_ref_t>(), counts);
+    const float4* src = raw;
+    if (undistort && rows > 0) {
+        // the stable time sort of every slot at once (slot index above cub's float key), then the backward pass per slot
+        size_t tmp = cub_.bytes;
+        FL_CUDA(cub::DeviceRadixSort::SortPairs(cub_.ptr, tmp, keys, keys_alt, raw, sraw, rows, 0, end_bit, st));
+        const int ub = 128;
+        k_batch_undistort<<<dim3((n_max + ub - 1) / ub, n_scans), ub, smem, st>>>(sraw, keys_alt, n_max, d_raws, n_pose_max, slots);
+        src = sraw;
+    }
+    if (rows > 0) {
+        k_batch_minmax<<<dim3(std::min(gx, 32), n_scans), block, 0, st>>>(src, n_max, slots);
+        k_batch_keys<<<dim3(gx, n_scans), block, 0, st>>>(src, n_max, leaf, slots, keys, vals);
+        size_t tmp = cub_.bytes;
+        FL_CUDA(cub::DeviceRadixSort::SortPairs(cub_.ptr, tmp, keys, keys_alt, vals, vals_alt, rows, 0, end_bit, st));
+        k_batch_heads<<<dim3(gx, n_scans), block, 0, st>>>(keys_alt, n_max, slots, heads);
+        tmp = cub_.bytes;
+        FL_CUDA(cub::DeviceScan::ExclusiveSum(cub_.ptr, tmp, heads, pos, rows, st));
+        k_batch_centroid<<<dim3(gx, n_scans), block, 0, st>>>(src, keys_alt, vals_alt, heads, pos, n_max, down, slots);
+    }
+    k_batch_commit<<<(n_scans + 127) / 128, 128, 0, st>>>(slots, n_scans, res_slots_, counts, d_status2);
+    FL_CUDA(cudaGetLastError());
+    return map_->query_end(st, joined);
+}
+
+int ScanBatch::refs(int which, const fl_scan_ref_t** out, int* n_max) const {
+    if ((which != 0 && which != 1) || !out) { set_last_error("scan batch get_refs: which must be 0 or 1, and out non-null"); return FL_ERR_ARG; }
+    if (!reserved_) { set_last_error("scan batch get_refs: call fl_scan_batch_reserve first"); return FL_ERR_STATE; }
+    *out = refs_.as<fl_scan_ref_t>() + (size_t)which * res_slots_;
+    if (n_max) *n_max = res_n_max_;
+    return FL_OK;
+}
+
+// the slot's entry of the table (where the last call put its rows) and its count, then the rows
+int ScanBatch::download(int which, int slot, float* out_xyzi, int cap, int* n) {
+    if (n) *n = 0;
+    if (which != 0 && which != 1) { set_last_error("scan batch download: which must be 0 or 1"); return FL_ERR_ARG; }
+    if (!reserved_) { set_last_error("scan batch download: call fl_scan_batch_reserve first"); return FL_ERR_STATE; }
+    if (slot < 0 || slot >= res_slots_) { set_last_error("scan batch download: slot %d outside [0, %d)", slot, res_slots_); return FL_ERR_ARG; }
+    FL_CUDA(cudaSetDevice(map_->device()));
+    cudaStream_t st = map_->stream();
+    fl_scan_ref_t r;
+    int c = 0;
+    const size_t e = (size_t)which * res_slots_ + slot;
+    FL_CUDA(cudaMemcpyAsync(&r, refs_.as<fl_scan_ref_t>() + e, sizeof(r), cudaMemcpyDeviceToHost, st));
+    FL_CUDA(cudaMemcpyAsync(&c, counts_.as<int>() + e, sizeof(int), cudaMemcpyDeviceToHost, st));
+    FL_CUDA(cudaStreamSynchronize(st));
+    c = std::max(c, 0);
+    if (n) *n = c;
+    const int take = std::min(c, cap);
+    if (take <= 0) return FL_OK;
+    if (!out_xyzi) { set_last_error("scan batch download: null buffer"); return FL_ERR_ARG; }
+    FL_CUDA(cudaMemcpyAsync(out_xyzi, r.body_xyzi, sizeof(float4) * (size_t)take, cudaMemcpyDeviceToHost, st));
+    FL_CUDA(cudaStreamSynchronize(st));
     return FL_OK;
 }
 

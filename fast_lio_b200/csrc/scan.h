@@ -66,6 +66,33 @@ private:
     bool dev_used_ = false, dev_uploaded_ = false, dev_undistorted_ = false, dev_down_ = false;
 };
 
+// The scan front end of many scans in one call (fl_scan_batch_run_device): slot s of the packed [n_scans][n_max] buffers goes through
+// the device forms' steps -- upload, stable time sort, de-skew, voxel grid -- with the kernels of ScanFrontEnd's stages run per slot,
+// and one cub sort or scan over every slot at once where ScanFrontEnd runs one per scan.  The buffers are fixed between reserves.
+class ScanBatch {
+public:
+    explicit ScanBatch(Map* map) : map_(map) {}
+    ~ScanBatch();
+    int reserve(int n_scans_max, int n_max, int n_pose_max);       // synchronous, grow-only
+    int run_on_stream(const fl_scan_raw_t* d_raws, int n_scans, int n_max, int n_pose_max, int undistort, float leaf, int* d_status2,
+                      cudaStream_t st);
+    int refs(int which, const fl_scan_ref_t** out, int* n_max) const;
+    int download(int which, int slot, float* out_xyzi, int cap, int* n);
+    Map* map() const { return map_; }
+
+private:
+    static constexpr size_t UNDISTORT_SMEM_MAX = 200 * 1024;       // as ScanFrontEnd's
+    static constexpr int SLOTS_MAX = 65535;                          // the grids' y dimension
+    int cub_bytes(int rows, int end_bit, size_t* bytes) const;
+    Map* map_;
+    int res_slots_ = 0, res_n_max_ = 0, res_pose_max_ = 0;
+    bool reserved_ = false;
+    size_t undistort_smem_ = 48 * 1024;
+    // rows as uploaded -> time-sorted and de-skewed -> down-sampled, each [n_scans][n_max]; the radix keys and values of both sorts,
+    // the heads and their positions; per slot a BatchSlot (scan.cu); the two ref tables [2][n_scans_max] and their counts
+    DeviceBuffer raw_, sraw_, down_, keys_, keys_alt_, vals_, vals_alt_, heads_, pos_, cub_, slots_, refs_, counts_;
+};
+
 // LocalMap_Points (:229) and Localmap_Initialized (:230)
 struct CubeBox {
     float lo[3], hi[3];

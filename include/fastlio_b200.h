@@ -525,6 +525,49 @@ int fl_scan_get_ref(fl_scan_t* s, fl_scan_ref_t* out, int* n_max);
 int fl_filter_update_scans_device(fl_filter_t* f, const fl_scan_ref_t* scans_device, int n_scans, int nq_max, double* x26_device,
                                   double* P_device, double R, int* status2_device, fl_pass_log_t* logs_device, void* stream);
 
+/* ---- batched scan front end: UndistortPcl and the voxel grid of many scans in one call, into the table the batched update reads
+ * (a fleet's raw scans in, every robot's feats_down_body out, then one fl_filter_update_scans_device)
+ * raws_device is a device table of n_scans fl_scan_raw_t.  For slot s the count c = *raws_device[s].n is read when `stream`
+ * reaches the call.  If 0 <= c <= n_max and the slot's pointers are valid, the slot's feats_undistort (which 0) and
+ * feats_down_body (which 1) rows and its feats_down_size equal, byte for byte, what one fl_scan_t gives for the same inputs:
+ * undistort 1: fl_scan_upload_device -> fl_scan_undistort_device -> fl_scan_voxel_downsample_device; undistort 0: upload ->
+ * voxel_downsample (the cloud in upload order).  status2_device[s] = (FL_OK, feats_down_size).
+ * A refused slot: a null or misaligned (4-byte) n; c < 0; a null or misaligned xyzi (16-byte) or offset_ms (4-byte) with c > 0; with
+ * undistort 1 a null or misaligned (8-byte) x26_end, a misaligned n_pose, or a null or misaligned (8-byte) imu_pose22 while
+ * *n_pose, clamped to [0, n_pose_max], is >= 2 (a null n_pose is no pose) -- each (FL_ERR_ARG, 0); c > n_max (FL_ERR_CAPACITY, 0).
+ * Its counts in both ref tables are -1, which fl_filter_update_scans_device refuses with (FL_ERR_ARG, 0); no other slot depends
+ * on it.  The inputs are copied on `stream`: the caller may reuse them once `stream` has passed the call.  Slots may share or
+ * overlap their inputs, and may point at fl_preprocess_device outputs (n = &out2_device[0]).
+ * The outputs live in the handle: per slot a region of n_max rows and a count.  fl_scan_batch_get_refs gives the device table of
+ * n_scans_max fl_scan_ref_t for `which` (0 or 1), to hand straight to fl_filter_update_scans_device(f, refs, n_scans, *n_max, ...);
+ * slots the last call did not cover have the count -1.  The table's address stays valid until a reserve that grows the handle
+ * (capture again after one); its entries are written by each call.  fl_scan_batch_download copies slot `slot`'s rows of the last
+ * call into host memory (synchronous, at most cap rows) and returns the slot's count, 0 for a refused slot.
+ * The conventions, ordering and capture rules of the scan front end's device forms: no host synchronisation, no allocation, grids
+ * follow n_scans x n_max, and the number of launches does not depend on n_scans.  n_scans = 0 returns FL_OK and enqueues nothing.
+ * Refusals enqueue nothing, also on a capturing stream.  FL_ERR_ARG: n_scans, n_max or n_pose_max < 0, leaf_size not > 0,
+ * undistort not 0 or 1, a host, wrong-device, null or misaligned table (8-byte) or status (4-byte).  FL_ERR_STATE: no
+ * fl_scan_batch_reserve yet.  FL_ERR_CAPACITY: n_scans, n_max or n_pose_max above what was reserved, or n_scans x n_max above
+ * INT_MAX.  fl_scan_batch_reserve (synchronous, grow-only) sizes the buffers, cub's temporary storage and k_undistort's shared
+ * memory; FL_ERR_CAPACITY when n_pose_max poses exceed the 200 KB of shared memory fl_scan_undistort allows, n_scans_max is
+ * above 65535 or n_scans_max x n_max above INT_MAX. */
+typedef struct fl_scan_raw {
+    const float* xyzi;          /* device: rows (x, y, z, intensity), 16-byte aligned -- Measures.lidar */
+    const float* offset_ms;     /* device: PointType::curvature per row, 4-byte aligned */
+    const int* n;               /* device: the row count, read when the stream reaches the call */
+    const double* imu_pose22;   /* device: IMUpose, n_pose x 22 doubles (fl_scan_undistort's layout); may be NULL when undistort is 0 */
+    const int* n_pose;          /* device: the pose count, clamped to [0, n_pose_max] as fl_scan_undistort_device does */
+    const double* x26_end;      /* device: kf_state.get_x() after the last predict (26 doubles); may be NULL when undistort is 0 */
+} fl_scan_raw_t;                /* 48 bytes */
+typedef struct fl_scan_batch fl_scan_batch_t;
+int fl_scan_batch_create(fl_scan_batch_t** out, fl_map_t* map);
+int fl_scan_batch_destroy(fl_scan_batch_t* b);
+int fl_scan_batch_reserve(fl_scan_batch_t* b, int n_scans_max, int n_max, int n_pose_max);
+int fl_scan_batch_run_device(fl_scan_batch_t* b, const fl_scan_raw_t* raws_device, int n_scans, int n_max, int n_pose_max,
+                             int undistort, float leaf_size, int* status2_device, void* stream);
+int fl_scan_batch_get_refs(fl_scan_batch_t* b, int which, const fl_scan_ref_t** refs_device, int* n_max);
+int fl_scan_batch_download(fl_scan_batch_t* b, int which, int slot, float* out_xyzi, int cap);
+
 /* ---- the scan's clouds in a frame: the clouds a FAST-LIO user consumes after map_incremental (laserMapping.cpp:980-982)
  * which (as in fl_scan_download): 0 feats_undistort (de-skewed, or as uploaded), 1 feats_down_body.  Per row, float (x, y, z,
  * intensity), the intensity passed through; the coordinates in FP64 with Eigen's _transformVector order, then rounded to float:
