@@ -897,9 +897,50 @@ __device__ __forceinline__ bool row_current(ulonglong2 v, unsigned tag) { return
 __device__ __forceinline__ double row_value(ulonglong2 v) { return __longlong_as_double((long long)((v.y << 32) | (v.x & 0xffffffffull))); }
 
 }  // namespace fl
+#include "wave_row.cuh"
 #include "wave_search.cuh"
 #include "wave_solver.cuh"
 namespace fl {
+
+// warp_accumulate into the wave row (wave_row.cuh): slot s + 32 j in lane s, register acc[j].  Each slot is warp_accumulate's
+// output for its entry -- the same products of the staged rows summed over the 32 lanes in the same order, effct the ballot's
+// __popc, sum |res| the same butterfly -- so a block's row holds k_update's partial sums.  With extrinsic estimation the row is
+// warp_accumulate's own; without it the 29 slots are one register per lane instead of three, and no hand-off through `stage`.
+template <bool EXTR>
+__device__ __forceinline__ void warp_accumulate_wave(bool contrib, const double* h, double z, float absres,
+                                                     double (&acc)[WaveRow<EXTR>::W / 32], int lane, double* stage) {
+    if constexpr (EXTR) {
+        warp_accumulate<EXTR>(contrib, h, z, absres, acc, lane, stage);
+    } else {
+        constexpr int NC = RowStage<EXTR>::NC, RS = RowStage<EXTR>::RS;
+        constexpr int S_EFFCT = wave_slot<EXTR>(90), S_RES = wave_slot<EXTR>(91);
+        const unsigned any = __ballot_sync(FULL, contrib);
+        if (!any) return;
+#pragma unroll
+        for (int a = 0; a < NC; a++) stage[lane * RS + a] = contrib ? h[a] : 0.0;
+        stage[lane * RS + NC] = contrib ? z : 0.0;
+        __syncwarp();
+        const int o = wave_entry<EXTR>(lane);
+        if (lane < S_EFFCT) {                                 // H^T H and H^T h: (a, b) of entry o, b = NC for H^T h
+            int a = o - 78, b = NC;
+            if (o < 78) {
+                a = 0; int rem = o;
+                while (rem >= 12 - a) { rem -= 12 - a; a++; }
+                b = a + rem;
+            }
+            double v = 0.0;
+#pragma unroll 8
+            for (int i = 0; i < 32; i++) v += stage[i * RS + a] * stage[i * RS + b];
+            acc[0] += v;
+        }
+        if (lane == S_EFFCT) acc[0] += (double)__popc(any);
+        double r = contrib ? (double)absres : 0.0;
+#pragma unroll
+        for (int k = 16; k > 0; k >>= 1) r += __shfl_xor_sync(FULL, r, k);
+        if (lane == S_RES) acc[0] += r;
+        __syncwarp();
+    }
+}
 
 // measure_fused<EXTR, 2> with the point's state in `pt` (slot threadIdx.x % 256) and the search of knn_block_wave; the same
 // outputs in memory
@@ -957,62 +998,72 @@ __device__ __forceinline__ bool measure_wave(const MapView& m, const ScanView& s
     return contrib;
 }
 
-// sol_reduce over tagged rows: warp w takes the rows w, w + 8, ... of pass `tag` GATHER_ROWS at a time, spins until each of them
-// is current (every poll reloads all the stale words of the batch at once: one round trip) and sums them in ascending order from
-// +0.0 (sol_reduce's order; the +0.0 rows it adds past nwork change no sum).  Ends with the warps' sums in S.wred after one
-// barrier: sol_pass_wave adds them up.
-constexpr int GATHER_ROWS = 8;
+// sol_reduce over tagged rows (wave_row.cuh): warp w takes the rows w, w + 8, ... of pass `tag` WaveGather<EXTR>::ROWS at a time,
+// spins until each of them is current (every poll reloads all the stale words of the batch at once: one round trip) and sums them
+// in ascending order from +0.0 (sol_reduce's order; the +0.0 rows it adds past nwork change no sum).  Ends with the warps' sums of
+// each slot in S.wred after one barrier: sol_pass_wave adds them up.  Without extrinsic estimation a row is one ulonglong2 per
+// lane, and 17 rows per warp hold every row of a 132-SM grid in one batch; with it, three per lane and 8 rows.
+template <bool EXTR> struct WaveGather { static constexpr int J = WaveRow<EXTR>::W / 32, ROWS = EXTR ? 8 : 17; };
+template <bool EXTR>
 __device__ void sol_gather(SolverSm& S, FilterCtl* ctl, const unsigned long long* __restrict__ rows, int nwork, unsigned tag) {
+    constexpr int W = WaveRow<EXTR>::W, J = WaveGather<EXTR>::J, ROWS = WaveGather<EXTR>::ROWS;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    double a0 = 0.0, a1 = 0.0, a2 = 0.0;
+    double acc[J];
+#pragma unroll
+    for (int j = 0; j < J; j++) acc[j] = 0.0;
     bool late = false;
     const long long t0 = clock64();
-    for (int b = warp; b < nwork; b += GATHER_ROWS * UPD_WARPS) {
-        const unsigned long long* base = rows + (size_t)b * PSTRIDE * 2 + 2 * lane;
-        ulonglong2 v[GATHER_ROWS][3];
+    for (int b = warp; b < nwork; b += ROWS * UPD_WARPS) {
+        const unsigned long long* base = rows + (size_t)b * W * 2 + 2 * lane;
+        ulonglong2 v[ROWS][J];
 #pragma unroll
-        for (int k = 0; k < GATHER_ROWS; k++) {
+        for (int k = 0; k < ROWS; k++) {
 #pragma unroll
-            for (int j = 0; j < 3; j++) v[k][j] = make_ulonglong2(0ull, 0ull);
+            for (int j = 0; j < J; j++) v[k][j] = make_ulonglong2(0ull, 0ull);
             if (b + k * UPD_WARPS < nwork) {
 #pragma unroll
-                for (int j = 0; j < 3; j++) v[k][j] = row_load(base + (size_t)k * UPD_WARPS * PSTRIDE * 2 + 64 * j);
+                for (int j = 0; j < J; j++) v[k][j] = row_load(base + (size_t)k * UPD_WARPS * W * 2 + 64 * j);
             }
         }
         while (true) {
             bool stale = false;
 #pragma unroll
-            for (int k = 0; k < GATHER_ROWS; k++) {
+            for (int k = 0; k < ROWS; k++) {
 #pragma unroll
-                for (int j = 0; j < 3; j++) stale |= b + k * UPD_WARPS < nwork && !row_current(v[k][j], tag);
+                for (int j = 0; j < J; j++) stale |= b + k * UPD_WARPS < nwork && !row_current(v[k][j], tag);
             }
             if (!stale) break;
             if (clock64() - t0 > SPIN_LIMIT) { late = true; break; }
 #pragma unroll
-            for (int k = 0; k < GATHER_ROWS; k++) {
+            for (int k = 0; k < ROWS; k++) {
 #pragma unroll
-                for (int j = 0; j < 3; j++) {
-                    if (b + k * UPD_WARPS < nwork && !row_current(v[k][j], tag)) v[k][j] = row_load(base + (size_t)k * UPD_WARPS * PSTRIDE * 2 + 64 * j);
+                for (int j = 0; j < J; j++) {
+                    if (b + k * UPD_WARPS < nwork && !row_current(v[k][j], tag)) v[k][j] = row_load(base + (size_t)k * UPD_WARPS * W * 2 + 64 * j);
                 }
             }
         }
 #pragma unroll
-        for (int k = 0; k < GATHER_ROWS; k++) {
-            if (b + k * UPD_WARPS < nwork) { a0 += row_value(v[k][0]); a1 += row_value(v[k][1]); a2 += row_value(v[k][2]); }
+        for (int k = 0; k < ROWS; k++) {
+            if (b + k * UPD_WARPS < nwork) {
+#pragma unroll
+                for (int j = 0; j < J; j++) acc[j] += row_value(v[k][j]);
+            }
         }
         if (late) break;
     }
-    S.wred[warp][lane] = a0; S.wred[warp][lane + 32] = a1; S.wred[warp][lane + 64] = a2;
+#pragma unroll
+    for (int j = 0; j < J; j++) S.wred[warp][lane + 32 * j] = acc[j];
     if (late) S.late = 2;
     sol_sync();
     if (tid == 0) ctl->prof[9] = clock64();
     // warp 0 adds the warps' sums itself and stores S.red (sol_pass_wave); warps 1..3 expand H^T H for the log from the same
-    // sums in the same order
-    if (tid >= 32 && tid < 32 + 78) {
-        const int o = tid - 32;
+    // sums in the same order (the entries no slot carries are +0.0 from update_wave_body's start)
+    constexpr int NPAIR = EXTR ? 78 : 21;
+    if (tid >= 32 && tid < 32 + NPAIR) {
+        const int s = tid - 32, o = wave_entry<EXTR>(s);
         double v = 0.0;
 #pragma unroll
-        for (int w = 0; w < UPD_WARPS; w++) v += S.wred[w][o];
+        for (int w = 0; w < UPD_WARPS; w++) v += S.wred[w][s];
         int a = 0, rem = o;
         while (rem >= 12 - a) { rem -= 12 - a; a++; }
         const int b = a + rem;
@@ -1022,7 +1073,7 @@ __device__ void sol_gather(SolverSm& S, FilterCtl* ctl, const unsigned long long
 }
 
 // update_body<EXTR, 2> for mode 0 with one tile per worker block (gridDim.x - 1 >= the tiles of [q_begin, q1)); rows: the
-// partial rows as tagged words, [worker block][PSTRIDE][2]
+// partial rows as tagged words, [worker block][WaveRow<EXTR>::W][2]
 template <bool EXTR, bool DET = false>
 __device__ __forceinline__ void update_wave_body(const UpdArgs& a, unsigned long long* __restrict__ rows, const int q1) {
     static_assert(sizeof(PairXch) <= sizeof(double) * WorkerSm<EXTR>::STAGE, "the partner's list fits the owner warp's stage slice");
@@ -1091,24 +1142,27 @@ __device__ __forceinline__ void update_wave_body(const UpdArgs& a, unsigned long
                 s.offR.x = x14[X_OFFR]; s.offR.y = x14[X_OFFR + 1]; s.offR.z = x14[X_OFFR + 2]; s.offR.w = x14[X_OFFR + 3];
                 s.offT = d3(x14[X_OFFT], x14[X_OFFT + 1], x14[X_OFFT + 2]);
             }
-            double acc[3] = {0.0, 0.0, 0.0};
+            constexpr int RW = WaveRow<EXTR>::W;
+            double acc[RW / 32];
+#pragma unroll
+            for (int j = 0; j < RW / 32; j++) acc[j] = 0.0;
             double h[12]; double z = 0.0; float ar = 0.f;
             bool contrib = false;
             if (owner || searched)
                 contrib = measure_wave<EXTR, DET>(a.m, a.sc, q, active, s, searched, a.search_only != 0, Wk.walks, walk_phase, stage, pt, h, z, ar);
-            if (owner && !a.search_only) warp_accumulate<EXTR>(contrib, h, z, ar, acc, lane, stage);
+            if (owner && !a.search_only) warp_accumulate_wave<EXTR>(contrib, h, z, ar, acc, lane, stage);
             if (a.search_only) return;
             if (owner) {
 #pragma unroll
-                for (int j = 0; j < 3; j++) Wk.wred[warp][lane + 32 * j] = acc[j];
+                for (int j = 0; j < RW / 32; j++) Wk.wred[warp][lane + 32 * j] = acc[j];
             }
             __syncthreads();
-            if (tid < PSTRIDE) {
+            if (tid < RW) {
                 double v = 0.0;
 #pragma unroll
                 for (int w = 0; w < UPD_WARPS; w++) v += Wk.wred[w][tid];
                 const unsigned long long bits = (unsigned long long)__double_as_longlong(v);
-                unsigned long long* dst = rows + ((size_t)wb * PSTRIDE + tid) * 2;
+                unsigned long long* dst = rows + ((size_t)wb * RW + tid) * 2;
                 const unsigned tag = row_tag(epoch, p);
                 pub_store(dst, tag, (unsigned)bits);
                 pub_store(dst + 1, tag, (unsigned)(bits >> 32));
@@ -1135,12 +1189,15 @@ __device__ __forceinline__ void update_wave_body(const UpdArgs& a, unsigned long
     }
     SolverSm& S = *reinterpret_cast<SolverSm*>(smem_raw);
     sol_load(S, ctl);
+    // the sums and H^T H entries no row slot carries stay +0.0 (wave_row.cuh); sol_prepare's barriers order these stores
+    if (tid < PSTRIDE) S.red[tid] = 0.0;
+    if (tid < 144) S.HTH[tid] = 0.0;
     for (int p = 0; p < a.max_passes && !S.done; p++) {
         if (tid == 0) ctl->prof[0] = clock64();
         if (S.converge && tid < XLEN) ctl->x_search[tid] = S.x[tid];
         sol_prepare(S);
         if (tid == 0) ctl->prof[8] = clock64();
-        sol_gather(S, ctl, rows, nwork, row_tag(epoch, p));
+        sol_gather<EXTR>(S, ctl, rows, nwork, row_tag(epoch, p));
         if (tid == 0) ctl->prof[1] = clock64();
         sol_pass_wave<EXTR>(S, ctl, a.logs, a.pub, pub_tag(a.nonce, p + 1));
         if (tid == 0) ctl->prof[7] = clock64();

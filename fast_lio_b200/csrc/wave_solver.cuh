@@ -3,8 +3,8 @@
 // sol_pass (the library builds with --fmad=false and IEEE division, so a value kept in a register equals the one sol_pass
 // stores and reloads), so the bits are sol_pass's: FASTLIO_B200_PAIR=1 runs k_update<EXTR, 1> with sol_pass, and the tests
 // compare the two byte for byte.  What is shorter, all in warp 0:
-//   * the sums: sol_gather ends after one barrier; warp 0 adds the warps' sums itself (sol_reduce's order, from +0.0), stores
-//     S.red and reads H^T H from it, while warps 1..3 expand S.HTH for the log off the chain;
+//   * the sums: sol_gather ends after one barrier; warp 0 adds the warps' sums of the row slots itself (sol_reduce's order, from
+//     +0.0), stores them at their entries of S.red and reads H^T H from it, while warps 1..3 expand S.HTH for the log off the chain;
 //   * the gain: gj_cols_wave broadcasts the pivot column once per step and every lane picks the pivot itself, so a step has
 //     no shuffle that waits on another; the dx_ factors, dx_new and the limits are loaded before the solve;
 //   * dx_ reaches the pose lanes by shuffles instead of shared memory and a __syncwarp.
@@ -58,12 +58,22 @@ __device__ void sol_pass_wave(SolverSm& S, FilterCtl* ctl, PassLog* logs, unsign
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const double Rinv = 1.0 / S.R;
     if (warp == 0) {
-        // the same sums as sol_gather's S.red: lane l forms red[l], red[l + 32], red[l + 64]
-        double r0 = 0.0, r1 = 0.0, r2 = 0.0;
+        // the same sums as sol_reduce's S.red: lane l forms those of row slots l, l + 32, ... (wave_row.cuh) and stores each at
+        // its entry; the entries no slot carries hold +0.0
+        constexpr int J = WaveRow<EXTR>::W / 32, S_EFFCT = wave_slot<EXTR>(90);
+        double r[J];
 #pragma unroll
-        for (int w = 0; w < UPD_WARPS; w++) { r0 += S.wred[w][lane]; r1 += S.wred[w][lane + 32]; r2 += S.wred[w][lane + 64]; }
-        S.red[lane] = r0; S.red[lane + 32] = r1; S.red[lane + 64] = r2;
-        const int effct = (int)(__shfl_sync(FULL, r2, 90 - 64) + 0.5);
+        for (int j = 0; j < J; j++) r[j] = 0.0;
+#pragma unroll
+        for (int w = 0; w < UPD_WARPS; w++) {
+#pragma unroll
+            for (int j = 0; j < J; j++) r[j] += S.wred[w][lane + 32 * j];
+        }
+#pragma unroll
+        for (int j = 0; j < J; j++) {
+            if (lane + 32 * j < WaveRow<EXTR>::LIVE) S.red[wave_entry<EXTR>(lane + 32 * j)] = r[j];
+        }
+        const int effct = (int)(__shfl_sync(FULL, r[S_EFFCT / 32], S_EFFCT % 32) + 0.5);
         const int late = S.late;
         // known before the solve: u (below), the dx_ factors Pt[lane, :ne] / R, dx_new and the limit of this lane
         const int ln = lane < n ? lane : 0;
