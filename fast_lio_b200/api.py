@@ -142,6 +142,33 @@ def scan_raws(entries, device=None):
     return torch.tensor(rows, dtype=torch.int64).reshape(-1, 6).to(device)
 
 
+class PreprocessRaw(C.Structure):
+    """fl_preprocess_raw_t: one slot's raw frame for fl_preprocess_batch_run_device, both pointers in device memory"""
+    _fields_ = [("raw", C.c_void_p), ("n_raw", C.c_void_p)]
+
+
+def preprocess_raws(entries, device=None):
+    """The device table of fl_preprocess_batch_run_device: an (S, 2) int64 CUDA tensor of fl_preprocess_raw_t rows.  Each entry
+    is a (raw, n_raw) pair: raw a contiguous uint8 CUDA tensor of the frame's points (point_step bytes each), n_raw a one-element
+    int32 CUDA tensor, or either one a raw device address (an int, 0 or None for null).  The table is copied from the host, so
+    build it outside stream capture; what it points at must stay alive until the stream has passed the calls that read it."""
+    import torch
+    rows = []
+    for raw, n in entries:
+        row = []
+        for v, name, dt in ((raw, "raw", torch.uint8), (n, "n_raw", torch.int32)):
+            if isinstance(v, torch.Tensor):
+                if not v.is_cuda or not v.is_contiguous() or v.dtype != dt:
+                    raise ValueError(f"preprocess_raws: {name} must be a contiguous {dt} CUDA tensor")
+                row.append(v.data_ptr())
+            else:
+                row.append(int(v or 0))
+        rows.append(row)
+    if device is None:
+        device = torch.device("cuda", torch.cuda.current_device())
+    return torch.tensor(rows, dtype=torch.int64).reshape(-1, 2).to(device)
+
+
 class FastLioError(RuntimeError):
     pass
 
@@ -215,6 +242,8 @@ SYMBOLS = [
     "fl_scan_get_ref", "fl_filter_update_scans_device",
     "fl_scan_batch_create", "fl_scan_batch_destroy", "fl_scan_batch_reserve", "fl_scan_batch_run_device", "fl_scan_batch_get_refs",
     "fl_scan_batch_download",
+    "fl_preprocess_batch_create", "fl_preprocess_batch_destroy", "fl_preprocess_batch_run_device", "fl_preprocess_batch_get_outputs",
+    "fl_preprocess_batch_download",
 ]
 
 
@@ -329,6 +358,12 @@ def load():
     L.fl_preprocess_destroy.argtypes = [_vp]
     L.fl_preprocess_device.argtypes = [_vp, _vp, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp]
     L.fl_preprocess.argtypes = [_vp, _vp, C.c_int, _f32p, _f32p, C.c_int, C.POINTER(C.c_float)]
+    L.fl_preprocess_batch_create.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.POINTER(PreprocessParams), C.c_int, C.c_int]
+    L.fl_preprocess_batch_destroy.argtypes = [_vp]
+    L.fl_preprocess_batch_run_device.argtypes = [_vp, _vp, C.c_int, C.c_int, _vp, _vp]
+    _pp = C.POINTER(C.c_void_p)
+    L.fl_preprocess_batch_get_outputs.argtypes = [_vp, _pp, _pp, _pp, _pp, C.POINTER(C.c_int)]
+    L.fl_preprocess_batch_download.argtypes = [_vp, C.c_int, _f32p, _f32p, C.c_int, C.POINTER(C.c_float)]
     L.fl_comm_unique_id.argtypes = [C.c_char_p]
     L.fl_filter_comm_init.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_char_p]
     L.fl_filter_set_shard.argtypes = [C.c_void_p, C.c_int, C.c_int]
@@ -1054,11 +1089,13 @@ class Scan:
 
 
 class _DeviceTable:
-    """A view of device memory the batch owns, for torch.as_tensor (the __cuda_array_interface__ protocol); holds the batch."""
+    """A view of device memory the batch owns, for torch.as_tensor (the __cuda_array_interface__ protocol); holds the batch.
+    Default: `rows` fl_scan_ref_t entries as (rows, 2) int64."""
 
-    def __init__(self, owner, ptr: int, rows: int):
+    def __init__(self, owner, ptr: int, rows: int, shape: tuple | None = None, typestr: str = "<i8"):
         self.owner = owner
-        self.__cuda_array_interface__ = {"shape": (rows, 2), "typestr": "<i8", "data": (ptr, False), "version": 2}
+        self.__cuda_array_interface__ = {"shape": (rows, 2) if shape is None else shape, "typestr": typestr, "data": (ptr, False),
+                                         "version": 2}
 
 
 class ScanBatch:
@@ -1259,6 +1296,90 @@ class Preprocess:
                                             xyzi.data_ptr() if n_max else None, offset_ms.data_ptr() if n_max else None,
                                             out2.data_ptr(), last_ms.data_ptr(), stream))
         return xyzi, offset_ms, out2, last_ms
+
+
+class PreprocessBatch:
+    """Preprocess::process of many raw frames in one call (fl_preprocess_batch_run_device): every slot a frame of one LiDAR type and
+    layout (the arguments of `Preprocess`), each slot's pl_surf equal to Preprocess.process_device's on the same frame.  The
+    outputs live in the handle, n_slots_max slots of n_raw_max rows at addresses fixed at creation (outputs())."""
+
+    def __init__(self, device: int, lidar_type: int, n_scans: int, scan_rate: int = 10, time_unit: int = TIME_US,
+                 point_filter_num: int = 1, blind: float = 0.01, layout: np.dtype | None = None, n_slots_max: int = 1,
+                 n_raw_max: int = 65536):
+        self._L = load()
+        self.device = device
+        self.layout = np.dtype(DEFAULT_LAYOUT[lidar_type] if layout is None else layout)
+        self.n_slots_max, self.n_raw_max = n_slots_max, n_raw_max
+        off = layout_offsets(self.layout, lidar_type)
+        p = PreprocessParams(lidar_type, n_scans, scan_rate, time_unit, point_filter_num, blind, self.layout.itemsize, *off)
+        h = C.c_void_p()
+        _check(self._L.fl_preprocess_batch_create(C.byref(h), device, C.byref(p), n_slots_max, n_raw_max))
+        self.h = h
+
+    def close(self):
+        if getattr(self, "h", None):
+            self._L.fl_preprocess_batch_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def run_device(self, raws, n_slots: int, n_max: int, status=None):
+        """fl_preprocess_batch_run_device on torch.cuda.current_stream(): raws the (>= n_slots, 2) int64 table of
+        preprocess_raws.  Returns status, an (n_slots, 2) int32 tensor = (FL_OK, |pl_surf|) or (refusal, 0) per slot."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        if not isinstance(raws, torch.Tensor) or raws.dtype != torch.int64 or raws.dim() != 2 or raws.shape[1] != 2 \
+                or not raws.is_contiguous() or raws.device != dev or raws.shape[0] < n_slots:
+            raise TypeError(f"raws must be the contiguous (S, 2) int64 tensor of preprocess_raws on {dev}, S >= n_slots")
+        if status is None:
+            status = torch.empty((max(n_slots, 0), 2), dtype=torch.int32, device=dev)
+        if not isinstance(status, torch.Tensor) or status.dtype != torch.int32 or not status.is_contiguous() or status.device != dev \
+                or status.numel() < 2 * max(n_slots, 0):
+            raise TypeError(f"status must be a contiguous int32 tensor of (n_slots, 2) on {dev}")
+        stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        _check(self._L.fl_preprocess_batch_run_device(self.h, raws.data_ptr() if n_slots > 0 else None, n_slots, n_max,
+                                                      status.data_ptr() if n_slots > 0 else None, stream))
+        return status
+
+    def outputs(self):
+        """fl_preprocess_batch_get_outputs as CUDA tensors over the handle's memory: xyzi (n_slots_max, n_raw_max, 4) float32,
+        offset_ms (n_slots_max, n_raw_max) float32, out2 (n_slots_max, 2) int32 and last_ms (n_slots_max,) float32."""
+        import torch
+        ptrs = [C.c_void_p() for _ in range(4)]
+        m = C.c_int(0)
+        _check(self._L.fl_preprocess_batch_get_outputs(self.h, *[C.byref(p) for p in ptrs], C.byref(m)))
+        S, m = self.n_slots_max, int(m.value)
+        views = [((S, m, 4), "<f4"), ((S, m), "<f4"), ((S, 2), "<i4"), ((S,), "<f4")]
+        return tuple(torch.as_tensor(_DeviceTable(self, int(p.value or 0), S, shape, ts), device=f"cuda:{self.device}")
+                     for p, (shape, ts) in zip(ptrs, views))
+
+    def download(self, slot: int):
+        """fl_preprocess_batch_download: slot `slot`'s pl_surf of the last call as (xyzi (m, 4) float32, offset_ms (m,) float32,
+        last_ms); a refused or uncovered slot has no rows."""
+        last = C.c_float(0.0)
+        one4, one = np.zeros((1, 4), np.float32), np.zeros(1, np.float32)
+        n = _check(self._L.fl_preprocess_batch_download(self.h, slot, one4, one, 0, C.byref(last)))
+        xyzi, ms = np.zeros((max(n, 1), 4), np.float32), np.zeros(max(n, 1), np.float32)
+        _check(self._L.fl_preprocess_batch_download(self.h, slot, xyzi, ms, n, C.byref(last)))
+        return xyzi[:n].copy(), ms[:n].copy(), last.value
+
+    def scan_raws(self, poses=None, n_pose=None, x_end=None, n_slots: int | None = None):
+        """The fl_scan_raw_t table of ScanBatch.run_device over this handle's outputs, slot s reading xyzi[s], offset_ms[s] and
+        the count out2[s, 0] in place: poses an (S, n_pose_max, 22) float64, n_pose an (S,) int32 and x_end an (S, 26) float64
+        CUDA tensor (each may be None when not de-skewing).  S is their first dimension, else n_slots, else n_slots_max."""
+        xyzi, ms, out2, _ = self.outputs()
+        S = next((t.shape[0] for t in (poses, n_pose, x_end) if t is not None), self.n_slots_max if n_slots is None else n_slots)
+        if S > self.n_slots_max:
+            raise ValueError(f"{S} slots, the handle has {self.n_slots_max}")
+        entries = []
+        for s in range(S):
+            entries.append((xyzi[s], ms[s], out2[s, :1], None if poses is None else poses[s], None if n_pose is None else n_pose[s:s + 1],
+                            None if x_end is None else x_end[s]))
+        return scan_raws(entries, device=xyzi.device)
 
 
 def reloc_grid_device(x_prior, n, step):

@@ -683,16 +683,15 @@ struct fl_preprocessor {
     std::mutex mu;
 };
 
-int fl_preprocess_create(fl_preprocess_t** out, int device, const fl_preprocess_params_t* pp, int n_raw_max) {
-    if (!out) return FL_ERR_ARG;
-    *out = nullptr;
-    if (!pp) { fl::set_last_error("fl_preprocess_create: null parameters"); return FL_ERR_ARG; }
+// fl_preprocess_params_t -> PpParams, with the checks of fl_preprocess_create (and of its batched form); `who` names the caller
+static int pp_params(const char* who, int device, const fl_preprocess_params_t* pp, int n_raw_max, fl::PpParams* out) {
+    if (!pp) { fl::set_last_error("%s: null parameters", who); return FL_ERR_ARG; }
     const fl_preprocess_params_t& p = *pp;
     if (p.lidar_type < FL_LIDAR_AVIA || p.lidar_type > FL_LIDAR_MARSIM || p.time_unit < 0 || p.time_unit > 3 || p.n_scans < 1 ||
         p.n_scans > 128 || p.point_filter_num < 1 || p.point_step < 1 || n_raw_max < 0 ||
         (p.lidar_type == FL_LIDAR_VELO16 && p.scan_rate < 1)) {
-        fl::set_last_error("fl_preprocess_create: bad lidar_type %d, time_unit %d, n_scans %d, scan_rate %d, point_filter_num %d, "
-                           "point_step %d or n_raw_max %d", p.lidar_type, p.time_unit, p.n_scans, p.scan_rate, p.point_filter_num,
+        fl::set_last_error("%s: bad lidar_type %d, time_unit %d, n_scans %d, scan_rate %d, point_filter_num %d, "
+                           "point_step %d or n_raw_max %d", who, p.lidar_type, p.time_unit, p.n_scans, p.scan_rate, p.point_filter_num,
                            p.point_step, n_raw_max);
         return FL_ERR_ARG;
     }
@@ -709,7 +708,7 @@ int fl_preprocess_create(fl_preprocess_t** out, int device, const fl_preprocess_
     for (int k = 0; k < 8; k++) {
         q.off[k] = size[k] ? offs[k] : -1;
         if (size[k] && (offs[k] < -1 || (offs[k] >= 0 && offs[k] + size[k] > p.point_step))) {
-            fl::set_last_error("fl_preprocess_create: field %d at offset %d does not fit point_step %d", k, offs[k], p.point_step);
+            fl::set_last_error("%s: field %d at offset %d does not fit point_step %d", who, k, offs[k], p.point_step);
             return FL_ERR_ARG;
         }
     }
@@ -722,9 +721,18 @@ int fl_preprocess_create(fl_preprocess_t** out, int device, const fl_preprocess_
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) {
         cudaGetLastError();
-        fl::set_last_error("fl_preprocess_create: no CUDA device %d", device);
+        fl::set_last_error("%s: no CUDA device %d", who, device);
         return FL_ERR_ARG;
     }
+    *out = q;
+    return FL_OK;
+}
+
+int fl_preprocess_create(fl_preprocess_t** out, int device, const fl_preprocess_params_t* pp, int n_raw_max) {
+    if (!out) return FL_ERR_ARG;
+    *out = nullptr;
+    fl::PpParams q{};
+    FL_CHECK(pp_params("fl_preprocess_create", device, pp, n_raw_max, &q));
     fl_preprocess_t* h = new (std::nothrow) fl_preprocess_t();
     if (!h) return FL_ERR_CAPACITY;
     h->impl = new (std::nothrow) fl::Preprocessor(device, q, n_raw_max);
@@ -751,6 +759,57 @@ int fl_preprocess(fl_preprocess_t* h, const void* raw_host, int n_raw, float* xy
     if (!h || !h->impl) { fl::set_last_error("null preprocess handle"); return FL_ERR_ARG; }
     std::lock_guard<std::mutex> lk(h->mu);
     return h->impl->run_host(raw_host, n_raw, xyzi_out, offset_ms_out, cap, last_ms);
+}
+// ------------------------------------------------------------------------------------ preprocessing of many frames
+static_assert(sizeof(fl_preprocess_raw_t) == 16, "fl_preprocess_raw_t is two device pointers");
+struct fl_preprocess_batch {
+    fl::PreprocessBatch* impl;
+    std::mutex mu;
+};
+int fl_preprocess_batch_create(fl_preprocess_batch_t** out, int device, const fl_preprocess_params_t* pp, int n_slots_max, int n_raw_max) {
+    if (!out) return FL_ERR_ARG;
+    *out = nullptr;
+    fl::PpParams q{};
+    FL_CHECK(pp_params("fl_preprocess_batch_create", device, pp, n_raw_max, &q));
+    if (n_slots_max < 0) { fl::set_last_error("fl_preprocess_batch_create: n_slots_max %d < 0", n_slots_max); return FL_ERR_ARG; }
+    if (n_slots_max > fl::PreprocessBatch::SLOTS_MAX || (long long)n_slots_max * n_raw_max > (long long)INT_MAX) {
+        fl::set_last_error("fl_preprocess_batch_create: %d slots (at most %d) or %lld rows (at most INT_MAX)", n_slots_max,
+                           fl::PreprocessBatch::SLOTS_MAX, (long long)n_slots_max * n_raw_max);
+        return FL_ERR_CAPACITY;
+    }
+    fl_preprocess_batch_t* b = new (std::nothrow) fl_preprocess_batch_t();
+    if (!b) return FL_ERR_CAPACITY;
+    b->impl = new (std::nothrow) fl::PreprocessBatch(device, q, n_slots_max, n_raw_max);
+    if (!b->impl) { delete b; return FL_ERR_CAPACITY; }
+    const int rc = b->impl->init();
+    if (rc != FL_OK) { delete b->impl; delete b; return rc; }
+    *out = b;
+    return FL_OK;
+}
+int fl_preprocess_batch_destroy(fl_preprocess_batch_t* b) {
+    if (!b) return FL_OK;
+    delete b->impl;
+    delete b;
+    return FL_OK;
+}
+#define PP_BATCH_GUARD(b)                                                                              \
+    if (!(b) || !(b)->impl) { fl::set_last_error("null preprocess batch handle"); return FL_ERR_ARG; } \
+    std::lock_guard<std::mutex> _lk((b)->mu)
+int fl_preprocess_batch_run_device(fl_preprocess_batch_t* b, const fl_preprocess_raw_t* raws_device, int n_slots, int n_max,
+                                   int* status2_device, void* stream) {
+    PP_BATCH_GUARD(b);
+    return b->impl->run_device(raws_device, n_slots, n_max, status2_device, static_cast<cudaStream_t>(stream));
+}
+int fl_preprocess_batch_get_outputs(fl_preprocess_batch_t* b, float** xyzi, float** offset_ms, int** out2, float** last_ms, int* n_raw_max) {
+    PP_BATCH_GUARD(b);
+    b->impl->outputs(xyzi, offset_ms, out2, last_ms, n_raw_max);
+    return FL_OK;
+}
+int fl_preprocess_batch_download(fl_preprocess_batch_t* b, int slot, float* out_xyzi, float* out_offset_ms, int cap, float* last_ms) {
+    PP_BATCH_GUARD(b);
+    int n = 0;
+    const int rc = b->impl->download(slot, out_xyzi, out_offset_ms, cap, last_ms, &n);
+    return rc == FL_OK ? n : rc;
 }
 
 // ------------------------------------------------------------------------------------ multi-GPU

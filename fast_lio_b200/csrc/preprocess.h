@@ -42,4 +42,31 @@ private:
     DeviceBuffer d_raw_, d_n_, d_xyzi_, d_ms_, d_out_;
 };
 
+// Preprocess::process of many frames in one call (fl_preprocess_batch_run_device): slot s owns rows [s n_max, (s + 1) n_max) of
+// the packed scratch and rows [s n_raw_max, (s + 1) n_raw_max) of the outputs; each of Preprocessor's steps runs per slot on grids
+// of (row blocks, slots), and each cub call runs once over every slot's rows.  Everything is sized at creation.
+class PreprocessBatch {
+public:
+    static constexpr int SLOTS_MAX = 65535;         // the grids' y dimension
+    PreprocessBatch(int device, const PpParams& p, int n_slots_max, int n_raw_max)
+        : dev_(device), p_(p), slots_max_(n_slots_max), n_raw_max_(n_raw_max) {}
+    ~PreprocessBatch();
+    int init();
+    int run_device(const fl_preprocess_raw_t* d_raws, int n_slots, int n_max, int* d_status2, cudaStream_t st);
+    void outputs(float** xyzi, float** ms, int** out2, float** last, int* n_raw_max) const;
+    int download(int slot, float* xyzi, float* ms, int cap, float* last, int* n);
+
+private:
+    size_t cub_bytes(int rows) const;
+    int dev_;
+    PpParams p_;
+    int slots_max_, n_raw_max_, sort_bits_ = 0;     // sort_bits_: the Velodyne ring sort's, key_bits + the bits of n_slots_max
+    cudaStream_t stream_ = nullptr;                 // download's
+    cudaEvent_t ev_ = nullptr;                      // the last call outside capture; download waits for it
+    // per packed row: the flags, positions, times and the Velodyne sort's keys, values, yaws and maps; per slot its PbSlot
+    // (preprocess.cu) and yaw_fp [slot][ring]
+    DeviceBuffer keep_, pos_, tm_, valid_, keys_, keys_alt_, vals_, vals_alt_, yaw_, tri_, tri_alt_, yaw_fp_, slots_, cub_;
+    DeviceBuffer xyzi_, ms_, out2_, last_;          // the outputs
+};
+
 }  // namespace fl

@@ -907,7 +907,8 @@ int ScanBatch::run_on_stream(const fl_scan_raw_t* d_raws, int n_scans, int n_max
         return FL_ERR_CAPACITY;
     }
     if (n_scans == 0) return FL_OK;
-    const int rows = n_scans * n_max, end_bit = 32 + slot_bits(n_scans);
+    // the sorts' bits follow the reserved slot count, not n_scans, so cub's passes (and launches) are the same for every n_scans
+    const int rows = n_scans * n_max, end_bit = 32 + slot_bits(res_slots_);
     size_t need = 0;
     FL_CHECK(cub_bytes(rows, end_bit, &need));
     if (need > cub_.bytes) { set_last_error("scan batch run_device: %d rows exceed what fl_scan_batch_reserve sized", rows); return FL_ERR_CAPACITY; }

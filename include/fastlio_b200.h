@@ -537,7 +537,8 @@ int fl_filter_update_scans_device(fl_filter_t* f, const fl_scan_ref_t* scans_dev
  * *n_pose, clamped to [0, n_pose_max], is >= 2 (a null n_pose is no pose) -- each (FL_ERR_ARG, 0); c > n_max (FL_ERR_CAPACITY, 0).
  * Its counts in both ref tables are -1, which fl_filter_update_scans_device refuses with (FL_ERR_ARG, 0); no other slot depends
  * on it.  The inputs are copied on `stream`: the caller may reuse them once `stream` has passed the call.  Slots may share or
- * overlap their inputs, and may point at fl_preprocess_device outputs (n = &out2_device[0]).
+ * overlap their inputs, and may point at fl_preprocess_device outputs (n = &out2_device[0]) or at the slots of a
+ * fl_preprocess_batch_t's outputs (below).
  * The outputs live in the handle: per slot a region of n_max rows and a count.  fl_scan_batch_get_refs gives the device table of
  * n_scans_max fl_scan_ref_t for `which` (0 or 1), to hand straight to fl_filter_update_scans_device(f, refs, n_scans, *n_max, ...);
  * slots the last call did not cover have the count -1.  The table's address stays valid until a reserve that grows the handle
@@ -675,6 +676,46 @@ int fl_preprocess_device(fl_preprocess_t* h, const void* raw_device, const int* 
 /* The host form: the same launches on the handle's own stream, after the handle's last device-form call outside capture.
  * Writes min(|pl_surf|, cap) rows, *last_ms (may be NULL) as above; returns |pl_surf| (>= 0) or an error (< 0). */
 int fl_preprocess(fl_preprocess_t* h, const void* raw_host, int n_raw, float* xyzi_out, float* offset_ms_out, int cap, float* last_ms);
+
+/* ---- batched preprocessing: Preprocess::process of many raw frames in one call (a fleet's driver points in, every robot's
+ * pl_surf out, ready for fl_scan_batch_run_device)
+ * One parameter set per handle: every slot is a frame of the handle's LiDAR type and layout (a mixed fleet makes one handle and
+ * one call per sensor model).  fl_preprocess_batch_create validates params as fl_preprocess_create does; it sizes everything
+ * once for n_slots_max frames of up to n_raw_max points.  FL_ERR_CAPACITY when n_slots_max is above 65535 or n_slots_max x
+ * n_raw_max above INT_MAX; FL_ERR_ARG for bad parameters or a negative size.
+ * raws_device is a device table of n_slots fl_preprocess_raw_t.  For slot s the count c = *raws_device[s].n_raw is read when
+ * `stream` reaches the call.  If 0 <= c <= n_max and the slot's pointers are valid, the slot's rows [0, |pl_surf|) of xyzi and
+ * offset_ms, out2[s] = (|pl_surf|, dropped rings) and last_ms[s] equal, byte for byte, what fl_preprocess_device writes for the
+ * same frame with the device count c; status2_device[s] = (FL_OK, |pl_surf|).  A refused slot: a null or misaligned (4-byte)
+ * n_raw, c < 0, or a null raw with c > 0 -- (FL_ERR_ARG, 0); c > n_max -- (FL_ERR_CAPACITY, 0) (where fl_preprocess_device
+ * clamps: a count above the bound means the caller's buffer overflowed).  It writes no row, gets out2[s] = (-1, 0) and
+ * last_ms[s] = 0, so fl_scan_batch_run_device (c < 0) and then fl_filter_update_scans_device refuse it too; no other slot
+ * depends on it.  Slots [n_slots, n_slots_max) get out2 = (-1, 0) and last_ms = 0.  Slots may share or overlap their raw
+ * buffers; the inputs may be reused once `stream` has passed the call.
+ * The outputs live in the handle, at addresses fixed at creation (fl_preprocess_batch_get_outputs, any pointer may be NULL):
+ * xyzi [n_slots_max][n_raw_max][4], offset_ms [n_slots_max][n_raw_max], out2 [n_slots_max][2], last_ms [n_slots_max]; the slot
+ * stride is the handle's n_raw_max, not the call's n_max, so a fl_scan_raw_t table over them (xyzi + s n_raw_max 4, offset_ms +
+ * s n_raw_max, n = out2 + 2 s) is built once and read in place by fl_scan_batch_run_device.  fl_preprocess_batch_download
+ * copies slot `slot`'s rows of the last call into host memory (synchronous, at most cap rows; last_ms may be NULL), after the
+ * handle's last call outside capture (synchronise graph replays first), and returns the slot's |pl_surf|, 0 for a refused slot.
+ * No host synchronisation, no allocation, no launch sized from a device value, and the number of launches does not depend on
+ * n_slots (the ring sort's bits are fixed by n_slots_max), so the call can be captured into a CUDA graph.  n_slots = 0 returns
+ * FL_OK and enqueues nothing.  Refusals enqueue nothing, also on a capturing stream.  FL_ERR_ARG: n_slots or n_max < 0; a host,
+ * wrong-device, null or misaligned table (8-byte) or status2 (4-byte).  FL_ERR_CAPACITY: n_slots above n_slots_max, n_max above
+ * n_raw_max.  Calls on one handle share its workspace: enqueue them in one stream order. */
+typedef struct fl_preprocess_raw {
+    const void* raw;            /* device: the driver's points, point_step bytes each, no alignment required */
+    const int* n_raw;           /* device: the row count, read when the stream reaches the call */
+} fl_preprocess_raw_t;          /* 16 bytes */
+typedef struct fl_preprocess_batch fl_preprocess_batch_t;
+int fl_preprocess_batch_create(fl_preprocess_batch_t** out, int device, const fl_preprocess_params_t* params, int n_slots_max,
+                               int n_raw_max);
+int fl_preprocess_batch_destroy(fl_preprocess_batch_t* b);
+int fl_preprocess_batch_run_device(fl_preprocess_batch_t* b, const fl_preprocess_raw_t* raws_device, int n_slots, int n_max,
+                                   int* status2_device, void* stream);
+int fl_preprocess_batch_get_outputs(fl_preprocess_batch_t* b, float** xyzi, float** offset_ms, int** out2, float** last_ms,
+                                    int* n_raw_max);
+int fl_preprocess_batch_download(fl_preprocess_batch_t* b, int slot, float* out_xyzi, float* out_offset_ms, int cap, float* last_ms);
 
 /* ------------------------------------------------------------------ multi-GPU (no reference counterpart)
  * scan points are sharded across ranks, the map is replicated, the 92 normal-equation doubles
