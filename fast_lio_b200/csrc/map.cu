@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "map.h"
+#include "map_rules.h"
 
 namespace fl {
 
@@ -564,14 +565,14 @@ __global__ void k_delete_plan(int* counters, const int* __restrict__ nb_dev, int
     counters[C_DEL_SKIP] = !ok;
     counters[C_DELETED] = 0;
 }
-// after the delete: the host form's bookkeeping (delete_boxes) and its maybe_rebuild, which here only marks maintenance as due
+// after the delete: the host form's bookkeeping (delete_boxes), and repack_due (map_rules.h), which maybe_rebuild acts on and
+// which here only marks maintenance as due
 __global__ void k_delete_account(MapView m, int* counters, int chain_limit) {
     const int d = counters[C_DELETED];
     if (d == 0) return;
     counters[C_VALID] -= d;
     counters[C_TOMBS] += d;
-    const int tombs = counters[C_TOMBS];
-    if ((tombs > 1024 && tombs > counters[C_VALID]) || counters[C_LEAF_USED] - m.n_main > chain_limit) counters[C_DUE] = 1;
+    if (repack_due(counters[C_LEAF_USED], m.n_main, chain_limit, counters[C_TOMBS], counters[C_VALID])) counters[C_DUE] = 1;
 }
 // status2 = (status, deleted)
 __global__ void k_delete_status(const int* __restrict__ counters, int* __restrict__ out) {
@@ -929,13 +930,12 @@ __global__ void __launch_bounds__(256) k_plan_reset(MapView m, const float4* __r
     }
 }
 // The host form's guards before an insert, for the whole call at once, in terms of the batch size (nothing is tombstoned yet):
-// overflow leaves for one fresh leaf per point, the table below 90 % load, the list pool for the counted need.  The fix list is
-// sized for 27 entries per point and cannot overflow.
+// batch_fits (map_rules.h: overflow leaves and table load), and the list pool for the counted need.  The fix list is sized for
+// 27 entries per point and cannot overflow.
 __global__ void k_plan(MapView m, int* counters) {
     const long long n = (long long)counters[C_RA] + counters[C_RB];
-    bool ok = counters[C_LEAF_USED] + n <= m.leaf_cap;
+    bool ok = batch_fits(counters[C_LEAF_USED], m.leaf_cap, counters[C_DIR_CELLS], m.dir.cap, n);
     if (m.dir.cap) {
-        ok = ok && ((long long)counters[C_DIR_CELLS] + 27 * n) * 10 <= (long long)m.dir.cap * 9;
         const long long miss = counters[C_MISS];
         // fresh cells: a fresh list of HALO_NEW_CAP each, and a new list for each (per insert) that more than HALO_NEW_CAP pairs hit
         const long long need = miss * HALO_NEW_CAP + 16ll * counters[C_FIXES] + 2 * (miss / (HALO_NEW_CAP + 1)) * HALO_FIX_MAX;
@@ -949,7 +949,7 @@ __global__ void k_plan(MapView m, int* counters) {
     counters[C_ADDED] = counters[C_GROUPS] = counters[C_NINSERT] = counters[C_TOMB] = 0;
 }
 // After one Add_Points of the call: the host form's bookkeeping of n_valid_ / n_tomb_ (add_points_host) and its decisions after
-// the insert (insert_device's re-list of a full or crowded directory, maybe_rebuild), which here only mark maintenance as due.
+// the insert, relist_due and repack_due (map_rules.h), which here only mark maintenance as due.
 __global__ void k_async_account(MapView m, int* counters, int slot, bool downsample_on, int chain_limit) {
     const int batch = counters[slot];
     if (batch == 0) return;
@@ -962,10 +962,9 @@ __global__ void k_async_account(MapView m, int* counters, int slot, bool downsam
     }
     counters[C_VALID] += inserted;
     bool due = false;
-    if (inserted > 0 && m.dir.cap) due = counters[C_DIR_ERROR] || counters[C_DIR_CROWDED] > max(64, counters[C_DIR_CELLS] / 1024);
+    if (inserted > 0 && m.dir.cap) due = relist_due(counters[C_DIR_ERROR], counters[C_DIR_CROWDED], counters[C_DIR_CELLS]);
     if (downsample_on) counters[C_TOMBS] = max(0, counters[C_TOMBS] - inserted);
-    const int tombs = counters[C_TOMBS];
-    due = due || counters[C_LEAF_USED] - m.n_main > chain_limit || (tombs > 1024 && tombs > counters[C_VALID]) || counters[C_ERROR];
+    due = due || repack_due(counters[C_LEAF_USED], m.n_main, chain_limit, counters[C_TOMBS], counters[C_VALID]) || counters[C_ERROR];
     if (due) counters[C_DUE] = 1;
 }
 // status2 = (status, added), or out4 = (list_counts[0], list_counts[1], added, status)
@@ -1388,7 +1387,7 @@ int Map::build_directory() {
         FL_CUDA(cudaGetLastError());
         FL_CUDA(cudaMemcpyAsync(&h_counters_[C_DIR_CELLS], &d_cnt[C_DIR_CELLS], sizeof(int) * 4, cudaMemcpyDeviceToHost, stream_));
         FL_CUDA(cudaStreamSynchronize(stream_));
-        if (h_counters_[C_DIR_ERROR]) { dir_min_pool_ = std::max<size_t>(dir_min_pool_ * 2, (size_t)HALO_NEW_CAP * 262144); continue; }
+        if (h_counters_[C_DIR_ERROR]) { dir_min_pool_ = list_pool_min_grown(dir_min_pool_, (size_t)HALO_NEW_CAP * 262144); continue; }
         layout_dirty_ = true;
         if (async_used_) {          // the plan's per-entry counters (k_plan_count): one int per table entry, all zero
             FL_CHECK(cellcnt_.reserve(sizeof(int) * (size_t)v_.dir.cap));
@@ -1522,12 +1521,11 @@ int Map::removed_cap() const { return (int)std::min<size_t>(removed_.bytes / siz
 // point went away.  Every grid is fixed on the host: the same launches whether or not anything is deleted.
 int Map::enqueue_delete(const float* boxes, const int* nb_dev, int nb_max, int* status2, cudaStream_t st) {
     int* d_cnt = counters_.as<int>();
-    const int chain_limit = std::max(64, (int)(rebuild_overflow_frac_ * v_.n_main));
     k_delete_plan<<<1, 1, 0, st>>>(d_cnt, nb_dev, nb_max, record_removed_, removed_cap());
     const int g = resident_blocks(k_delete_boxes, 256, (long long)v_.leaf_cap * LEAF, n_sm_);
     k_delete_boxes<<<g, 256, 0, st>>>(v_, boxes, nb_max, 0, d_cnt, record_removed_ ? removed_.as<float4>() : nullptr, removed_cap(),
                                       &d_cnt[C_DEL_NB], &d_cnt[C_LEAF_USED]);
-    k_delete_account<<<1, 1, 0, st>>>(v_, d_cnt, chain_limit);
+    k_delete_account<<<1, 1, 0, st>>>(v_, d_cnt, chain_limit(rebuild_overflow_frac_, v_.n_main));
     FL_CHECK(refit_on(st, &d_cnt[C_DELETED]));          // tighten every AABB, when something was deleted
     k_delete_status<<<1, 1, 0, st>>>(d_cnt, status2);
     FL_CUDA(cudaGetLastError());
@@ -1926,30 +1924,42 @@ int Map::rebuild() {
 }
 
 int Map::maybe_rebuild() {
-    const int overflow = h_counters_[C_LEAF_USED] - v_.n_main;
-    const bool too_chained = overflow > std::max(64, (int)(rebuild_overflow_frac_ * v_.n_main));
-    const bool too_sparse = n_tomb_ > 1024 && n_tomb_ > n_valid_;       // ikd-Tree's delete criterion (alpha_del = 0.5)
-    if (too_chained || too_sparse) return rebuild();
+    if (repack_due(h_counters_[C_LEAF_USED], v_.n_main, chain_limit(rebuild_overflow_frac_, v_.n_main), n_tomb_, n_valid_)) return rebuild();
     return FL_OK;
+}
+
+int Map::grow_for_batch(long long n, bool list_pool) {
+    if (!leaves_fit(h_counters_[C_LEAF_USED], v_.leaf_cap, n)) {
+        min_pool_ = pool_min_for_batch(min_pool_, n);
+        FL_CHECK(rebuild());            // re-packs the leaves and re-sizes the pool
+    }
+    if (v_.dir.cap) {
+        const bool grow_cap = !table_fits(h_counters_[C_DIR_CELLS], v_.dir.cap, n);
+        const long long need = std::max<long long>(h_counters_[C_NEED], 0);
+        const bool grow_pool = list_pool && (long long)h_counters_[C_DIR_POOL] + need > v_.dir.lists_cap;
+        if (grow_cap) dir_min_cap_ = dir_cap_min_for_batch(dir_min_cap_, h_counters_[C_DIR_CELLS], n);
+        if (grow_pool) dir_min_pool_ = list_pool_min_grown(dir_min_pool_, 2 * (size_t)need);
+        if (grow_cap || grow_pool) { n_dir_rebuilds_++; FL_CHECK(build_directory()); }
+    }
+    return FL_OK;
+}
+
+int Map::relist_if_due() {
+    if (!v_.dir.cap) return FL_OK;
+    if (h_counters_[C_DIR_ERROR]) {
+        dir_min_cap_ = dir_cap_min_after_error(dir_min_cap_, v_.dir.cap);
+        dir_min_pool_ = list_pool_min_grown(dir_min_pool_, (size_t)HALO_NEW_CAP * 262144);
+    }
+    if (!relist_due(h_counters_[C_DIR_ERROR], h_counters_[C_DIR_CROWDED], h_counters_[C_DIR_CELLS])) return FL_OK;
+    n_dir_rebuilds_++;
+    return build_directory();
 }
 
 int Map::insert_device(const float4* d_pts, int n) {
     if (n <= 0) return FL_OK;
-    // worst case one fresh overflow leaf per point: guarantee the pool can take the batch
-    if ((long long)h_counters_[C_LEAF_USED] + n > v_.leaf_cap) {
-        min_pool_ = std::max(min_pool_, n + 1024);
-        FL_CHECK(rebuild());            // re-packs the leaves and re-sizes the pool
-    }
-    if (v_.dir.cap) {
-        // the insert kernels cope with a full table / an exhausted list pool (they flag it, the directory is re-listed below);
-        // re-list beforehand only when the table could get so full that probing degenerates
-        const size_t cells = (size_t)h_counters_[C_DIR_CELLS] + (size_t)n * 27;
-        if (cells * 10 > (size_t)v_.dir.cap * 9) {
-            dir_min_cap_ = std::max(dir_min_cap_, cells * 2 + 16384);
-            n_dir_rebuilds_++;
-            FL_CHECK(build_directory());
-        }
-    }
+    // the insert kernels cope with a full table / an exhausted list pool (they flag it, the directory is re-listed after them);
+    // beforehand, only room in the overflow pool and a table that probing does not degenerate in
+    FL_CHECK(grow_for_batch(n, false));
     FL_CHECK(ins_slots_.reserve(sizeof(int) * (size_t)n));
     k_insert<<<blocks_for((long long)n * 32, 256), 256, 0, stream_>>>(v_, d_pts, n, nullptr, counters_.as<int>(), ins_slots_.as<int>());
     if (v_.dir.cap) {
@@ -1965,16 +1975,7 @@ int Map::insert_device(const float4* d_pts, int n) {
     FL_CUDA(cudaStreamSynchronize(stream_));
     if (h_counters_[C_ERROR]) { set_last_error("insert: overflow pool exhausted"); return FL_ERR_CAPACITY; }
     n_valid_ += n;
-    // directory: out of room, or too many over-full cells (their queries walk the BVH) -> re-list the live slots
-    if (v_.dir.cap) {
-        const bool crowded = h_counters_[C_DIR_CROWDED] > std::max(64, h_counters_[C_DIR_CELLS] / 1024);
-        if (h_counters_[C_DIR_ERROR]) {
-            dir_min_cap_ = std::max(dir_min_cap_, (size_t)v_.dir.cap + (size_t)v_.dir.cap / 2);
-            dir_min_pool_ = std::max<size_t>(dir_min_pool_ * 2, (size_t)HALO_NEW_CAP * 262144);
-        }
-        if (h_counters_[C_DIR_ERROR] || crowded) { n_dir_rebuilds_++; FL_CHECK(build_directory()); }
-    }
-    return FL_OK;
+    return relist_if_due();
 }
 
 int Map::add_points_device(const float4* d_pts, int n, bool downsample_on, int* added) {
@@ -2056,15 +2057,9 @@ int Map::settle(bool full, int* layout_changed) {
         pending_ = false;
     }
     if (full && (due_ || refused_)) {
-        // what the host form would have done after its inserts (insert_device, maybe_rebuild), then room for a refused call
-        if (v_.dir.cap) {
-            const bool crowded = h_counters_[C_DIR_CROWDED] > std::max(64, h_counters_[C_DIR_CELLS] / 1024);
-            if (h_counters_[C_DIR_ERROR]) {
-                dir_min_cap_ = std::max(dir_min_cap_, (size_t)v_.dir.cap + (size_t)v_.dir.cap / 2);
-                dir_min_pool_ = std::max<size_t>(dir_min_pool_ * 2, (size_t)HALO_NEW_CAP * 262144);
-            }
-            if (h_counters_[C_DIR_ERROR] || crowded) { n_dir_rebuilds_++; FL_CHECK(build_directory()); }
-        }
+        // what the host form would have done after its inserts, by the rules the device forms marked it due by (relist_due and
+        // repack_due, map_rules.h), then room for a refused call
+        FL_CHECK(relist_if_due());
         FL_CHECK(maybe_rebuild());
         if (refused_) FL_CHECK(async_grow(async_n_max_, true));
         due_ = refused_ = false;
@@ -2081,32 +2076,16 @@ int Map::settle(bool full, int* layout_changed) {
 }
 
 // the host's bound: the call fits when the points of every device-form call since the last settle and n_max more could each take
-// one fresh leaf and claim 27 fresh cells with the table below 90 % load -- insert_device's two guards.  The list pool's need
-// has no useful bound on the host (up to 27 fresh lists per point); the plan kernel checks it on the device.
+// one fresh leaf and claim 27 fresh cells with the table below 90 % load -- insert_device's two guards (batch_fits).  The list
+// pool's need has no useful bound on the host (up to 27 fresh lists per point); the plan kernel checks it on the device.
 bool Map::async_fits(long long n_max) const {
-    const long long n = ub_n_ + n_max;
-    if (h_counters_[C_LEAF_USED] + n > v_.leaf_cap) return false;
-    return !v_.dir.cap || (h_counters_[C_DIR_CELLS] + 27 * n) * 10 <= (long long)v_.dir.cap * 9;
+    return batch_fits(h_counters_[C_LEAF_USED], v_.leaf_cap, h_counters_[C_DIR_CELLS], v_.dir.cap, ub_n_ + n_max);
 }
 
-// Room for one call of n_max points, by insert_device's rules (a re-pack with a larger overflow pool, a re-list with a larger
-// table); after a refused call (pool = true) also a re-list with a larger list pool when the need the plan last computed does
-// not fit it.  Synchronous; the map must be settled.
+// Room for one call of n_max points, by insert_device's rules; after a refused call (pool = true) also a larger list pool when
+// the need the plan last computed does not fit it.  Synchronous; the map must be settled.
 int Map::async_grow(int n_max, bool pool) {
-    const long long n = std::max(n_max, 1);
-    if (h_counters_[C_LEAF_USED] + n > v_.leaf_cap) {
-        min_pool_ = (int)std::min<long long>(std::max<long long>(min_pool_, n + 1024), INT_MAX / 2);
-        FL_CHECK(rebuild());
-    }
-    if (v_.dir.cap) {
-        const long long cells = (long long)h_counters_[C_DIR_CELLS] + 27 * n;
-        const bool grow_cap = cells * 10 > (long long)v_.dir.cap * 9;
-        const long long need = std::max<long long>(h_counters_[C_NEED], 0);
-        const bool grow_pool = pool && (long long)h_counters_[C_DIR_POOL] + need > v_.dir.lists_cap;
-        if (grow_cap) dir_min_cap_ = std::max(dir_min_cap_, (size_t)cells * 2 + 16384);
-        if (grow_pool) dir_min_pool_ = std::max<size_t>(dir_min_pool_ * 2, 2 * (size_t)need);
-        if (grow_cap || grow_pool) { n_dir_rebuilds_++; FL_CHECK(build_directory()); }
-    }
+    FL_CHECK(grow_for_batch(std::max(n_max, 1), pool));
     FL_CUDA(cudaStreamSynchronize(stream_));
     return publish_counts();
 }
@@ -2193,7 +2172,6 @@ int Map::enqueue_insert(const float4* pts, const int* n_dev, int n_max, cudaStre
 // add_points_host on the device: the batch's count at counters_[slot]
 int Map::enqueue_add(const float4* pts, int slot, bool downsample_on, int n_max, cudaStream_t st) {
     int* d_cnt = counters_.as<int>();
-    const int chain_limit = std::max(64, (int)(rebuild_overflow_frac_ * v_.n_main));
     if (downsample_on) {
         unsigned long long* ki = a_keys_in_.as<unsigned long long>();
         unsigned long long* ko = a_keys_out_.as<unsigned long long>();
@@ -2207,7 +2185,7 @@ int Map::enqueue_add(const float4* pts, int slot, bool downsample_on, int n_max,
     } else {
         FL_CHECK(enqueue_insert(pts, &d_cnt[slot], n_max, st));
     }
-    k_async_account<<<1, 1, 0, st>>>(v_, d_cnt, slot, downsample_on, chain_limit);
+    k_async_account<<<1, 1, 0, st>>>(v_, d_cnt, slot, downsample_on, chain_limit(rebuild_overflow_frac_, v_.n_main));
     FL_CUDA(cudaGetLastError());
     return FL_OK;
 }

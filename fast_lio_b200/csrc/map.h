@@ -138,6 +138,12 @@ private:
     int ensure_capacity(int n_points);
     int build_from_sorted(const float4* d_src, int n);
     int insert_device(const float4* d_pts, int n);
+    // The host form's maintenance by the rules of map_rules.h, on the host's mirror of the counters.  grow_for_batch: room for a
+    // batch of n points (a re-pack with a larger overflow pool, a re-list with a larger table; with list_pool, also a larger
+    // list pool when the need the plan last computed does not fit it).  relist_if_due: after inserts, a re-list of a full or
+    // crowded directory.  maybe_rebuild: a re-pack of chained or sparse leaves.
+    int grow_for_batch(long long n, bool list_pool);
+    int relist_if_due();
     int maybe_rebuild();
     int add_points_host(const float4* d_pts, int n, bool downsample_on, int* added);
     // the host's n_valid_ / n_tomb_ into the device counters the device forms keep (after every host-form mutation)
